@@ -7,10 +7,13 @@
 //
 // Mapping to the hardware
 //   * GEMM view: D[m][co] = sum_{tap} sum_{c} A[m + shift(tap)][c] * Wt[co][tap*C + c], M = flat padded
-//     pixels (common.h), so the A tile of one (tap, 64-channel block) is ONE TMA box {64 ch x 128 rows x P planes}
-//     at a shifted row coordinate; zero padding = TMA out-of-bounds fill + never-written gap rows.
-//   * One producer warp stages A and B tiles with TMA (cp.async.bulk.tensor.3d, SWIZZLE_128B) into a ring of
-//     shared-memory slots; completion and release on mbarriers.
+//     pixels (common.h), so the A tile of one (tap, 64-channel block) is 128 consecutive rows at a shifted row
+//     coordinate, and the k taps of one filter row read 128 + k - 1 consecutive rows: ONE TMA box {64 ch x 136 rows x
+//     P planes} per (filter row, 64-channel block), the "A window"; tap q reads rows [q, q + 128) of it.  Zero padding
+//     = TMA out-of-bounds fill + never-written gap rows.
+//   * A producer warpgroup (one thread) stages A windows and B tiles with TMA (cp.async.bulk.tensor.3d, SWIZZLE_128B)
+//     into two rings of shared-memory slots; completion and release on mbarriers.  It gives its registers to the
+//     consumers (setmaxnreg).
 //   * Two consumer warpgroups (64 rows each) issue wgmma.mma_async m64nBNk16 from shared-memory descriptors,
 //     accumulators in registers, fp32.
 //   * Split precision: activations and weights are stored as P 16-bit "planes" whose sum is the fp32 value
@@ -88,8 +91,12 @@ __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepc
 
 // wgmma shared-memory matrix descriptor, K-major, SWIZZLE_128B (PTX ISA "Matrix Descriptor Format"):
 //   [0,14) start address >> 4 | [16,30) LBO >> 4 (unused for swizzled K-major, 1) | [32,46) SBO >> 4
-//   (8 rows x 128 B = 1024 B -> 64) | [62,64) layout type = 1 (SWIZZLE_128B).  Tiles start on 1024-byte boundaries;
-//   the K=16 steps inside a 128-byte swizzle row advance the start address by 32 bytes.
+//   (8 rows x 128 B = 1024 B -> 64) | [62,64) layout type = 1 (SWIZZLE_128B).  TMA boxes start on 1024-byte
+//   boundaries; the K=16 steps inside a 128-byte swizzle row advance the start address by 32 bytes, and a tap's row
+//   shift inside an A window by 128 bytes per row.  The wgmma unit takes the swizzle's row phase from the address bits
+//   [7,10) of each row, as TMA does when it writes the box, so a start address q rows into a box needs no correction:
+//   the matrix base offset [49,52) stays 0 (on the H100, setting it to (start >> 7) & 7 shifts the pattern a second
+//   time and reads wrong data).
 __device__ __forceinline__ uint64_t wg_desc(uint32_t saddr) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3FFF);
@@ -191,30 +198,40 @@ __device__ __forceinline__ void range_publish(unsigned* range, float m) {
 // ------------------------------------------------------------------------------------------------
 constexpr int TC_BM = 128;           // rows per CTA tile: two consumer warpgroups x 64
 constexpr int TC_BK = 64;            // 16-bit elements per K block = one 128-byte swizzle row
-constexpr int TC_THREADS = 288;      // warps 0-7: two consumer warpgroups, warp 8: TMA producer
+constexpr int TC_WROWS = TC_BM + 8;  // rows of an A window: the tile plus the row shifts q = 1..8 of a filter row (k <= 9)
+constexpr int TC_KMAX = TC_WROWS - TC_BM + 1;
+constexpr int TC_THREADS = 384;      // warpgroup 0: TMA producer, warpgroups 1-2: consumers
+constexpr int TC_PRODUCER_REGS = 40, TC_CONSUMER_REGS = 232;   // setmaxnreg: 128 x 40 + 256 x 232 <= 65536
 constexpr int TC_SMEM_BUDGET = 220 * 1024;   // of the 227 KB a block may use on H100; the rest: alignment + static
 
+// Rows of the A window box: a 1x1 filter row is a single tap and reads only the tile's 128 rows.
+__host__ __device__ constexpr int tc_window_rows(int ksize) { return ksize == 1 ? TC_BM : TC_WROWS; }
+
 template <int BN, int PLANES> struct TcShape {
-    static constexpr int A_BYTES = TC_BM * 128;
-    static constexpr int B_BYTES = BN * 128;
-    static constexpr int STAGE_BYTES = PLANES * (A_BYTES + B_BYTES);
-    static constexpr int STAGES = TC_SMEM_BUDGET / STAGE_BYTES >= 6 ? 6 : TC_SMEM_BUDGET / STAGE_BYTES;
-    static constexpr int SMEM = STAGES * STAGE_BYTES + 1024;
+    static constexpr int A_BYTES = PLANES * TC_WROWS * 128;   // an A window slot: 17 KB per plane, a multiple of 1024 B
+    static constexpr int B_PLANE = BN * 128;
+    static constexpr int B_BYTES = PLANES * B_PLANE;
+    // a window serves k consecutive weight tiles, so the weight ring is the deeper one
+    static constexpr int W_STAGES = 3 * A_BYTES + 6 * B_BYTES <= TC_SMEM_BUDGET ? 3 : 2;
+    static constexpr int B_FIT = (TC_SMEM_BUDGET - W_STAGES * A_BYTES) / B_BYTES;
+    static constexpr int B_STAGES = B_FIT > 8 ? 8 : B_FIT;
+    static constexpr int SMEM = W_STAGES * A_BYTES + B_STAGES * B_BYTES + 1024;
 };
 
 template <int BN, int PLANES>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcArgs a) {
     using S = TcShape<BN, PLANES>;
-    constexpr int STAGES = S::STAGES;
+    constexpr int WS = S::W_STAGES, BS = S::B_STAGES;
     constexpr bool F16 = planes_are_fp16(PLANES);
     constexpr int NACC = BN / 2;   // fp32 registers per thread of one m64 x BN accumulator
-    static_assert(STAGES >= 2, "shared memory holds fewer than two stages");
+    static_assert(S::B_STAGES >= 2, "shared memory holds fewer than two weight tiles");
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);   // SWIZZLE_128B needs 1024 B
-    __shared__ __align__(8) uint64_t full_bar[STAGES];
-    __shared__ __align__(8) uint64_t empty_bar[STAGES];
+    uint8_t* const wring = smem;                          // A windows
+    uint8_t* const bring = smem + WS * S::A_BYTES;        // B tiles
+    __shared__ __align__(8) uint64_t wfull[WS], wempty[WS], bfull[BS], bempty[BS];
     __shared__ float s_bias[BN];
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -224,7 +241,8 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int num_k = taps * a.kblocks_per_tap;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
+        for (int s = 0; s < WS; s++) { mbar_init(&wfull[s], 1); mbar_init(&wempty[s], 8); }
+        for (int s = 0; s < BS; s++) { mbar_init(&bfull[s], 1); mbar_init(&bempty[s], 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
@@ -234,61 +252,78 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     pdl_launch_dependents();
     pdl_wait();
 
-    if (warp == 8) {
-        // ===== TMA producer: per K iteration one A box {64 ch, 128 rows, P planes} at the tap's row shift, one B box {64, BN, P} =====
-        if (lane == 0) {
-            for (int it = 0; it < num_k; it++) {
-                const int s = it % STAGES;
-                mbar_wait(&empty_bar[s], ((uint32_t)(it / STAGES) & 1u) ^ 1u);
-                mbar_expect_tx(&full_bar[s], S::STAGE_BYTES);
-                const int kb = it / taps, tap = it % taps;
-                const int r = tap / ks, q = tap % ks;
-                const int row0 = (int)(m0 + (long long)(r - a.pad) * a.Wp + (q - a.pad));
-                uint8_t* st = smem + (size_t)s * S::STAGE_BYTES;
-                tma_load_3d(st, &tmA, &full_bar[s], kb * TC_BK, row0, 0);
-                tma_load_3d(st + PLANES * S::A_BYTES, &tmB, &full_bar[s], tap * a.cin_k + kb * TC_BK, n0, 0);
-            }
+    if (warp < 4) {
+        // ===== TMA producer: per (64-channel block, filter row) one A window {64 ch, 136 rows, P planes}, then per tap
+        // of the row one B box {64, BN, P}; K order = channel block, filter row, tap (the order of the weight K index) =====
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(TC_PRODUCER_REGS));
+        if (threadIdx.x == 0) {
+            const uint32_t a_tx = PLANES * tc_window_rows(ks) * 128;
+            int wc = 0, bc = 0;   // windows / weight tiles issued
+            for (int kb = 0; kb < a.kblocks_per_tap; kb++)
+                for (int r = 0; r < ks; r++, wc++) {
+                    const int w = wc % WS;
+                    mbar_wait(&wempty[w], ((uint32_t)(wc / WS) & 1u) ^ 1u);
+                    mbar_expect_tx(&wfull[w], a_tx);
+                    const int row0 = (int)(m0 + (long long)(r - a.pad) * a.Wp - a.pad);
+                    tma_load_3d(wring + (size_t)w * S::A_BYTES, &tmA, &wfull[w], kb * TC_BK, row0, 0);
+                    for (int q = 0; q < ks; q++, bc++) {
+                        const int b = bc % BS;
+                        mbar_wait(&bempty[b], ((uint32_t)(bc / BS) & 1u) ^ 1u);
+                        mbar_expect_tx(&bfull[b], S::B_BYTES);
+                        tma_load_3d(bring + (size_t)b * S::B_BYTES, &tmB, &bfull[b], (r * ks + q) * a.cin_k + kb * TC_BK, n0, 0);
+                    }
+                }
         }
         return;
     }
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(TC_CONSUMER_REGS));
 
     // ===== consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile =====
-    const int wg = warp >> 2;
+    const int wg = (warp >> 2) - 1;
     float acc_h[NACC], sum_h[NACC], acc_c[NACC];
 #pragma unroll
     for (int j = 0; j < NACC; j++) { acc_h[j] = 0.f; sum_h[j] = 0.f; acc_c[j] = 0.f; }
     const int cs = a.chunk_iters;
-    for (int it = 0; it < num_k; it++) {
-        const int s = it % STAGES;
-        mbar_wait(&full_bar[s], (uint32_t)(it / STAGES) & 1u);
-        const uint32_t sa = smem_u32(smem + (size_t)s * S::STAGE_BYTES) + (uint32_t)(wg * 64 * 128);
-        const uint32_t sb = smem_u32(smem + (size_t)s * S::STAGE_BYTES) + (uint32_t)(PLANES * S::A_BYTES);
-        const uint32_t h_acc = (it % cs) != 0;   // 0: hi*hi chunk starts from zero
-        wg_fence();
+    const uint32_t a_plane = tc_window_rows(ks) * 128;   // plane stride of the window as the TMA box lays it out
+    int it = 0, wc = 0;
+    for (int kb = 0; kb < a.kblocks_per_tap; kb++)
+        for (int r = 0; r < ks; r++, wc++) {
+            const int w = wc % WS;
+            mbar_wait(&wfull[w], (uint32_t)(wc / WS) & 1u);
+            const uint32_t wa = smem_u32(wring + (size_t)w * S::A_BYTES) + (uint32_t)(wg * 64 * 128);
+            for (int q = 0; q < ks; q++, it++) {
+                const int b = it % BS;
+                mbar_wait(&bfull[b], (uint32_t)(it / BS) & 1u);
+                const uint32_t sa = wa + (uint32_t)(q * 128);   // tap q: window rows [q + 64 wg, q + 64 wg + 64)
+                const uint32_t sb = smem_u32(bring + (size_t)b * S::B_BYTES);
+                const uint32_t h_acc = (it % cs) != 0;   // 0: hi*hi chunk starts from zero
+                wg_fence();
 #pragma unroll
-        for (int k = 0; k < TC_BK / 16; k++) {
-            Wgmma<BN>::template mma<F16>(acc_h, wg_desc(sa + k * 32), wg_desc(sb + k * 32), (k != 0) | h_acc);
-            if constexpr (PLANES > 1) {
+                for (int k = 0; k < TC_BK / 16; k++) {
+                    Wgmma<BN>::template mma<F16>(acc_h, wg_desc(sa + k * 32), wg_desc(sb + k * 32), (k != 0) | h_acc);
+                    if constexpr (PLANES > 1) {
 #pragma unroll
-                for (int pa = 0; pa < PLANES; pa++)
+                        for (int pa = 0; pa < PLANES; pa++)
 #pragma unroll
-                    for (int pb = 0; pb < PLANES - pa; pb++) {
-                        if (pa + pb == 0) continue;
-                        const uint32_t first = it == 0 && k == 0 && pa + pb == 1 && pa == 0;
-                        Wgmma<BN>::template mma<F16>(acc_c, wg_desc(sa + pa * S::A_BYTES + k * 32), wg_desc(sb + pb * S::B_BYTES + k * 32),
-                                                     first ? 0u : 1u);
+                            for (int pb = 0; pb < PLANES - pa; pb++) {
+                                if (pa + pb == 0) continue;
+                                const uint32_t first = it == 0 && k == 0 && pa + pb == 1 && pa == 0;
+                                Wgmma<BN>::template mma<F16>(acc_c, wg_desc(sa + pa * a_plane + k * 32),
+                                                             wg_desc(sb + pb * S::B_PLANE + k * 32), first ? 0u : 1u);
+                            }
                     }
-            }
-        }
-        wg_commit();
-        wg_wait_all();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[s]);   // this warp's share of the slot has been read
-        if ((it + 1) % cs == 0 || it + 1 == num_k) {
+                }
+                wg_commit();
+                wg_wait_all();
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&bempty[b]);   // this warp's share of the weight tile has been read
+                if ((it + 1) % cs == 0 || it + 1 == num_k) {
 #pragma unroll
-            for (int j = 0; j < NACC; j++) sum_h[j] = __fadd_rn(sum_h[j], acc_h[j]);
+                    for (int j = 0; j < NACC; j++) sum_h[j] = __fadd_rn(sum_h[j], acc_h[j]);
+                }
+            }
+            if (lane == 0) mbar_arrive(&wempty[w]);   // ... and of the window, after its last tap
         }
-    }
 
     // ===== epilogue: sum, bias, ReLU, re-split into planes, store =====
     const int per_img = a.Hs * a.Wp;
@@ -358,9 +393,10 @@ int tc_cout_pad(int cout) {
     if (cout > 16) return 32;
     return 16;
 }
-// Tile width: 128 output channels with one plane; with 2 or 3 planes the hi*hi chunk, its running sum and the cross-term
-// accumulator live in registers side by side, and 3 x 64 of them per thread (BN = 128) would leave no room: 64.
-static int tc_bn(int cout_pad, int planes) { return std::min(cout_pad, planes == 1 ? 128 : 64); }
+// Tile width: 128 output channels.  With 2 or 3 planes the hi*hi chunk, its running sum and the cross-term accumulator
+// live in registers side by side: 3 x 64 per consumer thread at BN = 128, which fits in the consumers' 232 registers.
+// Three planes (bf16x3, kept for A/B comparisons) stay at 64.
+static int tc_bn(int cout_pad, int planes) { return std::min(cout_pad, planes == 3 ? 64 : 128); }
 
 static int env_int(const char* name, int dflt) {
     const char* v = getenv(name);
@@ -393,7 +429,7 @@ template <int BN>
 static int launch_bn(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap) {
     switch (l.d.planes) {
         case 1: return launch_inst<BN, 1>(l, a, grid, st, bmap);
-        case 2: if constexpr (BN <= 64) return launch_inst<BN, 2>(l, a, grid, st, bmap); else break;
+        case 2: return launch_inst<BN, 2>(l, a, grid, st, bmap);
         default: if constexpr (BN <= 64) return launch_inst<BN, 3>(l, a, grid, st, bmap); else break;
     }
     return -1;   // no kernel for this tile width and plane count (tc_bn never picks one)
@@ -414,6 +450,7 @@ int tc_layer_create(const TcLayerDesc& d, TcLayer& out, std::string& err) {
     if (!enc) { err = "cuTensorMapEncodeTiled unavailable"; return -1; }
     if (d.in_cused % TC_BK) { err = "input channels not a multiple of 64"; return -1; }
     if (d.planes < 1 || d.planes > 3) { err = "1 to 3 planes"; return -1; }
+    if (d.ksize < 1 || d.ksize > TC_KMAX) { err = "filter size above " + std::to_string(TC_KMAX) + " (A window rows)"; return -1; }
     out.d = d;
     out.bn = tc_bn(d.cout_pad, d.planes);
     CUtensorMap* maps = nullptr;
@@ -421,8 +458,9 @@ int tc_layer_create(const TcLayerDesc& d, TcLayer& out, std::string& err) {
     memset(maps, 0, 3 * sizeof(CUtensorMap));
     const cuuint64_t K = (cuuint64_t)d.ksize * d.ksize * d.in_cused;
     const cuuint64_t P = (cuuint64_t)d.planes;
-    // A: [planes][M][pitch], box {64, 128, planes}
-    int r = encode(enc, &maps[0], d.in, d.in_cused, d.geo.M, P, (cuuint64_t)d.in_pitch * 2, (cuuint64_t)d.in_plane * 2, TC_BM, d.planes,
+    // A: [planes][M][pitch], box {64, window rows, planes}
+    int r = encode(enc, &maps[0], d.in, d.in_cused, d.geo.M, P, (cuuint64_t)d.in_pitch * 2, (cuuint64_t)d.in_plane * 2,
+                   tc_window_rows(d.ksize), d.planes,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
     // B: [planes][cout_pad][K], box {64, bn, planes}; and half as wide for small problems (more CTAs, see tc_layer_launch)
     if (!r) r = encode(enc, &maps[1], d.w, K, d.cout_pad, P, K * 2, K * 2 * d.cout_pad, out.bn, d.planes, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
