@@ -58,7 +58,9 @@ struct PoolSpec { std::string name; int in_act, out_act, level_in; };
 struct CopySpec { int src_act, dst_act, channels; };  // duplicate F into the second concat buffer
 struct ActSpec { int level, C; std::string blob; int blob_c; };  // blob: prototxt top living at channel 0
 struct OpRef { int type, idx; };                      // 0 conv, 1 pool, 2 copy
-struct BlobRef { std::string name; int act, coff, c; };
+// A fetchable blob: where it lives, which conv produced it (its stored values carry that conv's range scale; -1: the net
+// input), and the first later op of the forward that overwrites its channels (empty: none; the ping-pong concat buffers).
+struct BlobRef { std::string name; int act, coff, c; int prod = -1, pos = -1; std::string reused_by; };
 
 struct NetPlan {
     int model = 0, c_l1 = 0, c_l2 = 0, kp_input = 0;

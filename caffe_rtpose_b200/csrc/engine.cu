@@ -1410,6 +1410,8 @@ extern "C" int pe_fetch_blob(pe_engine* e, const char* blob_name, float* out, si
     const int nimg = std::max(e->last_n, 1) * e->cfg.num_scales;
     for (const BlobRef& b : e->plan.blobs) {
         if (b.name != blob_name) continue;
+        if (!b.reused_by.empty())
+            return fail(e, PE_ERR_STATE, "blob %s is not kept: %s, later in every forward, reuses its buffer", blob_name, b.reused_by.c_str());
         Geo g = e->geo[e->plan.acts[b.act].level];
         g.N = nimg;
         const size_t cnt = (size_t)nimg * b.c * g.H * g.W;
@@ -1426,7 +1428,10 @@ extern "C" int pe_fetch_blob(pe_engine* e, const char* blob_name, float* out, si
         }
         float* d = nullptr;
         CK(e, cudaMalloc(&d, cnt * sizeof(float)));
-        e->launches += launch_act_to_nchw(e->acts[b.act], e->plan.acts[b.act].C, b.coff, b.c, e->act_plane[b.act], e->planes, g, d, e->stream);
+        // stored value = true value * conv_scale[producer] (pools pass their producer's scale through; the net input has none)
+        const float inv = (b.prod >= 0 && b.prod < (int)e->conv_scale.size()) ? 1.f / e->conv_scale[b.prod] : 1.f;
+        e->launches += launch_act_to_nchw(e->acts[b.act], e->plan.acts[b.act].C, b.coff, b.c, e->act_plane[b.act], e->planes, g, inv, d,
+                                          e->stream);
         CK(e, cudaMemcpyAsync(out, d, cnt * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
         CK(e, cudaStreamSynchronize(e->stream));
         cudaFree(d);

@@ -113,8 +113,9 @@ struct PoolArgs {
 int launch_pool(const PoolArgs& a, cudaStream_t st);
 struct CopyArgs { const void* src; void* dst; int pitch, channels, elem_bytes; long long M, plane; int planes; };
 int launch_copy_channels(const CopyArgs& a, cudaStream_t st);
-// activation (flat padded, fp32 or bf16 planes) -> NCHW fp32 (debug / pe_fetch_blob)
-int launch_act_to_nchw(const void* act, int pitch, int coff, int c, long long plane, int planes, const Geo& g,
+// activation (flat padded, fp32 or bf16 planes) -> NCHW fp32 (debug / pe_fetch_blob); scale: the inverse of the power-of-two
+// range scale the stored values carry (engine.cu, fill_epilogue_fields), so that out holds true values
+int launch_act_to_nchw(const void* act, int pitch, int coff, int c, long long plane, int planes, const Geo& g, float scale,
                        float* out, cudaStream_t st);
 
 }  // namespace pe

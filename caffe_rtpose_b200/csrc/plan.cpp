@@ -257,7 +257,7 @@ int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, s
                 const int j = concat_slot[top].first, k = concat_slot[top].second;
                 const Slot& sdef = slots[j][k];
                 c.out_act = cc[j % nbuf]; c.out_coff = sdef.eng_off;
-                p.blobs.push_back({top, c.out_act, sdef.eng_off, sdef.c});
+                p.blobs.push_back({top, c.out_act, sdef.eng_off, sdef.c, (int)p.convs.size(), (int)p.order.size()});
                 if (sdef.shared || consumers[top].size() > 1) {   // also read directly by convolutions (conv4_4_CPM feeds stage 1)
                     if (sdef.eng_off != 0) return fail("blob " + top + ": a directly consumed Concat bottom must be first in the buffer");
                     Loc o; o.act = c.out_act; o.coff = 0; o.cused = round_up(sdef.c, 64); o.cmap = ident(sdef.c, o.cused);
@@ -268,6 +268,7 @@ int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, s
                 }
             } else {
                 c.out_act = new_act(c.level, c.cout, top, c.cout);
+                p.blobs.back().prod = (int)p.convs.size(); p.blobs.back().pos = (int)p.order.size();
                 Loc o; o.act = c.out_act; o.coff = 0; o.cused = p.acts[c.out_act].C; o.cmap = ident(c.cout, o.cused);
                 o.prod.assign(o.cused, -1);
                 for (int q = 0; q < c.cout; q++) o.prod[q] = (int)p.convs.size();
@@ -284,6 +285,7 @@ int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, s
             const Loc& in = loc[l.bottoms[0]];
             if (in.act < 0 || in.coff != 0 || p.acts[in.act].level != level[l.bottoms[0]]) return fail("layer " + l.name + ": unsupported pooling input");
             const int out = new_act(level[top], channels[top], top, channels[top]);
+            p.blobs.back().prod = in.prod.empty() ? -1 : in.prod[0]; p.blobs.back().pos = (int)p.order.size();
             if (p.acts[out].C != p.acts[in.act].C) return fail("layer " + l.name + ": channel pitch mismatch");
             p.pools.push_back({l.name, in.act, out, level[l.bottoms[0]]});
             p.order.push_back({1, (int)p.pools.size() - 1});
@@ -305,6 +307,23 @@ int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, s
         }
     }
     if (p.convs.empty() || !p.convs[0].im2col_input) return fail("the first layer must be a convolution on the net input");
+    // Every forward runs the whole order, so a blob whose channels a later op writes (a stage output in a ping-pong concat
+    // buffer that a later stage reuses) holds that op's data after the forward: record the first such op.
+    for (BlobRef& b : p.blobs)
+        for (int k = b.pos + 1; k < (int)p.order.size() && b.reused_by.empty(); k++) {
+            const OpRef& op = p.order[k];
+            int act = -1, c0 = 0, c1 = 0;
+            std::string who;
+            if (op.type == 0) {
+                const ConvSpec& c = p.convs[op.idx];
+                act = c.out_act; c0 = c.out_coff; c1 = c.out_coff + round_up(c.cout, 8); who = c.name;   // epilogues store 8-channel groups
+            } else if (op.type == 1) {
+                act = p.pools[op.idx].out_act; c1 = p.acts[act].C; who = p.pools[op.idx].name;
+            } else {
+                act = p.copies[op.idx].dst_act; c1 = p.copies[op.idx].channels; who = "the copy of the shared concat input";
+            }
+            if (act == b.act && c0 < b.coff + b.c && b.coff < c1) b.reused_by = who;
+        }
     return 0;
 }
 

@@ -120,7 +120,7 @@ int launch_copy_channels(const CopyArgs& a, cudaStream_t st) {
 }
 
 __global__ void __launch_bounds__(256) act_to_nchw_kernel(const void* act, int pitch, int coff, int c, long long plane,
-                                                          int planes, Geo g, float* out) {
+                                                          int planes, Geo g, float scale, float* out) {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const long long total = (long long)g.N * c * g.H * g.W;
     if (idx >= total) return;
@@ -135,12 +135,12 @@ __global__ void __launch_bounds__(256) act_to_nchw_kernel(const void* act, int p
         const uint16_t h = ((const uint16_t*)act)[p * plane + m * pitch + coff + ch];
         v += planes_are_fp16(planes) ? plane_to_float<true>(h) : plane_to_float<false>(h);
     }
-    out[idx] = v;
+    out[idx] = v * scale;   // a power of two: exact
 }
-int launch_act_to_nchw(const void* act, int pitch, int coff, int c, long long plane, int planes, const Geo& g,
+int launch_act_to_nchw(const void* act, int pitch, int coff, int c, long long plane, int planes, const Geo& g, float scale,
                        float* out, cudaStream_t st) {
     const long long total = (long long)g.N * c * g.H * g.W;
-    act_to_nchw_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(act, pitch, coff, c, plane, planes, g, out);
+    act_to_nchw_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(act, pitch, coff, c, plane, planes, g, scale, out);
     return 1;
 }
 

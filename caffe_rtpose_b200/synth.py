@@ -64,14 +64,20 @@ def conv_table(model, stages=6):
     return t
 
 
-def make_weights(model, kind="he", seed=1234, stages=6):
-    """dict name -> (w float32 [cout,cin,k,k], b float32 [cout])."""
+def make_weights(model, kind="he", seed=1234, stages=6, bias_std=0.0):
+    """dict name -> (w float32 [cout,cin,k,k], b float32 [cout]).
+
+    bias_std: 0 keeps the fillers' zero biases; a number gives every layer N(0, bias_std^2) biases, a dict name -> std one std
+    per layer.  The biases come from their own generator (seed + 1), so the weights do not depend on bias_std."""
     rng = np.random.default_rng(seed)
+    brng = np.random.default_rng(seed + 1)
     out = {}
     for name, co, ci, k in conv_table(model, stages):
         std = 0.01 if kind == "caffe" else float(np.sqrt(2.0 / (ci * k * k)))
         w = (rng.standard_normal((co, ci, k, k), dtype=np.float32) * np.float32(std)).astype(np.float32)
-        out[name] = (w, np.zeros(co, np.float32))
+        bstd = float(bias_std.get(name, 0.0)) if isinstance(bias_std, dict) else float(bias_std)
+        b = (brng.standard_normal(co, dtype=np.float32) * np.float32(bstd)).astype(np.float32) if bstd else np.zeros(co, np.float32)
+        out[name] = (w, b)
     return out
 
 

@@ -147,7 +147,10 @@ int pe_forward_maps(pe_engine* e, const float* maps8, int n);
 int pe_fetch(pe_engine* e, int idx, float* joints, int* num_people, float* peaks);
 /* stride-8 net output of the last forward, n x num_scales x C x net_h/8 x net_w/8 (blob "concat_stage7") */
 int pe_fetch_maps(pe_engine* e, float* maps8, int n);
-/* debugging / layer-wise parity: NCHW fp32 copy of an intermediate blob by its prototxt top name */
+/* debugging / layer-wise parity: NCHW fp32 copy of an intermediate blob by its prototxt top name, in true values (the range
+ * scale of pe_calibrate is divided out).  The stage outputs of the concat buffers that a later stage reuses (for the 6-stage
+ * nets: conv5_5_CPM_L1/_L2, Mconv7_stage2_* and Mconv7_stage3_*) are overwritten by every forward: PE_ERR_STATE, and
+ * pe_last_error names the layer that reuses the buffer. */
 int pe_fetch_blob(pe_engine* e, const char* blob_name, float* out, size_t cap, int* c, int* h, int* w);
 /* block until the engine's stream is idle */
 int pe_sync(pe_engine* e);
