@@ -13,7 +13,9 @@
 //     = TMA out-of-bounds fill + never-written gap rows.
 //   * A producer warpgroup (one thread) stages A windows and B tiles with TMA (cp.async.bulk.tensor.3d, SWIZZLE_128B)
 //     into two rings of shared-memory slots; completion and release on mbarriers.  It gives its registers to the
-//     consumers (setmaxnreg).
+//     consumers (setmaxnreg).  Row tiles start at every image (blockIdx.x = image, tile), and TC_CLUSTER consecutive
+//     row tiles form a thread block cluster: each CTA loads 1/TC_CLUSTER of every weight tile and multicasts it to all,
+//     and a slot of the weight ring is refilled once the consumers of every CTA in the cluster have released it.
 //   * Two consumer warpgroups (64 rows each) issue wgmma.mma_async m64nBNk16 from shared-memory descriptors,
 //     accumulators in registers, fp32.
 //   * Split precision: activations and weights are stored as P 16-bit "planes" whose sum is the fp32 value
@@ -47,6 +49,7 @@ struct TcArgs {
     int ksize, pad, kblocks_per_tap, cin_k;   // cin_k = channels per tap in the weight K ordering
     int W, H, Wp, Hs;
     long long M;
+    int tiles_img;                            // row tiles per image: blockIdx.x = image * tiles_img + tile
     int chunk_iters;                          // K iterations (64 channels of one tap each) per hi*hi accumulation chunk
     unsigned* range;                          // [0]: running max |stored value| of this layer as float bits (atomicMax; values are >= 0), or null
 };
@@ -80,6 +83,34 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
     asm volatile(
         "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
         ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
+// The same box written to the same shared-memory offset of every CTA in `mask`, each CTA's mbarrier at `bar`'s offset
+// receiving the bytes.
+__device__ __forceinline__ void tma_load_3d_mc(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, uint16_t mask) {
+    asm volatile(
+        "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5}], [%2], %6;"
+        ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "h"(mask) : "memory");
+}
+
+// Thread block clusters: rank within the cluster, a cluster-wide barrier of all threads, and an arrive on the mbarrier at
+// `bar`'s offset in the shared memory of cluster CTA `rank`.  The arrive keeps the default .release.cta: it only has to
+// follow the reads of the arriving warp's wgmma, which wgmma.wait_group has completed.  A .release.cluster arrive on the
+// consumers' path made the conv stack 16 % slower than the kernel without clusters (H100 80GB HBM3, 400 W limit).
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+    asm volatile(
+        "{\n\t"
+        ".reg .b32 ra;\n\t"
+        "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+        "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t"
+        "}" ::"r"(smem_u32(bar)), "r"(rank) : "memory");
 }
 
 // Programmatic dependent launch (PDL): a conv kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may
@@ -204,8 +235,18 @@ constexpr int TC_THREADS = 384;      // warpgroup 0: TMA producer, warpgroups 1-
 constexpr int TC_PRODUCER_REGS = 40, TC_CONSUMER_REGS = 232;   // setmaxnreg: 128 x 40 + 256 x 232 <= 65536
 constexpr int TC_SMEM_BUDGET = 220 * 1024;   // of the 227 KB a block may use on H100; the rest: alignment + static
 
+// CTAs along M that share every weight tile: each loads 1/TC_CLUSTER of the tile from L2 and multicasts it to all of them,
+// so the L2 -> shared-memory traffic of the weights, most of the kernel's, drops by this factor.  A windows stay per CTA.
+constexpr int TC_CLUSTER = 2;
+
 // Rows of the A window box: a 1x1 filter row is a single tap and reads only the tile's 128 rows.
 __host__ __device__ constexpr int tc_window_rows(int ksize) { return ksize == 1 ? TC_BM : TC_WROWS; }
+
+// Rows of the weight box {64, rows, 1 plane}.  A CTA's share of a tile is P*BN/TC_CLUSTER of its P*BN rows (planes stacked),
+// loaded in boxes that divide both that share and a plane, so none crosses a plane; a multiple of 8 rows keeps every box on
+// a 1024-byte swizzle atom.
+__host__ __device__ constexpr int tc_gcd(int a, int b) { return b ? tc_gcd(b, a % b) : a; }
+__host__ __device__ constexpr int tc_wbox_rows(int bn, int planes) { return tc_gcd(planes * bn / TC_CLUSTER, bn); }
 
 template <int BN, int PLANES> struct TcShape {
     static constexpr int A_BYTES = PLANES * TC_WROWS * 128;   // an A window slot: 17 KB per plane, a multiple of 1024 B
@@ -226,38 +267,46 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     constexpr bool F16 = planes_are_fp16(PLANES);
     constexpr int NACC = BN / 2;   // fp32 registers per thread of one m64 x BN accumulator
     static_assert(S::B_STAGES >= 2, "shared memory holds fewer than two weight tiles");
+    constexpr int WBOX = tc_wbox_rows(BN, PLANES), WSHARE = PLANES * BN / TC_CLUSTER;
+    static_assert(WSHARE * TC_CLUSTER == PLANES * BN && WBOX % 8 == 0, "weight tile does not split into whole swizzle atoms");
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);   // SWIZZLE_128B needs 1024 B
     uint8_t* const wring = smem;                          // A windows
-    uint8_t* const bring = smem + WS * S::A_BYTES;        // B tiles
+    uint8_t* const bring = smem + WS * S::A_BYTES;        // B tiles, written by the TMA multicasts of the whole cluster
     __shared__ __align__(8) uint64_t wfull[WS], wempty[WS], bfull[BS], bempty[BS];
     __shared__ float s_bias[BN];
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const long long m0 = (long long)blockIdx.x * TC_BM;
+    // Row tiles start at every image, so none covers only the gap rows after an image's last pixel.  A CTA past the last
+    // image (grid.x is rounded up to whole clusters) runs the load / consume protocol with its cluster and stores nothing.
+    const int img = blockIdx.x / a.tiles_img;
+    const long long m0 = (long long)img * a.Hs * a.Wp + (long long)(blockIdx.x % a.tiles_img) * TC_BM;
     const int n0 = blockIdx.y * BN;
     const int ks = a.ksize, taps = ks * ks;
     const int num_k = taps * a.kblocks_per_tap;
 
     if (threadIdx.x == 0) {
+        // bempty: released by the 8 consumer warps of every CTA in the cluster, since each weight tile is written into all
         for (int s = 0; s < WS; s++) { mbar_init(&wfull[s], 1); mbar_init(&wempty[s], 8); }
-        for (int s = 0; s < BS; s++) { mbar_init(&bfull[s], 1); mbar_init(&bempty[s], 8); }
+        for (int s = 0; s < BS; s++) { mbar_init(&bfull[s], 1); mbar_init(&bempty[s], 8 * TC_CLUSTER); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
     }
     for (int i = threadIdx.x; i < BN; i += TC_THREADS) s_bias[i] = (n0 + i < a.cout) ? a.bias[n0 + i] : 0.f;
-    __syncthreads();
+    cluster_sync();   // every CTA's barriers are initialised before any multicast or remote arrive reaches them
     pdl_launch_dependents();
     pdl_wait();
 
     if (warp < 4) {
         // ===== TMA producer: per (64-channel block, filter row) one A window {64 ch, 136 rows, P planes}, then per tap
-        // of the row one B box {64, BN, P}; K order = channel block, filter row, tap (the order of the weight K index) =====
+        // of the row this CTA's share of the B tile {64, BN, P}, multicast to the cluster; K order = channel block,
+        // filter row, tap (the order of the weight K index) =====
         asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(TC_PRODUCER_REGS));
         if (threadIdx.x == 0) {
             const uint32_t a_tx = PLANES * tc_window_rows(ks) * 128;
+            const int f0 = (int)cluster_ctarank() * WSHARE;   // first row of this CTA's share in the stacked planes
             int wc = 0, bc = 0;   // windows / weight tiles issued
             for (int kb = 0; kb < a.kblocks_per_tap; kb++)
                 for (int r = 0; r < ks; r++, wc++) {
@@ -268,11 +317,16 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                     tma_load_3d(wring + (size_t)w * S::A_BYTES, &tmA, &wfull[w], kb * TC_BK, row0, 0);
                     for (int q = 0; q < ks; q++, bc++) {
                         const int b = bc % BS;
-                        mbar_wait(&bempty[b], ((uint32_t)(bc / BS) & 1u) ^ 1u);
-                        mbar_expect_tx(&bfull[b], S::B_BYTES);
-                        tma_load_3d(bring + (size_t)b * S::B_BYTES, &tmB, &bfull[b], (r * ks + q) * a.cin_k + kb * TC_BK, n0, 0);
+                        mbar_wait(&bempty[b], ((uint32_t)(bc / BS) & 1u) ^ 1u);   // free in every CTA of the cluster
+                        mbar_expect_tx(&bfull[b], S::B_BYTES);                    // the whole tile, from all the CTAs
+#pragma unroll
+                        for (int f = f0; f < f0 + WSHARE; f += WBOX)
+                            tma_load_3d_mc(bring + (size_t)b * S::B_BYTES + (size_t)f * 128, &tmB, &bfull[b],
+                                           (r * ks + q) * a.cin_k + kb * TC_BK, n0 + f % BN, f / BN, (uint16_t)((1u << TC_CLUSTER) - 1));
                     }
                 }
+            // The partners' consumers arrive on this CTA's bempty: stay until the last use of every slot is released.
+            for (int i = 0; i < BS; i++, bc++) mbar_wait(&bempty[bc % BS], ((uint32_t)(bc / BS) & 1u) ^ 1u);
         }
         return;
     }
@@ -316,7 +370,7 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                 wg_commit();
                 wg_wait_all();
                 __syncwarp();
-                if (lane == 0) mbar_arrive(&bempty[b]);   // this warp's share of the weight tile has been read
+                if (lane < TC_CLUSTER) mbar_arrive_cluster(&bempty[b], lane);   // this warp has read the weight tile: tell every producer
                 if ((it + 1) % cs == 0 || it + 1 == num_k) {
 #pragma unroll
                     for (int j = 0; j < NACC; j++) sum_h[j] = __fadd_rn(sum_h[j], acc_h[j]);
@@ -333,15 +387,10 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
     for (int hr = 0; hr < 2; hr++) {
         const long long m = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + hr * 8;
-        bool valid = m < a.M;
-        int n = 0, y = 0, x = 0;
-        if (valid) {
-            n = (int)(m / per_img);
-            const int rem = (int)(m % per_img);
-            y = rem / a.Wp; x = rem % a.Wp;
-            valid = (x < a.W) && (y < a.H);
-        }
-        if (!valid) continue;   // gap rows are never written and stay zero
+        const int n = (int)(m / per_img), rem = (int)(m % per_img);
+        const int y = rem / a.Wp, x = rem % a.Wp;
+        // gap rows are never written and stay zero; the rows of the next image belong to its own tiles
+        if (m >= a.M || n != img || x >= a.W || y >= a.H) continue;
 #pragma unroll
         for (int g = 0; g < BN / 8; g++) {
             const int c = g * 8 + (lane & 3) * 2, j = g * 4 + hr * 2;
@@ -417,10 +466,13 @@ static int launch_inst(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_
     // PDL (see pdl_wait): back-to-back conv kernels overlap the next one's prologue with the previous one's tail
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = grid; cfg.blockDim = dim3(TC_THREADS, 1, 1); cfg.dynamicSmemBytes = (size_t)smem; cfg.stream = st;
-    cudaLaunchAttribute at[1];
+    cudaLaunchAttribute at[2];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
+    // clusters of TC_CLUSTER row tiles share the weight tiles (see conv_wg_kernel); grid.x is a multiple of TC_CLUSTER
+    at[1].id = cudaLaunchAttributeClusterDimension;
+    at[1].val.clusterDim.x = TC_CLUSTER; at[1].val.clusterDim.y = 1; at[1].val.clusterDim.z = 1;
+    cfg.attrs = at; cfg.numAttrs = 2;
     const CUtensorMap* maps = (const CUtensorMap*)l.maps;
     return cudaLaunchKernelEx(&cfg, kern, maps[0], maps[bmap], a) == cudaSuccess ? 1 : -1;
 }
@@ -462,9 +514,12 @@ int tc_layer_create(const TcLayerDesc& d, TcLayer& out, std::string& err) {
     int r = encode(enc, &maps[0], d.in, d.in_cused, d.geo.M, P, (cuuint64_t)d.in_pitch * 2, (cuuint64_t)d.in_plane * 2,
                    tc_window_rows(d.ksize), d.planes,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
-    // B: [planes][cout_pad][K], box {64, bn, planes}; and half as wide for small problems (more CTAs, see tc_layer_launch)
-    if (!r) r = encode(enc, &maps[1], d.w, K, d.cout_pad, P, K * 2, K * 2 * d.cout_pad, out.bn, d.planes, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
-    if (!r && out.bn >= 64) r = encode(enc, &maps[2], d.w, K, d.cout_pad, P, K * 2, K * 2 * d.cout_pad, out.bn / 2, d.planes, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+    // B: [planes][cout_pad][K], box {64, part of a plane, 1} (a CTA's share of a {64, bn, planes} tile is one or more such
+    // boxes, tc_wbox_rows); and for half-width tiles (more CTAs for small problems, see tc_layer_launch)
+    if (!r) r = encode(enc, &maps[1], d.w, K, d.cout_pad, P, K * 2, K * 2 * d.cout_pad, tc_wbox_rows(out.bn, d.planes), 1,
+                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+    if (!r && out.bn >= 64) r = encode(enc, &maps[2], d.w, K, d.cout_pad, P, K * 2, K * 2 * d.cout_pad, tc_wbox_rows(out.bn / 2, d.planes), 1,
+                                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
     if (r) { err = "cuTensorMapEncodeTiled failed: " + std::to_string(r); free(maps); return -1; }
     out.maps = maps;
     return 0;
@@ -502,7 +557,10 @@ int tc_layer_launch(const TcLayer& l, int nimg, cudaStream_t st, int share) {
         const double shalf = (double)std::min<long long>(mt * (d.cout_pad / (l.bn / 2)), sms) * 0.80;
         if (shalf > sfull) { bn = l.bn / 2; bmap = 2; }
     }
-    const dim3 grid((unsigned)mt, (unsigned)(d.cout_pad / bn), 1);
+    // row tiles per image: up to its last pixel (H - 1) * Wp + W - 1; the grid in whole clusters
+    a.tiles_img = ((d.geo.H - 1) * d.geo.Wp + d.geo.W + TC_BM - 1) / TC_BM;
+    const long long tiles = ((long long)nimg * a.tiles_img + TC_CLUSTER - 1) / TC_CLUSTER * TC_CLUSTER;
+    const dim3 grid((unsigned)tiles, (unsigned)(d.cout_pad / bn), 1);
     switch (bn) {
         case 128: return launch_bn<128>(l, a, grid, st, bmap);
         case 64: return launch_bn<64>(l, a, grid, st, bmap);
