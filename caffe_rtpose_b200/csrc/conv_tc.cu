@@ -19,11 +19,12 @@
 //   * Two consumer warpgroups (64 rows each) issue wgmma.mma_async m64nBNk16 from shared-memory descriptors,
 //     accumulators in registers, fp32.
 //   * Split precision: activations and weights are stored as P 16-bit "planes" whose sum is the fp32 value
-//     (hi / lo); the kernel issues the cross products with pa + pb < P on the tensor core.  P=1 plain bf16,
-//     P=2 = parity mode on fp16 planes (kernels.h), ~1e-5 over the whole net (DESIGN.md section 3).
+//     (hi / lo); the kernel issues the cross products with pa + pb < P on the tensor core.  The format (kernels.h,
+//     PlaneFmt): P=2 fp16 = parity mode, ~1e-5 over the whole net (DESIGN.md section 3); P=1 fp16 = fast mode, the
+//     parity mode's hi plane alone (one MMA per MAC); P=1 bf16 and P=3 bf16 are kept for A/B comparisons.
 //     hi*hi goes to its own accumulator, cut into chunks of a few hundred K that are added in registers with
 //     round-to-nearest (the tensor core's fp32 accumulation truncates, so a long chain drifts); the cross terms
-//     are 2^-11 smaller and run over the whole tile in a second accumulator.
+//     are 2^-11 smaller and run over the whole tile in a second accumulator.  bf16x1 keeps one unchunked chain.
 //   * Epilogue: sum, bias, ReLU, re-split into planes and store NHWC planes (channel-slice stores implement
 //     Concat), or - for the last stage - the planar fp32 concat_stage7 blob.
 #include <cuda.h>
@@ -259,12 +260,11 @@ template <int BN, int PLANES> struct TcShape {
     static constexpr int SMEM = W_STAGES * A_BYTES + B_STAGES * B_BYTES + 1024;
 };
 
-template <int BN, int PLANES>
+template <int BN, int PLANES, bool F16>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcArgs a) {
     using S = TcShape<BN, PLANES>;
     constexpr int WS = S::W_STAGES, BS = S::B_STAGES;
-    constexpr bool F16 = planes_are_fp16(PLANES);
     constexpr int NACC = BN / 2;   // fp32 registers per thread of one m64 x BN accumulator
     static_assert(S::B_STAGES >= 2, "shared memory holds fewer than two weight tiles");
     constexpr int WBOX = tc_wbox_rows(BN, PLANES), WSHARE = PLANES * BN / TC_CLUSTER;
@@ -452,9 +452,9 @@ static int env_int(const char* name, int dflt) {
     return v ? atoi(v) : dflt;
 }
 
-template <int BN, int PLANES>
+template <int BN, int PLANES, bool F16>
 static int launch_inst(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap) {
-    auto kern = conv_wg_kernel<BN, PLANES>;
+    auto kern = conv_wg_kernel<BN, PLANES, F16>;
     constexpr int smem = TcShape<BN, PLANES>::SMEM;
     int dev = 0;
     cudaGetDevice(&dev);
@@ -479,12 +479,11 @@ static int launch_inst(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_
 
 template <int BN>
 static int launch_bn(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap) {
-    switch (l.d.planes) {
-        case 1: return launch_inst<BN, 1>(l, a, grid, st, bmap);
-        case 2: return launch_inst<BN, 2>(l, a, grid, st, bmap);
-        default: if constexpr (BN <= 64) return launch_inst<BN, 3>(l, a, grid, st, bmap); else break;
-    }
-    return -1;   // no kernel for this tile width and plane count (tc_bn never picks one)
+    const PlaneFmt f = l.d.fmt;
+    if (f.planes == 1) return f.f16 ? launch_inst<BN, 1, true>(l, a, grid, st, bmap) : launch_inst<BN, 1, false>(l, a, grid, st, bmap);
+    if (f.planes == 2 && f.f16 == PARITY_F16) return launch_inst<BN, 2, PARITY_F16>(l, a, grid, st, bmap);
+    if constexpr (BN <= 64) { if (f.planes == 3 && !f.f16) return launch_inst<BN, 3, false>(l, a, grid, st, bmap); }
+    return -1;   // no kernel for this tile width and plane format (tc_bn never picks one)
 }
 
 static int encode(EncodeTiledFn enc, CUtensorMap* map, const void* base, cuuint64_t d0, cuuint64_t d1, cuuint64_t d2, cuuint64_t s1,
@@ -501,24 +500,24 @@ int tc_layer_create(const TcLayerDesc& d, TcLayer& out, std::string& err) {
     EncodeTiledFn enc = get_encode();
     if (!enc) { err = "cuTensorMapEncodeTiled unavailable"; return -1; }
     if (d.in_cused % TC_BK) { err = "input channels not a multiple of 64"; return -1; }
-    if (d.planes < 1 || d.planes > 3) { err = "1 to 3 planes"; return -1; }
+    if (d.fmt.planes < 1 || d.fmt.planes > 3) { err = "1 to 3 planes"; return -1; }
     if (d.ksize < 1 || d.ksize > TC_KMAX) { err = "filter size above " + std::to_string(TC_KMAX) + " (A window rows)"; return -1; }
     out.d = d;
-    out.bn = tc_bn(d.cout_pad, d.planes);
+    out.bn = tc_bn(d.cout_pad, d.fmt.planes);
     CUtensorMap* maps = nullptr;
     if (posix_memalign((void**)&maps, 64, 3 * sizeof(CUtensorMap))) { err = "alloc"; return -1; }
     memset(maps, 0, 3 * sizeof(CUtensorMap));
     const cuuint64_t K = (cuuint64_t)d.ksize * d.ksize * d.in_cused;
-    const cuuint64_t P = (cuuint64_t)d.planes;
+    const cuuint64_t P = (cuuint64_t)d.fmt.planes;
     // A: [planes][M][pitch], box {64, window rows, planes}
     int r = encode(enc, &maps[0], d.in, d.in_cused, d.geo.M, P, (cuuint64_t)d.in_pitch * 2, (cuuint64_t)d.in_plane * 2,
-                   tc_window_rows(d.ksize), d.planes,
+                   tc_window_rows(d.ksize), d.fmt.planes,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
     // B: [planes][cout_pad][K], box {64, part of a plane, 1} (a CTA's share of a {64, bn, planes} tile is one or more such
     // boxes, tc_wbox_rows); and for half-width tiles (more CTAs for small problems, see tc_layer_launch)
-    if (!r) r = encode(enc, &maps[1], d.w, K, d.cout_pad, P, K * 2, K * 2 * d.cout_pad, tc_wbox_rows(out.bn, d.planes), 1,
+    if (!r) r = encode(enc, &maps[1], d.w, K, d.cout_pad, P, K * 2, K * 2 * d.cout_pad, tc_wbox_rows(out.bn, d.fmt.planes), 1,
                        CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
-    if (!r && out.bn >= 64) r = encode(enc, &maps[2], d.w, K, d.cout_pad, P, K * 2, K * 2 * d.cout_pad, tc_wbox_rows(out.bn / 2, d.planes), 1,
+    if (!r && out.bn >= 64) r = encode(enc, &maps[2], d.w, K, d.cout_pad, P, K * 2, K * 2 * d.cout_pad, tc_wbox_rows(out.bn / 2, d.fmt.planes), 1,
                                        CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
     if (r) { err = "cuTensorMapEncodeTiled failed: " + std::to_string(r); free(maps); return -1; }
     out.maps = maps;
@@ -540,9 +539,10 @@ int tc_layer_launch(const TcLayer& l, int nimg, cudaStream_t st, int share) {
     a.ksize = d.ksize; a.pad = d.pad; a.kblocks_per_tap = d.in_cused / TC_BK; a.cin_k = d.in_cused;
     a.W = d.geo.W; a.H = d.geo.H; a.Wp = d.geo.Wp; a.Hs = d.geo.Hs;
     a.M = (long long)nimg * d.geo.Hs * d.geo.Wp;
-    // hi*hi accumulation chunk with split planes: one 7-tap filter row (448 K), two 3-tap rows (384 K) or four 1x1 blocks (256 K)
+    // hi*hi accumulation chunk with split planes and in the fp16 fast mode: one 7-tap filter row (448 K), two 3-tap rows (384 K)
+    // or four 1x1 blocks (256 K); bf16x1 runs one chain over the whole K
     const int nk = d.ksize * d.ksize * a.kblocks_per_tap;
-    a.chunk_iters = d.planes >= 2 ? (d.ksize >= 7 ? 7 : (d.ksize >= 3 ? 6 : 4)) : nk;
+    a.chunk_iters = (d.fmt.planes >= 2 || d.fmt.f16) ? (d.ksize >= 7 ? 7 : (d.ksize >= 3 ? 6 : 4)) : nk;
     static int nsm = 0;
     if (!nsm) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev); }
     // Tile width: the full width is the efficient shape (the A tile is re-read per N tile), but a single frame at the

@@ -3,18 +3,20 @@
 #include <string>
 
 #include "common.h"
+#include "kernels.h"
 
 namespace pe {
 
 struct TcLayerDesc {
-    const void* in; int in_pitch, in_cused; long long in_plane;   // bf16 planes [P][M][pitch]
-    const void* w;                                                // bf16 planes [P][cout_pad][K]
+    const void* in; int in_pitch, in_cused; long long in_plane;   // 16-bit planes [P][M][pitch]
+    const void* w;                                                // 16-bit planes [P][cout_pad][K]
     const float* bias;
-    int cout, cout_pad, ksize, pad, relu, planes;
+    int cout, cout_pad, ksize, pad, relu;
+    PlaneFmt fmt;                                                 // plane count and fp16 / bf16 (kernels.h)
     const float* out_scale = nullptr;                             // device: epilogue factor 2^-k (weights packed with 2^k)
     unsigned* range = nullptr;                                    // device: running max |stored value| (float bits), or null
     Geo geo;                                                      // geo.N = max images
-    void* out; int out_pitch, out_coff; long long out_plane;      // bf16 planes, or
+    void* out; int out_pitch, out_coff; long long out_plane;      // 16-bit planes, or
     float* planar; int planar_C, planar_coff;                     // final fp32 maps (N, planar_C, H, W)
 };
 struct TcLayer {

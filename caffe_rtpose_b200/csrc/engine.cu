@@ -35,7 +35,7 @@ struct pe_engine {
     const ModelTables* mt = nullptr;
     ModelTables mt_own;     // model tables with the prototxt's nms max_peaks
     Geo geo[4];
-    int planes = 0;         // 0: fp32 SIMT, else bf16 planes
+    PlaneFmt fmt = {0, false};   // storage of activations and packed weights (kernels.h): 0 planes = fp32 SIMT
     int elem = 4;
     std::vector<void*> acts;        // device
     std::vector<long long> act_plane;  // elements per plane
@@ -44,7 +44,7 @@ struct pe_engine {
     // packed weights (one device buffer): per conv offsets (bytes)
     void* d_packed = nullptr; size_t packed_bytes = 0;
     std::shared_ptr<void> packed_owner;   // frees d_packed when the last handle using it goes (pe_share_weights)
-    // fp16-plane range management (parity mode): per-conv-output power-of-two scale s (stored value = true value * s), the true
+    // fp16-plane range management (F16X2, F16X1): per-conv-output power-of-two scale s (stored value = true value * s), the true
     // biases / weight-scale inverses the packed epilogue fields derive from, and the kernels' running max |stored value| per conv
     std::vector<float> conv_scale, wsi;   // per conv: scale of its stored output; inverse of the power of two folded into its weights
     std::vector<std::vector<float>> bias_true;
@@ -287,7 +287,7 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
     if (cfg->num_scales < 1 || cfg->num_scales > PE_MAX_SCALES) return fail(nullptr, PE_ERR_INVALID, "num_scales %d out of [1,%d]", cfg->num_scales, PE_MAX_SCALES);
     if (cfg->max_batch < 1 || cfg->max_batch > 64) return fail(nullptr, PE_ERR_INVALID, "max_batch %d out of [1,64]", cfg->max_batch);
     if (cfg->disp_w <= 0 || cfg->disp_h <= 0) return fail(nullptr, PE_ERR_INVALID, "bad display resolution");
-    if (cfg->precision < 0 || cfg->precision > 3) return fail(nullptr, PE_ERR_INVALID, "unknown precision %d", cfg->precision);
+    if (cfg->precision < 0 || cfg->precision > 4) return fail(nullptr, PE_ERR_INVALID, "unknown precision %d", cfg->precision);
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
         return fail(nullptr, PE_ERR_CUDA, "no CUDA device visible: the pose engine has no CPU fallback");
@@ -300,18 +300,18 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
     e->mt_own = model_tables(cfg->model);
     if (prototxt_path) e->mt_own.max_peaks = proto_plan.nms_max_peaks;   // nms_param.max_peaks (NmsLayer::GetMaxPeaks, rtpose.cpp:195)
     e->mt = &e->mt_own;
-    e->planes = cfg->precision;  // 0 fp32, else number of bf16 planes
+    e->fmt = plane_fmt(cfg->precision);
     if (const char* g = getenv("PE_GRAPH")) e->use_graphs = atoi(g) != 0;
     if (const char* g = getenv("PE_CONV11_DIRECT")) e->conv11_direct = atoi(g) != 0;
     if (const char* g = getenv("PE_CHECK_RANGE")) e->check_range = atoi(g) != 0;
-    e->elem = e->planes == 0 ? 4 : 2;
+    e->elem = e->fmt.planes == 0 ? 4 : 2;
     e->start_scale_f = (float)cfg->start_scale;  // ImResizeLayer::SetStartScale(float)
     e->scale_gap_f = (float)cfg->scale_gap;
     auto bail = [&](int rc) { g_create_error = e->err; pe_destroy(e); return rc; };
 #define CKC(call) do { cudaError_t err_ = (call); if (err_ != cudaSuccess) { \
     fail(e, PE_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(err_), __FILE__, __LINE__); return bail(PE_ERR_CUDA); } } while (0)
     CKC(cudaSetDevice(cfg->device));
-    if (e->planes) {
+    if (e->fmt.planes) {
         cudaDeviceProp prop;
         CKC(cudaGetDeviceProperties(&prop, cfg->device));
         if (prop.major != 9) { fail(e, PE_ERR_INVALID, "wgmma precision modes need sm_90 (found sm_%d%d)", prop.major, prop.minor); return bail(PE_ERR_INVALID); }
@@ -326,9 +326,9 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
         w = pooled(w); h = pooled(h);
     }
     if (e->geo[3].W * 8 != cfg->net_w || e->geo[3].H * 8 != cfg->net_h) { fail(e, PE_ERR_INVALID, "net size not divisible by 8 after pooling"); return bail(PE_ERR_INVALID); }
-    e->plan = prototxt_path ? proto_plan : build_plan(cfg->model, e->planes ? 64 : 32, e->planes ? 64 : 16);
+    e->plan = prototxt_path ? proto_plan : build_plan(cfg->model, e->fmt.planes ? 64 : 32, e->fmt.planes ? 64 : 16);
     e->hw.resize(e->plan.convs.size());
-    if (e->planes && setup_lanes(e)) return bail(PE_ERR_CUDA);
+    if (e->fmt.planes && setup_lanes(e)) return bail(PE_ERR_CUDA);
     // FLOPs (SURVEY.md section 8d): 2*Cout*Cin*k^2*Hout*Wout per conv and image
     e->flops_per_scale = 0;
     for (auto& c : e->plan.convs) {
@@ -343,7 +343,7 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
         const ActSpec& a = e->plan.acts[i];
         const Geo& g = e->geo[a.level];
         e->act_plane[i] = g.M * a.C;
-        const size_t bytes = (size_t)e->act_plane[i] * e->elem * (e->planes ? e->planes : 1);
+        const size_t bytes = (size_t)e->act_plane[i] * e->elem * (e->fmt.planes ? e->fmt.planes : 1);
         CKC(cudaMalloc(&e->acts[i], bytes));
         CKC(cudaMemsetAsync(e->acts[i], 0, bytes, e->stream));
     }
@@ -362,7 +362,7 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
     if (build_pre_tables(e)) return bail(PE_ERR_INVALID);
     e->pre.frames = e->d_frames; e->pre.resized = e->d_resized;
     e->pre.out = e->acts[e->plan.input_act]; e->pre.kp = e->plan.kp_input;
-    e->pre.out_plane = e->act_plane[e->plan.input_act]; e->pre.planes = e->planes;
+    e->pre.out_plane = e->act_plane[e->plan.input_act]; e->pre.fmt = e->fmt;
     e->pre.Wp = e->geo[0].Wp; e->pre.Hs = e->geo[0].Hs;
 
     // post-processing state
@@ -502,7 +502,7 @@ static inline void split_bf16(float x, int planes, uint16_t* out) {
         r = r - hf;
     }
 }
-static inline void split_fp16(float x, int planes, uint16_t* out) {   // parity mode: IEEE fp16 planes (kernels.h)
+static inline void split_fp16(float x, int planes, uint16_t* out) {   // IEEE fp16 planes (kernels.h)
     float r = x;
     for (int p = 0; p < planes; p++) {
         const __half h = __float2half_rn(r);
@@ -520,10 +520,10 @@ static size_t packed_layout(pe_engine* e) {
     for (size_t i = 0; i < nc; i++) {
         const ConvSpec& c = e->plan.convs[i];
         e->cin_pad[i] = c.in_cused;
-        e->cout_pad[i] = e->planes ? tc_cout_pad(c.cout) : (c.cout + 63) / 64 * 64;
+        e->cout_pad[i] = e->fmt.planes ? tc_cout_pad(c.cout) : (c.cout + 63) / 64 * 64;
         const size_t K = (size_t)(c.im2col_input ? 1 : c.k * c.k) * e->cin_pad[i];
         e->w_off[i] = total;
-        total = align256(total + K * e->cout_pad[i] * e->elem * (e->planes ? e->planes : 1));
+        total = align256(total + K * e->cout_pad[i] * e->elem * (e->fmt.planes ? e->fmt.planes : 1));
         e->b_off[i] = total;
         total = align256(total + (size_t)(e->cout_pad[i] + 1) * 4);   // bias[cout_pad] + the layer's epilogue scale
     }
@@ -575,9 +575,9 @@ static void pack_conv_weights(pe_engine* e, int i, uint8_t* dst) {
         if (ci < 0) return 0.f;
         return hw.w[((size_t)co * c.cin + ci) * c.k * c.k + tap] * chan[ec];
     };
-    memset(dst, 0, K * cop * e->elem * (e->planes ? e->planes : 1));
+    memset(dst, 0, K * cop * e->elem * (e->fmt.planes ? e->fmt.planes : 1));
     float wscale_inv = 1.f;
-    if (e->planes == 0) {  // fp32 [K][cout_pad]
+    if (e->fmt.planes == 0) {  // fp32 [K][cout_pad]
         float* W = (float*)dst;
         for (size_t kk = 0; kk < K; kk++)
             for (int co = 0; co < c.cout; co++) W[kk * cop + co] = src(co, (int)kk);
@@ -587,7 +587,7 @@ static void pack_conv_weights(pe_engine* e, int i, uint8_t* dst) {
         // fp16 planes: scale the layer by 2^k so that max|w| lands in [2^13, 2^14) - small weights would otherwise
         // put their lo plane into fp16 subnormals.  Exact (power of two); the epilogue multiplies by 2^-k.
         float wscale = 1.f;
-        if (planes_are_fp16(e->planes)) {
+        if (e->fmt.f16) {
             float mx = 0.f;
             for (int co = 0; co < c.cout; co++)
                 for (size_t kk = 0; kk < K; kk++) mx = fmaxf(mx, fabsf(src(co, (int)kk)));
@@ -598,9 +598,9 @@ static void pack_conv_weights(pe_engine* e, int i, uint8_t* dst) {
         for (int co = 0; co < c.cout; co++)
             for (size_t kk = 0; kk < K; kk++) {
                 uint16_t h[3];
-                if (planes_are_fp16(e->planes)) split_fp16(src(co, (int)kk) * wscale, e->planes, h);
-                else split_bf16(src(co, (int)kk), e->planes, h);
-                for (int p = 0; p < e->planes; p++) W[p * plane + (size_t)co * K + kk] = h[p];
+                if (e->fmt.f16) split_fp16(src(co, (int)kk) * wscale, e->fmt.planes, h);
+                else split_bf16(src(co, (int)kk), e->fmt.planes, h);
+                for (int p = 0; p < e->fmt.planes; p++) W[p * plane + (size_t)co * K + kk] = h[p];
             }
     }
     e->wsi[i] = wscale_inv;
@@ -609,11 +609,11 @@ static void pack_conv_weights(pe_engine* e, int i, uint8_t* dst) {
 // per-layer launch state (TMA descriptors) over the packed buffer the handle currently points at
 static int bind_packed(pe_engine* e) {
     const size_t nc = e->plan.convs.size();
-    if (planes_are_fp16(e->planes) && !e->d_range) {
+    if (e->fmt.f16 && !e->d_range) {
         CK(e, cudaMalloc(&e->d_range, nc * sizeof(unsigned)));
         CK(e, cudaMemset(e->d_range, 0, nc * sizeof(unsigned)));
     }
-    if (e->planes) {
+    if (e->fmt.planes) {
         for (auto& t : e->tc) tc_layer_destroy(t);
         e->tc.assign(nc, TcLayer());
         for (size_t i = 0; i < nc; i++) {
@@ -623,8 +623,8 @@ static int bind_packed(pe_engine* e) {
             d.in = e->acts[c.in_act]; d.in_pitch = e->plan.acts[c.in_act].C; d.in_cused = c.in_cused; d.in_plane = e->act_plane[c.in_act];
             d.w = (char*)e->d_packed + e->w_off[i]; d.bias = (const float*)((char*)e->d_packed + e->b_off[i]);
             d.cout = c.cout; d.cout_pad = e->cout_pad[i]; d.ksize = c.im2col_input ? 1 : c.k; d.pad = c.im2col_input ? 0 : c.pad;
-            d.relu = c.relu; d.planes = e->planes; d.geo = g; d.out_scale = d.bias + e->cout_pad[i];
-            d.range = (planes_are_fp16(e->planes) && e->d_range) ? e->d_range + i : nullptr;
+            d.relu = c.relu; d.fmt = e->fmt; d.geo = g; d.out_scale = d.bias + e->cout_pad[i];
+            d.range = (e->fmt.f16 && e->d_range) ? e->d_range + i : nullptr;
             if (c.out_act >= 0) {
                 d.out = e->acts[c.out_act]; d.out_pitch = e->plan.acts[c.out_act].C; d.out_coff = c.out_coff; d.out_plane = e->act_plane[c.out_act];
                 d.planar = nullptr; d.planar_C = 0; d.planar_coff = 0;
@@ -827,7 +827,7 @@ static int run_op(pe_engine* e, const OpRef& op, int nimg, cudaStream_t st = nul
                                                  c.relu, nimg, st);
             return PE_OK;
         }
-        if (e->planes) {
+        if (e->fmt.planes) {
             const int n = tc_layer_launch(e->tc[op.idx], nimg, st, share);
             if (n < 0) return fail(e, PE_ERR_CUDA, "conv %s: tensor-core launch failed or no kernel fits the tile (%s)", c.name.c_str(), cudaGetErrorString(cudaGetLastError()));
             e->launches += n;
@@ -848,7 +848,7 @@ static int run_op(pe_engine* e, const OpRef& op, int nimg, cudaStream_t st = nul
         const Geo& gi = e->geo[p.level_in]; const Geo& go = e->geo[p.level_in + 1];
         PoolArgs a;
         a.in = e->acts[p.in_act]; a.out = e->acts[p.out_act]; a.C = e->plan.acts[p.in_act].C;
-        a.in_plane = e->act_plane[p.in_act]; a.out_plane = e->act_plane[p.out_act]; a.planes = e->planes;
+        a.in_plane = e->act_plane[p.in_act]; a.out_plane = e->act_plane[p.out_act]; a.fmt = e->fmt;
         a.Wi = gi.W; a.Hi = gi.H; a.Wpi = gi.Wp; a.Hsi = gi.Hs; a.Wo = go.W; a.Ho = go.H; a.Wpo = go.Wp; a.Hso = go.Hs; a.N = nimg;
         e->launches += launch_pool(a, st);
     } else {
@@ -856,7 +856,7 @@ static int run_op(pe_engine* e, const OpRef& op, int nimg, cudaStream_t st = nul
         const Geo& g = e->geo[3];
         CopyArgs a;
         a.src = e->acts[c.src_act]; a.dst = e->acts[c.dst_act]; a.pitch = e->plan.acts[c.src_act].C; a.channels = c.channels;
-        a.elem_bytes = e->elem; a.M = (long long)nimg * g.Hs * g.Wp; a.plane = e->act_plane[c.src_act]; a.planes = e->planes;
+        a.elem_bytes = e->elem; a.M = (long long)nimg * g.Hs * g.Wp; a.plane = e->act_plane[c.src_act]; a.fmt = e->fmt;
         e->launches += launch_copy_channels(a, st);
     }
     return PE_OK;
@@ -986,7 +986,7 @@ extern "C" int pe_forward_frames_device(pe_engine* e, const void* d_frames, int 
     PreArgs a = e->pre;
     a.frames = (const uint8_t*)d_frames; a.nframes = n;
     if (e->input_lo_dirty) {   // the uint8 path only writes the hi plane; drop what the planar path left behind
-        const size_t bytes = (size_t)e->act_plane[e->plan.input_act] * e->elem * (e->planes ? e->planes : 1);
+        const size_t bytes = (size_t)e->act_plane[e->plan.input_act] * e->elem * (e->fmt.planes ? e->fmt.planes : 1);
         CK(e, cudaMemsetAsync(e->acts[e->plan.input_act], 0, bytes, e->stream));
         e->input_lo_dirty = false;
     }
@@ -1125,7 +1125,7 @@ extern "C" int pe_forward_camera_frames(pe_engine* e, const uint8_t* const* fram
 }
 
 // ---------------------------------------------------------------------------------------------
-// Range calibration of the fp16-plane parity mode.  The planes hold value * s with a per-activation power-of-two s; without
+// Range calibration of the fp16-plane modes (parity F16X2 and fast F16X1).  The planes hold value * s with a per-activation power-of-two s; without
 // calibration s = 1, which suits nets whose activations are O(1e-2 .. 1e3) (the trained pose models).  A net outside that range -
 // the prototxt's own gaussian(0.01) filler shrinks every layer until the maps are ~3e-11 - would flush to zero (or overflow to inf)
 // silently.  pe_calibrate runs ONE forward layer by layer: each conv first runs with s_out = 1 while the epilogue records the
@@ -1145,7 +1145,7 @@ static int upload_fields(pe_engine* e, int i) {
 static int upload_weights(pe_engine* e, int i) {   // re-pack layer i with the current input scales (host fp32 copy needed)
     const ConvSpec& c = e->plan.convs[i];
     const size_t K = (size_t)(c.im2col_input ? 1 : c.k * c.k) * e->cin_pad[i];
-    std::vector<uint8_t> buf(K * e->cout_pad[i] * e->elem * (e->planes ? e->planes : 1));
+    std::vector<uint8_t> buf(K * e->cout_pad[i] * e->elem * (e->fmt.planes ? e->fmt.planes : 1));
     pack_conv_weights(e, i, buf.data());
     CK(e, cudaMemcpyAsync((char*)e->d_packed + e->w_off[i], buf.data(), buf.size(), cudaMemcpyHostToDevice, e->stream));
     CK(e, cudaStreamSynchronize(e->stream));
@@ -1156,7 +1156,7 @@ extern "C" int pe_calibrate(pe_engine* e, const uint8_t* const* frames, int n) {
     int rc = check_n(e, n); if (rc) return rc;
     if (!frames) return fail(e, PE_ERR_INVALID, "null frames");
     if (!e->committed) return fail(e, PE_ERR_STATE, "pe_commit_weights has not been called");
-    if (!planes_are_fp16(e->planes)) return PE_OK;   // fp32 / bf16 modes have fp32's exponent range
+    if (!e->fmt.f16) return PE_OK;   // fp32 / bf16 modes have fp32's exponent range
     const size_t nc = e->plan.convs.size();
     if (e->bias_true.size() != nc || e->bias_true[0].empty() || e->hw[0].w.empty())
         return fail(e, PE_ERR_STATE, "this handle received its weights by broadcast / sharing: calibrate the source handle before replicating");
@@ -1238,7 +1238,7 @@ extern "C" int pe_range_status(pe_engine* e, float* worst_ratio, char* layer64) 
     if (worst_ratio) *worst_ratio = worst;
     if (worst >= 1.f) {
         if (layer64) snprintf(layer64, 64, "%s", e->plan.convs[iw].name.c_str());
-        return fail(e, PE_ERR_RANGE, "layer %s produced values outside the fp16 range of the parity mode (max |v| = %.3g x scale): run pe_calibrate",
+        return fail(e, PE_ERR_RANGE, "layer %s produced values outside the range of the fp16 planes (max |v| = %.3g x scale): run pe_calibrate",
                     e->plan.convs[iw].name.c_str(), worst * 65504.f);
     }
     if (is >= 0 && smallest < 9.765625e-4f) {
@@ -1261,7 +1261,7 @@ extern "C" int pe_forward_net_input(pe_engine* e, const float* net_input, int n)
     PreArgs a = e->pre;
     a.nframes = n;
     e->launches += launch_input_from_planar(e->d_planar, a, n * e->cfg.num_scales, e->stream);
-    e->input_lo_dirty = e->planes > 0;
+    e->input_lo_dirty = e->fmt.planes > 0;
     e->last_frames = nullptr;
     if (e->input_from_frames) drop_graphs(e);   // the captured graphs hold the other conv1_1 kernel
     e->input_from_frames = false;
@@ -1430,7 +1430,7 @@ extern "C" int pe_fetch_blob(pe_engine* e, const char* blob_name, float* out, si
         CK(e, cudaMalloc(&d, cnt * sizeof(float)));
         // stored value = true value * conv_scale[producer] (pools pass their producer's scale through; the net input has none)
         const float inv = (b.prod >= 0 && b.prod < (int)e->conv_scale.size()) ? 1.f / e->conv_scale[b.prod] : 1.f;
-        e->launches += launch_act_to_nchw(e->acts[b.act], e->plan.acts[b.act].C, b.coff, b.c, e->act_plane[b.act], e->planes, g, inv, d,
+        e->launches += launch_act_to_nchw(e->acts[b.act], e->plan.acts[b.act].C, b.coff, b.c, e->act_plane[b.act], e->fmt, g, inv, d,
                                           e->stream);
         CK(e, cudaMemcpyAsync(out, d, cnt * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
         CK(e, cudaStreamSynchronize(e->stream));
@@ -1469,6 +1469,47 @@ extern "C" int pe_write_json(const float* joints, int num_people, int num_parts,
     s += "]\n}\n";
     if (buf && (int)s.size() < cap) memcpy(buf, s.c_str(), s.size() + 1);
     return (int)s.size();
+}
+
+// ---------------------------------------------------------------------------------------------
+// Result comparison (DESIGN.md section 6 (3)): peaks, person count and joints of two fetched results of one frame
+// ---------------------------------------------------------------------------------------------
+extern "C" int pe_compare_results(const float* joints_a, int people_a, const float* peaks_a, const float* joints_b, int people_b,
+                                  const float* peaks_b, int num_parts, int max_peaks, float tol_px, pe_result_diff* out) {
+    if (!out || !peaks_a || !peaks_b || num_parts <= 0 || max_peaks < 0 || people_a < 0 || people_b < 0 || !(tol_px >= 0.f) ||
+        (people_a > 0 && !joints_a) || (people_b > 0 && !joints_b))
+        return PE_ERR_INVALID;
+    memset(out, 0, sizeof *out);
+    auto dist = [](const float* p, const float* q) { return hypot((double)p[0] - q[0], (double)p[1] - q[1]); };
+    const size_t part_stride = (size_t)(max_peaks + 1) * 3;
+    for (int p = 0; p < num_parts; p++) {
+        const float* pa = peaks_a + p * part_stride;
+        const float* pb = peaks_b + p * part_stride;
+        const int ca = std::min((int)pa[0], max_peaks), cb = std::min((int)pb[0], max_peaks);
+        if (ca != cb) { out->parts_count_differ++; continue; }
+        for (int k = 1; k <= ca; k++)
+            if (!(dist(pa + 3 * k, pb + 3 * k) <= tol_px)) out->peaks_moved++;
+    }
+    bool joints_ok = true;
+    double worst = 0.0;
+    for (int i = 0; i < std::min(people_a, people_b); i++) {
+        const float* ja = joints_a + (size_t)i * num_parts * 3;
+        const float* jb = joints_b + (size_t)i * num_parts * 3;
+        bool same = true;
+        for (int p = 0; p < num_parts && same; p++) same = (ja[3 * p + 2] > 0.f) == (jb[3 * p + 2] > 0.f);
+        if (!same) continue;
+        out->persons_matched++;
+        for (int p = 0; p < num_parts; p++)
+            if (ja[3 * p + 2] > 0.f) {
+                const double d = dist(ja + 3 * p, jb + 3 * p);
+                if (!(d <= tol_px)) joints_ok = false;
+                worst = std::max(worst, d);
+            }
+    }
+    out->max_joint_dist = (float)worst;
+    out->identical = out->parts_count_differ == 0 && out->peaks_moved == 0 && people_a == people_b &&
+                     out->persons_matched == people_a && joints_ok;
+    return PE_OK;
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -4,15 +4,26 @@
 
 namespace pe {
 
-// 16-bit "plane" formats of the tensor-core conv stack.  The parity mode (2 planes) stores IEEE fp16 planes: 11 + 11
-// significant bits, so hi*hi + hi*lo + lo*hi carries ~2^-22 (bf16 planes: 8 + 8 bits, ~2^-17 - measured 2.2e-5 over
-// the net with exact accumulation vs 3e-6 for fp16).  fp16's range (65504) is ample for this net (inputs in
-// [-0.5, 0.5], activations O(1-100)); the 1- and 3-plane modes keep bf16.
+// Storage format of the conv stack's activations and packed weights: `planes` 16-bit planes whose sum is the value (0: fp32),
+// IEEE fp16 planes when f16 is set, else bf16.  The parity mode (2 planes) stores fp16 planes: 11 + 11 significant bits, so
+// hi*hi + hi*lo + lo*hi carries ~2^-22 (bf16 planes: 8 + 8 bits, ~2^-17 - measured 2.2e-5 over the net with exact accumulation
+// vs 3e-6 for fp16).  The fast mode (F16X1) is the parity mode's hi plane alone.  fp16's range (65504) needs the per-layer
+// power-of-two range scales of pe_calibrate for nets outside O(1e-2 .. 1e3); the bf16 modes (BF16X1, BF16X3) have fp32's range.
+struct PlaneFmt { int planes; bool f16; };
 #ifdef PE_PARITY_PLANES_BF16   // A/B build: parity mode on bf16 planes (8 + 8 bits, 2.1e-5 over the net), see DESIGN.md section 3
-__host__ __device__ constexpr bool planes_are_fp16(int) { return false; }
+constexpr bool PARITY_F16 = false;
 #else
-__host__ __device__ constexpr bool planes_are_fp16(int planes) { return planes == 2; }
+constexpr bool PARITY_F16 = true;
 #endif
+inline PlaneFmt plane_fmt(int precision) {   // PE_PREC_* -> format
+    switch (precision) {
+        case PE_PREC_BF16X1: return {1, false};
+        case PE_PREC_F16X2: return {2, PARITY_F16};
+        case PE_PREC_BF16X3: return {3, false};
+        case PE_PREC_F16X1: return {1, true};
+        default: return {0, false};   // PE_PREC_FP32_SIMT
+    }
+}
 #ifdef __CUDACC__
 template <bool F16> __device__ __forceinline__ float plane_to_float(uint16_t h) {
     return F16 ? __half2float(__ushort_as_half(h)) : __uint_as_float((uint32_t)h << 16);
@@ -87,7 +98,7 @@ struct PreArgs {
     AreaTab tab[PE_MAX_SCALES];
     int nframes, S, disp_w, disp_h, net_w, net_h;
     // im2col'ed network input, flat padded level-0 geometry
-    void* out; int kp; long long out_plane; int planes;   // planes == 0: fp32, else bf16 planes
+    void* out; int kp; long long out_plane; PlaneFmt fmt;
     int Wp, Hs;
 };
 int launch_preprocess(const PreArgs& a, cudaStream_t st, bool with_im2col = true);
@@ -107,15 +118,15 @@ int launch_input_from_planar(const float* planar, const PreArgs& a, int nimages,
 // ---- convolution / pooling (conv_simt.cu, conv_tc.cu, pool.cu)
 int launch_conv_simt(const ConvArgs& a, cudaStream_t st);
 struct PoolArgs {
-    const void* in; void* out; int C; long long in_plane, out_plane; int planes;  // planes==0: fp32
+    const void* in; void* out; int C; long long in_plane, out_plane; PlaneFmt fmt;
     int Wi, Hi, Wpi, Hsi, Wo, Ho, Wpo, Hso, N;
 };
 int launch_pool(const PoolArgs& a, cudaStream_t st);
-struct CopyArgs { const void* src; void* dst; int pitch, channels, elem_bytes; long long M, plane; int planes; };
+struct CopyArgs { const void* src; void* dst; int pitch, channels, elem_bytes; long long M, plane; PlaneFmt fmt; };
 int launch_copy_channels(const CopyArgs& a, cudaStream_t st);
-// activation (flat padded, fp32 or bf16 planes) -> NCHW fp32 (debug / pe_fetch_blob); scale: the inverse of the power-of-two
+// activation (flat padded, fp32 or 16-bit planes) -> NCHW fp32 (debug / pe_fetch_blob); scale: the inverse of the power-of-two
 // range scale the stored values carry (engine.cu, fill_epilogue_fields), so that out holds true values
-int launch_act_to_nchw(const void* act, int pitch, int coff, int c, long long plane, int planes, const Geo& g, float scale,
+int launch_act_to_nchw(const void* act, int pitch, int coff, int c, long long plane, PlaneFmt fmt, const Geo& g, float scale,
                        float* out, cudaStream_t st);
 
 }  // namespace pe

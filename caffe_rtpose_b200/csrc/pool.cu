@@ -1,7 +1,7 @@
 // 2x2 stride-2 MAX pooling (ceil dims), channel-slice copy and layout conversion on the flat padded layout.
 //
 // Pooling semantics: src/caffe/layers/pooling_layer.cpp:90-93 (ceil), :128-187 (max over the window clipped
-// to the image).  Activations are either fp32 [M][C] or bf16 "planes" whose SUM is the value (split
+// to the image).  Activations are either fp32 [M][C] or 16-bit "planes" whose SUM is the value (split
 // precision for the wgmma conv, see conv_tc.cu); the max is taken on the reconstructed value and the
 // winner's planes are copied, which keeps the split exact.
 #include "common.h"
@@ -34,8 +34,8 @@ __global__ void __launch_bounds__(256) pool_f32_kernel(PoolArgs a) {
     *((float4*)((float*)a.out + mo * a.C) + g) = best;
 }
 
-template <int PLANES>
-__global__ void __launch_bounds__(256) pool_bf16_kernel(PoolArgs a) {
+template <int PLANES, bool F16>
+__global__ void __launch_bounds__(256) pool_planes_kernel(PoolArgs a) {
     const unsigned cv = a.C / 8;  // 8 channels (16 bytes) per thread and plane
     const int n = blockIdx.y;     // grid.y = image; 32-bit index math inside an image
     const unsigned per_img = (unsigned)a.Hso * (unsigned)a.Wpo;
@@ -67,7 +67,7 @@ __global__ void __launch_bounds__(256) pool_bf16_kernel(PoolArgs a) {
         for (int w = 0; w < 4; w++) {
             float sum = 0.f;
 #pragma unroll
-            for (int p = 0; p < PLANES; p++) sum += plane_to_float<planes_are_fp16(PLANES)>(((const uint16_t*)&v[w][p])[j]);
+            for (int p = 0; p < PLANES; p++) sum += plane_to_float<F16>(((const uint16_t*)&v[w][p])[j]);
             if (ok[w] && sum > best) { best = sum; bw = w; }
         }
 #pragma unroll
@@ -86,15 +86,17 @@ __global__ void __launch_bounds__(256) pool_bf16_kernel(PoolArgs a) {
 
 int launch_pool(const PoolArgs& a, cudaStream_t st) {
     const long long rows_out = (long long)a.N * a.Hso * a.Wpo;
-    if (a.planes == 0) {
+    const PlaneFmt f = a.fmt;
+    if (f.planes == 0) {
         const long long total = rows_out * (a.C / 4);
         pool_f32_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(a);
     } else {
         const unsigned per = (unsigned)a.Hso * a.Wpo * (a.C / 8);
         const dim3 grid((per + 255) / 256, a.N);
-        if (a.planes == 1) pool_bf16_kernel<1><<<grid, 256, 0, st>>>(a);
-        else if (a.planes == 2) pool_bf16_kernel<2><<<grid, 256, 0, st>>>(a);
-        else pool_bf16_kernel<3><<<grid, 256, 0, st>>>(a);
+        if (f.planes == 1 && f.f16) pool_planes_kernel<1, true><<<grid, 256, 0, st>>>(a);
+        else if (f.planes == 1) pool_planes_kernel<1, false><<<grid, 256, 0, st>>>(a);
+        else if (f.planes == 2) pool_planes_kernel<2, PARITY_F16><<<grid, 256, 0, st>>>(a);
+        else pool_planes_kernel<3, false><<<grid, 256, 0, st>>>(a);
     }
     return 1;
 }
@@ -103,7 +105,7 @@ int launch_pool(const PoolArgs& a, cudaStream_t st) {
 __global__ void __launch_bounds__(256) copy_channels_kernel(CopyArgs a) {
     const int chunks = a.channels * a.elem_bytes / 16;
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const int np = a.planes == 0 ? 1 : a.planes;
+    const int np = a.fmt.planes == 0 ? 1 : a.fmt.planes;
     if (idx >= a.M * chunks * np) return;
     const int ch = (int)(idx % chunks);
     const long long r = idx / chunks;
@@ -114,13 +116,13 @@ __global__ void __launch_bounds__(256) copy_channels_kernel(CopyArgs a) {
 }
 int launch_copy_channels(const CopyArgs& a, cudaStream_t st) {
     const int chunks = a.channels * a.elem_bytes / 16;
-    const long long total = a.M * chunks * (a.planes == 0 ? 1 : a.planes);
+    const long long total = a.M * chunks * (a.fmt.planes == 0 ? 1 : a.fmt.planes);
     copy_channels_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(a);
     return 1;
 }
 
 __global__ void __launch_bounds__(256) act_to_nchw_kernel(const void* act, int pitch, int coff, int c, long long plane,
-                                                          int planes, Geo g, float scale, float* out) {
+                                                          PlaneFmt fmt, Geo g, float scale, float* out) {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const long long total = (long long)g.N * c * g.H * g.W;
     if (idx >= total) return;
@@ -130,17 +132,17 @@ __global__ void __launch_bounds__(256) act_to_nchw_kernel(const void* act, int p
     const int n = (int)(idx / ((long long)g.W * g.H * c));
     const long long m = ((long long)n * g.Hs + y) * g.Wp + x;
     float v = 0.f;
-    if (planes == 0) v = ((const float*)act)[m * pitch + coff + ch];
-    else for (int p = 0; p < planes; p++) {
+    if (fmt.planes == 0) v = ((const float*)act)[m * pitch + coff + ch];
+    else for (int p = 0; p < fmt.planes; p++) {
         const uint16_t h = ((const uint16_t*)act)[p * plane + m * pitch + coff + ch];
-        v += planes_are_fp16(planes) ? plane_to_float<true>(h) : plane_to_float<false>(h);
+        v += fmt.f16 ? plane_to_float<true>(h) : plane_to_float<false>(h);
     }
     out[idx] = v * scale;   // a power of two: exact
 }
-int launch_act_to_nchw(const void* act, int pitch, int coff, int c, long long plane, int planes, const Geo& g, float scale,
+int launch_act_to_nchw(const void* act, int pitch, int coff, int c, long long plane, PlaneFmt fmt, const Geo& g, float scale,
                        float* out, cudaStream_t st) {
     const long long total = (long long)g.N * c * g.H * g.W;
-    act_to_nchw_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(act, pitch, coff, c, plane, planes, g, scale, out);
+    act_to_nchw_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(act, pitch, coff, c, plane, fmt, g, scale, out);
     return 1;
 }
 

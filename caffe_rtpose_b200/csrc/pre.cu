@@ -132,7 +132,7 @@ __global__ void __launch_bounds__(256) input_im2col_kernel(PreArgs a, const floa
     // uint8 pixels normalised by /256-0.5 are exact in bf16 (8 significant bits) and in fp16, so the SRC=0 path fills only the
     // hi plane and only the 32 channels that can be non-zero (27 used); everything else stays zero from init
     // (the engine clears the other planes when it switches from the planar-input path, see engine.cu).
-    const int parts = (SRC == 0 && a.planes > 0) ? 4 : a.kp / 8;
+    const int parts = (SRC == 0 && a.fmt.planes > 0) ? 4 : a.kp / 8;
     // grid.y = image; 32-bit index math inside an image (64-bit divisions cost hundreds of cycles on the GPU)
     const int n = blockIdx.y;
     const unsigned per_img = (unsigned)a.Hs * (unsigned)a.Wp;
@@ -166,7 +166,7 @@ __global__ void __launch_bounds__(256) input_im2col_kernel(PreArgs a, const floa
         }
         v[j] = val;
     }
-    if (a.planes == 0) {
+    if (a.fmt.planes == 0) {
         float4* o = (float4*)((float*)a.out + (size_t)m * a.kp + part * 8);
         o[0] = make_float4(v[0], v[1], v[2], v[3]);
         o[1] = make_float4(v[4], v[5], v[6], v[7]);
@@ -175,14 +175,14 @@ __global__ void __launch_bounds__(256) input_im2col_kernel(PreArgs a, const floa
 #pragma unroll
         for (int j = 0; j < 8; j += 2) {
             uint16_t h0, m0, l0, h1, m1, l1;
-            if (planes_are_fp16(a.planes)) { split3<true>(v[j], h0, m0, l0); split3<true>(v[j + 1], h1, m1, l1); }
+            if (a.fmt.f16) { split3<true>(v[j], h0, m0, l0); split3<true>(v[j + 1], h1, m1, l1); }
             else { split3<false>(v[j], h0, m0, l0); split3<false>(v[j + 1], h1, m1, l1); }
             pk[0][j / 2] = (uint32_t)h0 | ((uint32_t)h1 << 16);
             pk[1][j / 2] = (uint32_t)m0 | ((uint32_t)m1 << 16);
             pk[2][j / 2] = (uint32_t)l0 | ((uint32_t)l1 << 16);
         }
         __nv_bfloat16* o0 = (__nv_bfloat16*)a.out + (size_t)m * a.kp + part * 8;
-        const int np = SRC == 0 ? 1 : a.planes;
+        const int np = SRC == 0 ? 1 : a.fmt.planes;
         for (int p = 0; p < np; p++)
             *(uint4*)(o0 + (size_t)p * a.out_plane) = make_uint4(pk[p][0], pk[p][1], pk[p][2], pk[p][3]);
     }
@@ -232,13 +232,13 @@ __global__ void __launch_bounds__(256) input_im2col_u8_kernel(PreArgs a) {
 }
 
 int launch_im2col_u8(const PreArgs& a, cudaStream_t st) {
-    if (a.planes > 0 && a.kp >= 32) {
+    if (a.fmt.planes > 0 && a.kp >= 32) {
         const dim3 g((a.net_w + 31) / 32, (a.net_h + 7) / 8, a.nframes * a.S), b(32, 8);
-        if (planes_are_fp16(a.planes)) input_im2col_u8_kernel<true><<<g, b, 0, st>>>(a);
+        if (a.fmt.f16) input_im2col_u8_kernel<true><<<g, b, 0, st>>>(a);
         else input_im2col_u8_kernel<false><<<g, b, 0, st>>>(a);
         return 1;
     }
-    const unsigned work = (unsigned)a.Hs * a.Wp * (a.planes > 0 ? 4 : a.kp / 8);
+    const unsigned work = (unsigned)a.Hs * a.Wp * (a.fmt.planes > 0 ? 4 : a.kp / 8);
     input_im2col_kernel<0><<<dim3((work + 255) / 256, a.nframes * a.S), 256, 0, st>>>(a, nullptr, a.nframes * a.S);
     return 1;
 }
@@ -259,7 +259,7 @@ int launch_preprocess(const PreArgs& a, cudaStream_t st, bool with_im2col) {
 // order (c, kh, kw) in fp32 - exact fp32 products, so closer to the reference than the split-fp16 path - and the
 // result leaves as coalesced 512-byte rows (staged per warp through swizzled shared memory).
 // ------------------------------------------------------------------------------------------------
-template <int PLANES>   // 0: fp32 activations, otherwise the number of 16-bit planes (2 = fp16 parity mode)
+template <int PLANES, bool F16>   // PLANES 0: fp32 activations, otherwise the plane format (kernels.h, PlaneFmt)
 __global__ void __launch_bounds__(256) conv1_1_direct_kernel(PreArgs a, const float* __restrict__ wT /*[27][64]*/, const float* __restrict__ bias,
                                                               void* out, int out_pitch, long long out_plane, int relu) {
     constexpr int TX = 32, TY = 8;
@@ -330,7 +330,7 @@ __global__ void __launch_bounds__(256) conv1_1_direct_kernel(PreArgs a, const fl
         for (int ch = 0; ch < 8; ch++) {
             uint32_t pk[4];
 #pragma unroll
-            for (int j = 0; j < 4; j++) pk[j] = split_pair<planes_are_fp16(PLANES)>(acc[ch * 8 + 2 * j], acc[ch * 8 + 2 * j + 1]);
+            for (int j = 0; j < 4; j++) pk[j] = split_pair<F16>(acc[ch * 8 + 2 * j], acc[ch * 8 + 2 * j + 1]);
             *(uint4*)(stage + lx * 128 + ((ch ^ (lx & 7)) * 16)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
         }
         __syncwarp();
@@ -349,12 +349,12 @@ __global__ void __launch_bounds__(256) conv1_1_direct_kernel(PreArgs a, const fl
 int launch_conv1_1_direct(const PreArgs& a, const float* wT, const float* bias, void* out, int out_pitch, long long out_plane, int relu,
                           int nimages, cudaStream_t st) {
     dim3 g((a.net_w + 31) / 32, (a.net_h + 7) / 8, nimages), b(32, 8);
-    switch (a.planes) {
-        case 0: conv1_1_direct_kernel<0><<<g, b, 0, st>>>(a, wT, bias, out, out_pitch, out_plane, relu); break;
-        case 1: conv1_1_direct_kernel<1><<<g, b, 0, st>>>(a, wT, bias, out, out_pitch, out_plane, relu); break;
-        case 2: conv1_1_direct_kernel<2><<<g, b, 0, st>>>(a, wT, bias, out, out_pitch, out_plane, relu); break;
-        default: conv1_1_direct_kernel<3><<<g, b, 0, st>>>(a, wT, bias, out, out_pitch, out_plane, relu); break;
-    }
+    const PlaneFmt f = a.fmt;
+    if (f.planes == 0) conv1_1_direct_kernel<0, false><<<g, b, 0, st>>>(a, wT, bias, out, out_pitch, out_plane, relu);
+    else if (f.planes == 1 && f.f16) conv1_1_direct_kernel<1, true><<<g, b, 0, st>>>(a, wT, bias, out, out_pitch, out_plane, relu);
+    else if (f.planes == 1) conv1_1_direct_kernel<1, false><<<g, b, 0, st>>>(a, wT, bias, out, out_pitch, out_plane, relu);
+    else if (f.planes == 2) conv1_1_direct_kernel<2, PARITY_F16><<<g, b, 0, st>>>(a, wT, bias, out, out_pitch, out_plane, relu);
+    else conv1_1_direct_kernel<3, false><<<g, b, 0, st>>>(a, wT, bias, out, out_pitch, out_plane, relu);
     return 1;
 }
 

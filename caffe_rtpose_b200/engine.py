@@ -20,6 +20,7 @@ LIB_PATH = os.environ.get("PE_LIB") or os.path.join(HERE, "libposeengine.so")
 MPI_15, COCO_18 = 0, 1
 PREC_FP32_SIMT, PREC_BF16X1, PREC_BF16X2, PREC_BF16X3 = 0, 1, 2, 3
 PREC_F16X2 = PREC_BF16X2   # the parity mode: 2 fp16 planes, chunked round-to-nearest accumulation (poseengine.h)
+PREC_F16X1 = 4             # the fast mode: the parity mode's hi plane alone, one MMA per MAC (poseengine.h)
 MAX_PEOPLE = 96
 
 _f32p = np.ctypeslib.ndpointer(dtype=np.float32, flags="C_CONTIGUOUS")
@@ -33,6 +34,11 @@ class _Config(C.Structure):
 
 class PoseEngineError(RuntimeError):
     pass
+
+
+class _ResultDiff(C.Structure):
+    _fields_ = [("identical", C.c_int), ("parts_count_differ", C.c_int), ("peaks_moved", C.c_int), ("persons_matched", C.c_int),
+                ("max_joint_dist", C.c_float)]
 
 
 _lib = None
@@ -51,6 +57,7 @@ ABI_SYMBOLS = [
     "pe_caffemodel_last_error", "pe_create_from_prototxt", "pe_plan_describe", "pe_render_device", "pe_host_alloc", "pe_host_free", "pe_forward_camera_frames", "pe_broadcast_weights", "pe_render", "pe_encode_jpeg", "pe_decode_jpeg", "pe_decode_png",
     "pe_video_open", "pe_video_close", "pe_video_info", "pe_video_read", "pe_video_last_error",
     "pe_camera_open", "pe_camera_close", "pe_camera_info", "pe_camera_grab", "pe_camera_last_error", "pe_yuyv_to_bgr",
+    "pe_compare_results",
 ]
 
 
@@ -106,6 +113,8 @@ def lib():
     L.pe_host_alloc.restype = C.c_void_p
     L.pe_host_free.argtypes = [C.c_void_p]
     L.pe_write_json.argtypes = [_f32p, C.c_int, C.c_int, C.c_double, C.c_char_p, C.c_int]
+    L.pe_compare_results.argtypes = [C.c_void_p, C.c_int, _f32p, C.c_void_p, C.c_int, _f32p, C.c_int, C.c_int, C.c_float,
+                                     C.POINTER(_ResultDiff)]
     for f in ("pe_model_num_parts", "pe_model_num_limbs"):
         getattr(L, f).argtypes = [C.c_int]
     for f in ("pe_model_limb_sequence", "pe_model_map_idx"):
@@ -543,6 +552,30 @@ def write_caffemodel(path, weights, table, legacy_v1=False, legacy_dims=False):
             net += _pb_len(100, _pb_len(1, ("relu_" + name).encode()) + _pb_len(2, b"ReLU"))   # blob-less layer, ignored
     with open(path, "wb") as f:
         f.write(net)
+
+
+def compare_results(a, b, tol_px):
+    """pe_compare_results of two results of one frame, each (num_people, joints, peaks) as PoseEngine.fetch returns it:
+    equal peak counts per part with every peak within tol_px, equal person counts, person i of a with the same present parts
+    as person i of b and every joint within tol_px.  Joints are in display pixels and peaks in net pixels, both compared
+    against tol_px.  Returns a dict with identical, parts_count_differ, peaks_moved, persons_matched, max_joint_dist."""
+    (na, ja, pa), (nb, jb, pb) = a, b
+    pa = np.ascontiguousarray(pa, np.float32)
+    pb = np.ascontiguousarray(pb, np.float32)
+    if pa.shape != pb.shape or pa.ndim != 3 or pa.shape[2] != 3:
+        raise ValueError("peaks must both be (num_parts, max_peaks + 1, 3), got %s and %s" % (pa.shape, pb.shape))
+    num_parts, max_peaks = pa.shape[0], pa.shape[1] - 1
+    ja = np.ascontiguousarray(np.asarray(ja, np.float32).reshape(-1, num_parts, 3)[:na])
+    jb = np.ascontiguousarray(np.asarray(jb, np.float32).reshape(-1, num_parts, 3)[:nb])
+    if ja.shape[0] != na or jb.shape[0] != nb:
+        raise ValueError("fewer joint rows than people")
+    d = _ResultDiff()
+    rc = lib().pe_compare_results(ja.ctypes.data_as(C.c_void_p), int(na), pa, jb.ctypes.data_as(C.c_void_p), int(nb), pb,
+                                  num_parts, max_peaks, float(tol_px), C.byref(d))
+    if rc != 0:
+        raise PoseEngineError("pe_compare_results failed (%d)" % rc)
+    return {"identical": bool(d.identical), "parts_count_differ": d.parts_count_differ, "peaks_moved": d.peaks_moved,
+            "persons_matched": d.persons_matched, "max_joint_dist": float(d.max_joint_dist)}
 
 
 def share_weights(src, dst):

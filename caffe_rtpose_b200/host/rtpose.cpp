@@ -83,13 +83,17 @@ static void define_flags() {
     define("synthetic", "0", "[extension] process N procedurally generated frames instead of a camera/video/image_dir");
     define("random_init", "", "[extension] 'he' or 'caffe': random weights instead of --caffemodel (no checkpoint offline)");
     define("model", "", "[extension] COCO or MPI when --caffeproto is not readable");
-    define("precision", "2", "[extension] conv arithmetic: 0 fp32 SIMT, 1 bf16, 2 split-bf16 parity mode");
+    define("precision", "2", "[extension] conv arithmetic: 0 fp32 SIMT, 1 bf16 (A/B only), 2 parity mode (two fp16 planes, 3 MMAs per MAC), "
+           "3 three bf16 planes (A/B only), 4 fast mode (one fp16 plane, 1 MMA per MAC; see --audit_every)");
     define("batch", "0", "[extension] frames per forward per GPU: 1 = the reference's behaviour, 0 = automatic (file / synthetic sources "
            "fill two waves of 128-row tiles on the GPU, e.g. 9 frames at 656x368; results do not depend on it)");
     define("engines_per_gpu", "0", "[extension] worker handles per GPU: 1 = the reference's topology (one Net per GPU), 0 = automatic (2 when "
            "--batch is automatic: the copies and the kernel tails of one batch overlap the other; weights are shared, not duplicated)");
-    define("calibrate_range", "true", "[extension] parity mode: derive per-layer power-of-two activation scales from one synthetic frame at start-up "
+    define("calibrate_range", "true", "[extension] fp16 modes (--precision 2 and 4): derive per-layer power-of-two activation scales from one synthetic frame at start-up "
            "(pe_calibrate), so that a model of any magnitude keeps fp32-level results", true);
+    define("audit_every", "0", "[extension] N > 0: every worker also holds a parity-mode (--precision 2) handle and forwards every N-th batch "
+           "through it too; each frame's peaks, person count and joints are compared with the fast handle's (within 1e-3 net px). The status "
+           "line reports how many frames agree, and a summary is printed at exit. Output stays the --precision handle's. 0 = off");
     define("num_writers", "0", "[extension] threads that format / encode and write the --write_json and --write_frames files (a quality-98 720p JPEG takes ~20 ms to encode): "
            "1 = on the display thread like the reference, 0 = automatic (a quarter of the host's cores, at most 16)");
     define("keys_from_stdin", "false", "[extension] read the reference's runtime keys (- = _ + [ ] { } ; ' , . 0-9 q-p a s, ESC or Q to quit) from stdin", true);
@@ -390,6 +394,10 @@ struct Global {
     std::atomic<bool> googly_eyes{false}, video_paused{false};
     std::atomic<int> seek_delta{0};
     int queue_limit = 64, batch = 1, engines_per_gpu = 1;
+    // --audit_every: frames compared with the parity mode, how many were identical, the largest joint distance (display px)
+    std::mutex audit_mutex;
+    long long audit_frames = 0, audit_identical = 0;
+    float audit_max_joint = 0.f;
 } global;
 
 // --image_dir frame: .jpg / .png decode straight into a page-locked buffer of the pool; other formats (and an exhausted pool) go
@@ -618,21 +626,21 @@ static int load_weights(pe_engine* e, int device) {   // CopyTrainedLayersFrom (
 // packs it and the replicas receive the packed buffer by one ncclBroadcast (the path's only collective).
 // engines[g * per_gpu + k] = handle k of GPU g.  Handle 0 of GPU 0 loads the model; handle 0 of the other GPUs receives the packed
 // weights by broadcast; handles k > 0 share their GPU's buffer (Net::ShareTrainedLayersWith).
-static bool create_engines(int num_gpu, int per_gpu, std::vector<pe_engine*>& engines) {
+static bool create_engines(int num_gpu, int per_gpu, int precision, std::vector<pe_engine*>& engines) {
     const int batch = global.batch;
     for (int tid = 0; tid < num_gpu * per_gpu; tid++) {
         pe_config c;
         memset(&c, 0, sizeof c);
         c.device = Fi("start_device") + tid / per_gpu; c.model = global.model; c.net_w = global.net_w; c.net_h = global.net_h;
         c.disp_w = global.disp_w; c.disp_h = global.disp_h; c.num_scales = Fi("num_scales");
-        c.start_scale = Fd("start_scale"); c.scale_gap = Fd("scale_gap"); c.max_batch = batch; c.precision = Fi("precision");
+        c.start_scale = Fd("start_scale"); c.scale_gap = Fd("scale_gap"); c.max_batch = batch; c.precision = precision;
         pe_engine* e = nullptr;
         const int rc = global.proto_readable ? pe_create_from_prototxt(&c, F("caffeproto").c_str(), &e) : pe_create(&c, &e);
         if (rc) { LOG_ERROR("GPU %d: %s", c.device, pe_last_error(nullptr)); return false; }
         engines.push_back(e);
     }
     if (load_weights(engines[0], Fi("start_device"))) return false;
-    if (Fb("calibrate_range") && Fi("precision") == 2) {   // before the weights are replicated: the scales travel inside the packed buffer
+    if (Fb("calibrate_range") && (precision == PE_PREC_F16X2 || precision == PE_PREC_F16X1)) {   // before the weights are replicated: the scales travel inside the packed buffer
         std::vector<uint8_t> probe;
         synthetic_frame(0, global.disp_w, global.disp_h, probe);
         const uint8_t* ptr = probe.data();
@@ -656,7 +664,24 @@ static bool create_engines(int num_gpu, int per_gpu, std::vector<pe_engine*>& en
     return true;
 }
 
-static void worker(int tid, pe_engine* e) {
+// --audit_every: frame i of the last forward of `e` against the parity handle `ref` (same frames)
+static bool audit_frame(pe_engine* e, pe_engine* ref, int i, const std::vector<float>& joints, int cnt, const std::vector<float>& peaks) {
+    const int P = pe_nms_get_num_parts(e), MP = pe_nms_get_max_peaks(e);
+    std::vector<float> rj((size_t)PE_MAX_PEOPLE * P * 3), rp((size_t)P * (MP + 1) * 3);
+    int rcnt = 0;
+    if (pe_fetch(ref, i, rj.data(), &rcnt, rp.data())) return false;
+    // the north-star bar (DESIGN.md section 6): 1e-3 net px, in display px for the joints
+    const float tol = 1e-3f * (float)std::max((double)global.disp_w / global.net_w, (double)global.disp_h / global.net_h);
+    pe_result_diff d;
+    if (pe_compare_results(joints.data(), cnt, peaks.data(), rj.data(), rcnt, rp.data(), P, MP, tol, &d)) return false;
+    std::lock_guard<std::mutex> l(global.audit_mutex);
+    global.audit_frames++;
+    global.audit_identical += d.identical;
+    global.audit_max_joint = std::max(global.audit_max_joint, d.max_joint_dist);
+    return true;
+}
+
+static void worker(int tid, pe_engine* e, pe_engine* ref) {
     const int device = Fi("start_device") + tid / global.engines_per_gpu, batch = global.batch;
     struct Done { ~Done() { global.finished++; global.output_queue.wake(); } } done_guard;   // every exit path counts
     caffe::NmsLayer<float> nms_layer(e);
@@ -666,7 +691,9 @@ static void worker(int tid, pe_engine* e) {
     LOG_INFO("GPU %d is ready (model %s, max_peaks %d, %d frame(s) per forward)", device, nms_layer.GetNumParts() == 15 ? "MPI" : "COCO",
              nms_layer.GetMaxPeaks(), batch);
     const int P = nms_layer.GetNumParts();
-    std::vector<float> joints((size_t)PE_MAX_PEOPLE * P * 3);
+    std::vector<float> joints((size_t)PE_MAX_PEOPLE * P * 3), peaks((size_t)P * (nms_layer.GetMaxPeaks() + 1) * 3);
+    const int audit_every = ref ? Fi("audit_every") : 0;
+    long long batches = 0;
     Frame pending;
     bool pending_valid = false;
     int seen_version = -1;
@@ -710,9 +737,18 @@ static void worker(int tid, pe_engine* e) {
         else frc = pe_forward_camera_frames(e, ptrs.data(), (int)ptrs.size(), frames[0].w, frames[0].h, &scale);   // warpAffine on the GPU
         for (auto& f : frames) f.scale = scale;
         if (frc) { LOG_ERROR("GPU %d: %s", device, pe_last_error(e)); global.failed = global.quit = true; break; }
+        const bool audit = audit_every > 0 && batches++ % audit_every == 0;
+        if (audit) {   // the same frames through the parity handle; its results are only compared, never written
+            if (frames[0].w == global.disp_w && frames[0].h == global.disp_h) frc = pe_forward_frames(ref, ptrs.data(), (int)ptrs.size());
+            else frc = pe_forward_camera_frames(ref, ptrs.data(), (int)ptrs.size(), frames[0].w, frames[0].h, &scale);
+            if (frc) { LOG_ERROR("GPU %d (audit): %s", device, pe_last_error(ref)); global.failed = global.quit = true; break; }
+        }
         for (size_t i = 0; i < frames.size(); i++) {
             int cnt = 0;
-            if (pe_fetch(e, (int)i, joints.data(), &cnt, nullptr)) { LOG_ERROR("GPU %d: %s", device, pe_last_error(e)); global.failed = global.quit = true; break; }
+            if (pe_fetch(e, (int)i, joints.data(), &cnt, audit ? peaks.data() : nullptr)) { LOG_ERROR("GPU %d: %s", device, pe_last_error(e)); global.failed = global.quit = true; break; }
+            if (audit && !audit_frame(e, ref, (int)i, joints, cnt, peaks)) {
+                LOG_ERROR("GPU %d (audit): %s", device, pe_last_error(ref)); global.failed = global.quit = true; break;
+            }
             frames[i].num_people = cnt;
             frames[i].joints.assign(joints.begin(), joints.begin() + (size_t)cnt * P * 3);
             if (!F("write_frames").empty()) {   // render() + postProcessFrame (rtpose.cpp:271-300, 1286-1296) on the GPU
@@ -910,6 +946,11 @@ static void orderer_and_writer(int num_workers) {
                      30.0 / (t - last));
             fps_now = 30.0 / (t - last);
             last = t;
+            if (Fi("audit_every") > 0) {
+                std::lock_guard<std::mutex> l(global.audit_mutex);
+                LOG_INFO("Audit: %lld/%lld frames identical, max joint \xce\x94 %.3g px", global.audit_identical, global.audit_frames,
+                         (double)global.audit_max_joint);
+            }
         }
     };
     while (true) {
@@ -935,6 +976,9 @@ static void orderer_and_writer(int num_workers) {
     writers.finish();   // every image is on disk before the run reports its end
     const double dt = now_s() - t0;
     LOG_INFO("Done, exiting. # frames: %d  (%.1f frames/s overall, %d dropped)", written, written / std::max(dt, 1e-9), global.dropped.load());
+    if (Fi("audit_every") > 0)
+        LOG_INFO("Audit summary: %lld/%lld audited frames identical to the parity mode, max joint \xce\x94 %.3g px (every %d-th batch)",
+                 global.audit_identical, global.audit_frames, (double)global.audit_max_joint, Fi("audit_every"));
 }
 
 static bool ensure_dir(const std::string& d) {
@@ -970,6 +1014,11 @@ int main(int argc, char** argv) {
         LOG_INFO("Camera %d: %dx%d %s", Fi("camera"), global.camera_w, global.camera_h, cc);
     }
     if (F("frame_format") != "jpg" && F("frame_format") != "bmp") { LOG_ERROR("--frame_format must be jpg or bmp"); return 1; }
+    if (Fi("audit_every") < 0) { LOG_ERROR("--audit_every must be 0 (off) or a positive number of batches"); return 1; }
+    if (Fi("audit_every") > 0 && Fi("precision") == PE_PREC_F16X2) {
+        LOG_ERROR("--audit_every compares a faster precision with the parity mode; with --precision 2 there is nothing to compare");
+        return 1;
+    }
     if (sscanf(F("resolution").c_str(), "%dx%d", &global.disp_w, &global.disp_h) != 2) { LOG_ERROR("Error, resolution format (%s) invalid, should be e.g., 960x540", F("resolution").c_str()); return 1; }
     if (sscanf(F("net_resolution").c_str(), "%dx%d", &global.net_w, &global.net_h) != 2) { LOG_ERROR("Error, net resolution format (%s) invalid, should be e.g., 656x368 (multiples of 16)", F("net_resolution").c_str()); return 1; }
     if (!F("image_dir").empty()) {   // readImageDirIfFlagEnabled (rtpose.cpp:1732-1755): sorted list of image files
@@ -1032,20 +1081,23 @@ int main(int argc, char** argv) {
     if (Fb("keys_from_stdin")) std::thread(key_reader).detach();   // blocks in getchar(): never joined
     if (Fb("decode_bench")) return decode_bench();
     const int num_gpu = std::max(1, Fi("num_gpu"));
-    std::vector<pe_engine*> engines;
+    std::vector<pe_engine*> engines, audit;
     const int per_gpu = global.engines_per_gpu, num_workers = num_gpu * per_gpu;
-    if (!create_engines(num_gpu, per_gpu, engines)) {
+    if (!create_engines(num_gpu, per_gpu, Fi("precision"), engines) ||
+        (Fi("audit_every") > 0 && !create_engines(num_gpu, per_gpu, PE_PREC_F16X2, audit))) {
         for (pe_engine* e : engines) pe_destroy(e);
+        for (pe_engine* e : audit) pe_destroy(e);
         return 1;
     }
     std::vector<std::thread> workers;
-    for (int i = 0; i < num_workers; i++) workers.emplace_back(worker, i, engines[i]);
+    for (int i = 0; i < num_workers; i++) workers.emplace_back(worker, i, engines[i], audit.empty() ? nullptr : audit[i]);
     std::thread prod(run_producers);
     std::thread ord(orderer_and_writer, num_workers);
     prod.join();
     for (auto& t : workers) t.join();
     ord.join();
     for (pe_engine* e : engines) pe_destroy(e);
+    for (pe_engine* e : audit) pe_destroy(e);
     g_pinned.clear();
     pe_video_close(global.video);
     pe_camera_close(global.camera);

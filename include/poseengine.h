@@ -22,7 +22,7 @@ extern "C" {
 #define PE_ERR_CUDA 2      /* CUDA runtime / driver failure (message in pe_last_error) */
 #define PE_ERR_STATE 3     /* call out of order (e.g. forward before weights) */
 #define PE_ERR_IO 4        /* file could not be read / parsed */
-#define PE_ERR_RANGE 5     /* parity mode: a layer's values left the range of the fp16 planes (see pe_calibrate) */
+#define PE_ERR_RANGE 5     /* fp16 modes: a layer's values left the range of the fp16 planes (see pe_calibrate) */
 
 #define PE_MODEL_MPI_15 0  /* ModelDescriptorFactory::Type::MPI_15  (modelDescriptorFactory.h:16-19) */
 #define PE_MODEL_COCO_18 1 /* ModelDescriptorFactory::Type::COCO_18 */
@@ -37,6 +37,12 @@ extern "C" {
 #define PE_PREC_BF16X2 PE_PREC_F16X2 /* historical name of the parity mode (its planes were bf16 at first) */
 #define PE_PREC_BF16X3 3    /* wgmma, 3 bf16 planes, 6 MMAs: hi*hi chunked as in mode 2, the 5 cross products in a second
                              * accumulator (bf16 planes carry fewer bits: LESS accurate than mode 2) */
+#define PE_PREC_F16X1 4     /* wgmma FAST mode: the parity mode's hi plane alone - one fp16 plane (11 bits) of activations and
+                             * weights, 1 MMA per MAC, the same per-layer power-of-two weight / range scales (pe_calibrate) and the
+                             * same chunked round-to-nearest fp32 accumulation.  Each layer's output is rounded to fp16 (unit
+                             * roundoff 2^-11): 1.5e-3 - 2.4e-3 of the map range over the whole net against 1.7e-2 for
+                             * PE_PREC_BF16X1 at the same cost, 1.9x the parity mode's frames/s (H100 80GB HBM3, 700 W; DESIGN.md
+                             * sections 5, 6).  pe_compare_results measures what that does to the poses. */
 
 #define PE_MAX_PEOPLE 96   /* RENDER_MAX_PEOPLE, renderFunctions.h:6 / rtpose.cpp:88 */
 
@@ -91,7 +97,8 @@ int pe_caffemodel_blob(const pe_caffemodel* m, int layer, int blob, const float*
 const char* pe_caffemodel_last_error(void);
 /* pack + upload; must be called once after the weights are set and before any forward */
 int pe_commit_weights(pe_engine* e);
-/* Range management of the parity mode (PE_PREC_F16X2).  Its activation planes are fp16 x power-of-two scale per layer; the default
+/* Range management of the fp16 modes (PE_PREC_F16X2, PE_PREC_F16X1; a no-op in the others).  Their activation planes are fp16 x
+ * power-of-two scale per layer; the default
  * scale 1 suits the trained pose models.  pe_calibrate runs one forward on the given HOST frames layer by layer, measures every
  * layer's largest |output| in fp32 and sets the scales so that the stored maxima sit in [32, 64) - after that a net of any
  * magnitude (e.g. the prototxt's gaussian(0.01) filler, whose maps are ~3e-11) keeps fp32-level parity.  Exact: scales are powers
@@ -162,6 +169,23 @@ void pe_host_free(void* p);
 
 /* JSON writer of displayFrame (rtpose.cpp:1383-1416).  Returns the text length (writes if < cap). */
 int pe_write_json(const float* joints, int num_people, int num_parts, double frame_scale, char* buf, int cap);
+
+/* Result comparison of two fetched results of one frame (host only, no GPU), e.g. the fast mode against the parity mode.
+ * joints_*: people_* x num_parts x 3 as pe_fetch returns them; peaks_*: num_parts x (max_peaks+1) x 3 (count in [part][0][0]).
+ * Distances are Euclidean in the units of the inputs (display pixels for pe_fetch).  The results are identical when
+ *   - every part has the same peak count in a and b, and peak k of a part lies within tol_px of peak k of b;
+ *   - the person counts are equal;
+ *   - person i of a has the same present parts (score > 0) as person i of b, each joint within tol_px.
+ * Returns PE_OK, or PE_ERR_INVALID for bad arguments. */
+typedef struct pe_result_diff {
+    int identical;          /* 1 when all three conditions hold */
+    int parts_count_differ; /* parts whose peak count differs */
+    int peaks_moved;        /* peaks (of parts with equal counts) farther than tol_px from their counterpart */
+    int persons_matched;    /* persons i < min(people_a, people_b) with the same present parts */
+    float max_joint_dist;   /* largest joint distance over the matched persons */
+} pe_result_diff;
+int pe_compare_results(const float* joints_a, int people_a, const float* peaks_a, const float* joints_b, int people_b,
+                       const float* peaks_b, int num_parts, int max_peaks, float tol_px, pe_result_diff* out);
 
 /* ---- renderers: render() (rtpose.cpp:271-300) + render_mpi_parts / render_coco_parts / render_coco_aff
  * (src/rtpose/renderFunctions.cu:331-389, 978-1080) on the display frame `idx` of the last forward, followed by the
