@@ -16,6 +16,7 @@
 #include "common.h"
 #include "kernels.h"
 #include "conv_tc.h"
+#include "jpeg_coefs.h"
 #include "prototxt.h"
 
 // NVTX ranges (header-only nvtx3: resolved at run time, no-ops without a profiler attached) around the phases of a forward, so that
@@ -86,6 +87,9 @@ struct pe_engine {
     int warp_w = 0, warp_h = 0; double warp_scale = 1.0;
     int *d_wa = nullptr, *d_wb = nullptr, *d_wx0 = nullptr, *d_wy0 = nullptr; short* d_wtab = nullptr;
     bool input_lo_dirty = false;
+    // JPEG coefficient images (pe_forward_jpeg_coefs): device copies, pinned staging for pageable callers, component planes
+    uint8_t* d_jcoef = nullptr; size_t jcoef_cap = 0; uint8_t* h_jcoef = nullptr; size_t h_jcoef_cap = 0;
+    uint8_t* d_jplanes = nullptr; size_t jplanes_cap = 0;
     // renderers: canvas, uint8 image, heat-map scratch (allocated on first pe_render); display frames of the last forward
     float* d_canvas = nullptr; uint8_t* d_render_u8 = nullptr; uint8_t* d_render_src = nullptr; float* d_heat = nullptr; size_t heat_cap = 0;
     const uint8_t* last_frames = nullptr;
@@ -414,6 +418,7 @@ extern "C" void pe_destroy(pe_engine* e) {
     for (void* p : e->acts) if (p) cudaFree(p);
     for (void* p : e->d_tabs) cudaFree(p);
     for (auto& t : e->tc) tc_layer_destroy(t);
+    cudaFree(e->d_jcoef); cudaFreeHost(e->h_jcoef); cudaFree(e->d_jplanes);
     cudaFree(e->d_raw); cudaFreeHost(e->h_raw); cudaFree(e->d_wa); cudaFree(e->d_wb); cudaFree(e->d_wx0); cudaFree(e->d_wy0); cudaFree(e->d_wtab);
     e->packed_owner.reset(); cudaFree(e->d_range); cudaFree(e->d_frames); cudaFree(e->d_resized); cudaFree(e->d_planar); cudaFree(e->d_maps);
     cudaFreeHost(e->h_frames); cudaFreeHost(e->h_planar); cudaFreeHost(e->h_maps);
@@ -1121,6 +1126,75 @@ extern "C" int pe_forward_camera_frames(pe_engine* e, const uint8_t* const* fram
     w.src = e->d_raw; w.dst = e->d_frames; w.sw = orig_w; w.sh = orig_h; w.dw = e->cfg.disp_w; w.dh = e->cfg.disp_h;
     w.adelta = e->d_wa; w.bdelta = e->d_wb; w.x0 = e->d_wx0; w.y0 = e->d_wy0; w.tab = e->d_wtab;
     e->launches += launch_warp_affine(w, n, e->stream);
+    return pe_forward_frames_device(e, e->d_frames, n);
+}
+
+// (re)allocates *p to hold at least `need` bytes; the stream is drained first because queued work may still use the old buffer
+static int grow_buffer(pe_engine* e, uint8_t** p, size_t* cap, size_t need, bool host) {
+    if (*cap >= need) return PE_OK;
+    CK(e, cudaStreamSynchronize(e->stream));
+    if (host) { cudaFreeHost(*p); *p = nullptr; CK(e, cudaMallocHost((void**)p, need)); }
+    else { cudaFree(*p); *p = nullptr; CK(e, cudaMalloc((void**)p, need)); }
+    *cap = need;
+    return PE_OK;
+}
+
+extern "C" int pe_forward_jpeg_coefs(pe_engine* e, const void* const* coefs, int n, double* scale) {
+    NvtxRange r("pe_forward_jpeg_coefs (H2D + reconstruction)");
+    int rc = check_n(e, n); if (rc) return rc;
+    if (!coefs) return fail(e, PE_ERR_INVALID, "null coefficient images");
+    CK(e, cudaSetDevice(e->cfg.device));
+    // the kernels index with the headers' numbers: every header must be one pe_jpeg_read_coefs writes, all frames one size
+    int W = 0, H = 0;
+    long long max_bytes = 0, max_blocks = 0;
+    std::vector<long long> bytes(n);
+    for (int i = 0; i < n; i++) {
+        if (!coefs[i]) return fail(e, PE_ERR_INVALID, "null coefficient image %d", i);
+        pe_jpeg_coef_header hd;
+        memcpy(&hd, coefs[i], sizeof hd);
+        if (!pe_jpeg::coef_header_valid(hd)) return fail(e, PE_ERR_INVALID, "coefficient image %d: not a pe_jpeg_read_coefs header", i);
+        if (i == 0) { W = hd.width; H = hd.height; }
+        else if (hd.width != W || hd.height != H)
+            return fail(e, PE_ERR_INVALID, "coefficient image %d is %dx%d, frame 0 %dx%d: one size per call", i, hd.width, hd.height, W, H);
+        bytes[i] = hd.total_bytes;
+        max_bytes = std::max(max_bytes, (long long)hd.total_bytes);
+        max_blocks = std::max(max_blocks, (long long)(hd.total_bytes - (long long)sizeof hd) / 128);
+    }
+    const bool display = W == e->cfg.disp_w && H == e->cfg.disp_h;
+    uint8_t* dst = e->d_frames;
+    if (!display) {   // reconstructed at the original size into the warpAffine source, as pe_forward_camera_frames uploads it
+        rc = prepare_warp(e, W, H); if (rc) return rc;
+        rc = grow_buffer(e, &e->d_raw, &e->raw_cap, (size_t)W * H * 3 * e->cfg.max_batch, false); if (rc) return rc;
+        dst = e->d_raw;
+    }
+    if (scale) *scale = display ? 1.0 : e->warp_scale;
+    const size_t stride = ((size_t)max_bytes + 255) & ~(size_t)255, pstride = ((size_t)max_blocks * 64 + 255) & ~(size_t)255;
+    rc = grow_buffer(e, &e->d_jcoef, &e->jcoef_cap, stride * n, false); if (rc) return rc;
+    rc = grow_buffer(e, &e->d_jplanes, &e->jplanes_cap, pstride * n, false); if (rc) return rc;
+    // page-locked caller buffers (pe_host_alloc) are DMA'd directly; pageable ones are staged, which drains the stream
+    bool pinned = true;
+    for (int i = 0; i < n && pinned; i++) {
+        cudaPointerAttributes at;
+        if (cudaPointerGetAttributes(&at, coefs[i]) != cudaSuccess || at.type != cudaMemoryTypeHost) { pinned = false; cudaGetLastError(); }
+    }
+    if (pinned) {
+        for (int i = 0; i < n; i++) CK(e, cudaMemcpyAsync(e->d_jcoef + i * stride, coefs[i], bytes[i], cudaMemcpyHostToDevice, e->stream));
+    } else {
+        CK(e, cudaStreamSynchronize(e->stream));
+        rc = grow_buffer(e, &e->h_jcoef, &e->h_jcoef_cap, stride * n, true); if (rc) return rc;
+        for (int i = 0; i < n; i++) memcpy(e->h_jcoef + i * stride, coefs[i], bytes[i]);
+        CK(e, cudaMemcpyAsync(e->d_jcoef, e->h_jcoef, stride * n, cudaMemcpyHostToDevice, e->stream));
+    }
+    JpegArgs ja;
+    ja.coefs = e->d_jcoef; ja.coef_stride = (long long)stride; ja.planes = e->d_jplanes; ja.plane_stride = (long long)pstride;
+    ja.dst = dst; ja.W = W; ja.H = H; ja.n = n; ja.max_blocks = max_blocks;
+    e->launches += launch_jpeg_reconstruct(ja, e->stream);
+    if (!display) {
+        WarpArgs w;
+        w.src = e->d_raw; w.dst = e->d_frames; w.sw = W; w.sh = H; w.dw = e->cfg.disp_w; w.dh = e->cfg.disp_h;
+        w.adelta = e->d_wa; w.bdelta = e->d_wb; w.x0 = e->d_wx0; w.y0 = e->d_wy0; w.tab = e->d_wtab;
+        e->launches += launch_warp_affine(w, n, e->stream);
+    }
     return pe_forward_frames_device(e, e->d_frames, n);
 }
 

@@ -20,8 +20,11 @@
 // the 64-bit scalar form, so corrupt data decodes identically too), and row-wise fused upsampling + colour conversion.  Anything
 // unusual (second scan, failure, no AVX2) re-runs the general route, whose result is the definition.  PE_JPEG_FAST=0 disables
 // the fast route (tests compare the two).
+// pe_jpeg_read_coefs stops after the entropy stage: both routes store the coefficient image (jpeg_coefs.h) instead of transforming
+// it, and the GPU reconstructs the pixels (jpeg_gpu.cu); pe_jpeg_coefs_to_bgr is the same reconstruction on the host.
 // Host code, no GPU.
 #include "jpeg_tables.h"
+#include "jpeg_coefs.h"
 #include <stdint.h>
 #include <stdlib.h>
 #include <string.h>
@@ -556,7 +559,16 @@ static void output_rows(const std::vector<Comp>& comps, int hmax, int vmax, int 
     output_rows_impl<false>(comps, hmax, vmax, W, H, bgr);
 }
 
-static int decode_impl(const uint8_t* data, long long size, int* w, int* h, uint8_t* bgr, long long cap, bool allow_fast);
+// Coefficient output of pe_jpeg_read_coefs: the entropy stage alone, its result stored instead of transformed
+struct CoefOut {
+    uint8_t* buf;       // NULL: only the size is wanted
+    long long cap;
+    pe_jpeg_coef_header hdr;
+    short* coef(int k) const { return (short*)(buf + hdr.comp[k].offset); }
+};
+
+static int decode_impl(const uint8_t* data, long long size, int* w, int* h, uint8_t* bgr, long long cap, bool allow_fast, CoefOut* co = nullptr);
+static void reconstruct(std::vector<Comp>& comps, int hmax, int vmax, int W, int H, uint8_t* bgr);
 
 }  // namespace
 
@@ -568,7 +580,7 @@ extern "C" int pe_decode_jpeg(const uint8_t* data, long long size, int* w, int* 
 }
 
 namespace {
-static int decode_impl(const uint8_t* data, long long size, int* w, int* h, uint8_t* bgr, long long cap, bool allow_fast) {
+static int decode_impl(const uint8_t* data, long long size, int* w, int* h, uint8_t* bgr, long long cap, bool allow_fast, CoefOut* co) {
     if (!data || size < 4 || data[0] != 0xFF || data[1] != 0xD8) return -1;
     uint16_t quant[4][64];
     bool quant_set[4] = {false, false, false, false};
@@ -636,8 +648,17 @@ static int decode_impl(const uint8_t* data, long long size, int* w, int* h, uint
             have_sof = true;
             if (w) *w = W;
             if (h) *h = H;
-            if (!bgr) return 0;
-            if (cap < (long long)W * H * 3) return -1;
+            if (!bgr && !co) return 0;
+            if (bgr && cap < (long long)W * H * 3) return -1;
+            if (co) {   // the same geometry as below, written into the header
+                pe_jpeg_coef_header& hd = co->hdr;
+                memset(&hd, 0, sizeof hd);
+                hd.magic = PE_JPEG_COEF_MAGIC; hd.width = W; hd.height = H; hd.num_comps = nc;
+                for (int i = 0; i < nc; i++) { hd.comp[i].h = comps[i].h; hd.comp[i].v = comps[i].v; }
+                if (!pe_jpeg::coef_layout(hd)) return -2;
+                if (!co->buf) return 0;
+                if (co->cap < hd.total_bytes) return -1;
+            }
             mcux = (W + 8 * hmax - 1) / (8 * hmax); mcuy = (H + 8 * vmax - 1) / (8 * vmax);
             for (auto& c : comps) {
                 c.bw = mcux * c.h; c.bh = mcuy * c.v;
@@ -697,7 +718,7 @@ static int decode_impl(const uint8_t* data, long long size, int* w, int* h, uint
                 if ((need_dc && sp.Ah == 0 && !dc[c->td].set) || (need_ac && !ac[c->ta].set)) return -1;
                 c->pred = 0;
             }
-            if (fast_done) return decode_impl(data, size, w, h, bgr, cap, false);   // more scans after a complete one: the general route decides
+            if (fast_done) return decode_impl(data, size, w, h, bgr, cap, false, co);   // more scans after a complete one: the general route decides
             // interleaved: MCUs of h x v blocks per component over the padded grid; single component: its real blocks
             const int units_x = ns > 1 ? mcux : sc[0]->nbw, units_y = ns > 1 ? mcuy : sc[0]->nbh;
             bool distinct = true;   // a (corrupt) scan that names a component twice accumulates coefficients: general route only
@@ -705,7 +726,8 @@ static int decode_impl(const uint8_t* data, long long size, int* w, int* h, uint
                 for (int j = i + 1; j < ns; j++) distinct = distinct && sc[i] != sc[j];
             if (allow_fast && !progressive && !any_scan && distinct && ns == (int)comps.size()) {
                 // ---- fast route: one interleaved sequential scan, every block transformed as it leaves the entropy decoder
-                for (auto& c : comps) c.plane.resize((size_t)c.pw * c.ph);
+                if (!co)
+                    for (auto& c : comps) c.plane.resize((size_t)c.pw * c.ph);
                 FastBits fb;
                 fb.p = p + len; fb.end = end;
                 int until = restart;
@@ -727,15 +749,17 @@ static int decode_impl(const uint8_t* data, long long size, int* w, int* h, uint
                             for (int by = 0; by < nby && ok; by++)
                                 for (int bx = 0; bx < nbx && ok; bx++) {
                                     const int col = ux * nbx + bx, rowb = uy * nby + by;
-                                    memset(blk, 0, sizeof blk);
+                                    // coefficient output: the block goes straight into the caller's buffer, untransformed
+                                    short* dst = co ? co->coef((int)(c - comps.data())) + ((size_t)rowb * c->bw + col) * 64 : blk;
+                                    memset(dst, 0, 64 * sizeof(short));
                                     bool dc_only = false;
-                                    ok = decode_block_seq(fb, c->pred, dc[c->td], ac[c->ta], blk, dc_only);
-                                    if (ok) idct_block(blk, c->q, c->plane.data() + (size_t)rowb * 8 * c->pw + (size_t)col * 8, c->pw, dc_only);
+                                    ok = decode_block_seq(fb, c->pred, dc[c->td], ac[c->ta], dst, dc_only);
+                                    if (ok && !co) idct_block(blk, c->q, c->plane.data() + (size_t)rowb * 8 * c->pw + (size_t)col * 8, c->pw, dc_only);
                                 }
                         }
                         if (restart) until--;
                     }
-                if (!ok) return decode_impl(data, size, w, h, bgr, cap, false);   // the general route defines the outcome of broken streams
+                if (!ok) return decode_impl(data, size, w, h, bgr, cap, false, co);   // the general route defines the outcome of broken streams
                 fast_done = any_scan = true;
                 p = fb.p;
                 continue;
@@ -776,8 +800,21 @@ static int decode_impl(const uint8_t* data, long long size, int* w, int* h, uint
         p += len;
     }
     if (!have_sof) return -1;
-    if (!bgr) return 0;
+    if (!bgr && !co) return 0;
     if (!any_scan) return -1;
+    if (co) {   // coefficient output: what the loop below would transform, and the tables it would use
+        for (size_t k = 0; k < comps.size(); k++) {
+            Comp& c = comps[k];
+            if (!c.q_latched) { if (!quant_set[c.tq]) return -1; memcpy(c.q, quant[c.tq], sizeof c.q); }
+            memcpy(co->hdr.comp[k].quant, c.q, sizeof c.q);
+            if (fast_done) continue;   // already stored by the fast route
+            const size_t n = (size_t)c.bw * c.bh * 64;
+            if (c.coef.empty()) memset(co->coef((int)k), 0, n * sizeof(short));
+            else memcpy(co->coef((int)k), c.coef.data(), n * sizeof(short));
+        }
+        memcpy(co->buf, &co->hdr, sizeof co->hdr);
+        return 0;
+    }
     for (auto& c : comps) {   // inverse DCT of every block (a component without any scan decodes as mid-grey, like libjpeg)
         if (fast_done) break;   // already transformed
         if (!c.q_latched) { if (!quant_set[c.tq]) return -1; memcpy(c.q, quant[c.tq], sizeof c.q); }
@@ -787,6 +824,12 @@ static int decode_impl(const uint8_t* data, long long size, int* w, int* h, uint
             for (int bx = 0; bx < c.bw; bx++)
                 idct_block(&c.coef[((size_t)by * c.bw + bx) * 64], c.q, c.plane.data() + (size_t)by * 8 * c.pw + (size_t)bx * 8, c.pw, false);
     }
+    reconstruct(comps, hmax, vmax, W, H, bgr);
+    return 0;
+}
+
+// planes (every block transformed) -> BGR: grey replicated, or upsampled chroma + colour conversion
+static void reconstruct(std::vector<Comp>& comps, int hmax, int vmax, int W, int H, uint8_t* bgr) {
     const int nc = (int)comps.size();
     if (nc == 1) {
         const Comp& c = comps[0];
@@ -796,10 +839,41 @@ static int decode_impl(const uint8_t* data, long long size, int* w, int* h, uint
                 uint8_t* o = bgr + ((size_t)y * W + x) * 3;
                 o[0] = o[1] = o[2] = g;
             }
-        return 0;
+        return;
     }
     output_rows(comps, hmax, vmax, W, H, bgr);
-    return 0;
 }
 }  // namespace
+
+extern "C" long long pe_jpeg_read_coefs(const uint8_t* data, long long size, void* buf, long long cap) {
+    const char* env = getenv("PE_JPEG_FAST");
+    CoefOut co;
+    co.buf = (uint8_t*)buf;
+    co.cap = cap;
+    memset(&co.hdr, 0, sizeof co.hdr);
+    const int rc = decode_impl(data, size, nullptr, nullptr, nullptr, 0, !(env && env[0] == '0'), &co);
+    return rc ? rc : co.hdr.total_bytes;
+}
+
+extern "C" int pe_jpeg_coefs_to_bgr(const void* coefs, uint8_t* bgr, long long cap) {
+    if (!coefs || !bgr) return -1;
+    pe_jpeg_coef_header hd;
+    memcpy(&hd, coefs, sizeof hd);
+    if (!pe_jpeg::coef_header_valid(hd) || cap < (long long)hd.width * hd.height * 3) return -1;
+    std::vector<Comp> comps(hd.num_comps);
+    for (int k = 0; k < hd.num_comps; k++) {
+        Comp& c = comps[k];
+        const pe_jpeg_coef_comp& h = hd.comp[k];
+        c.h = h.h; c.v = h.v; c.bw = h.bw; c.bh = h.bh; c.dw = h.dw; c.dh = h.dh;
+        c.pw = c.bw * 8; c.ph = c.bh * 8;
+        memcpy(c.q, h.quant, sizeof c.q);
+        c.plane.assign((size_t)c.pw * c.ph, 0);
+        const short* coef = (const short*)((const uint8_t*)coefs + h.offset);
+        for (int by = 0; by < c.bh; by++)
+            for (int bx = 0; bx < c.bw; bx++)
+                idct_block(coef + ((size_t)by * c.bw + bx) * 64, c.q, c.plane.data() + (size_t)by * 8 * c.pw + (size_t)bx * 8, c.pw, false);
+    }
+    reconstruct(comps, hd.hmax, hd.vmax, hd.width, hd.height, bgr);
+    return 0;
+}
 

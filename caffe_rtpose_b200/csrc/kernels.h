@@ -115,6 +115,16 @@ int launch_warp_affine(const WarpArgs& a, int nframes, cudaStream_t st);
 // planar fp32 net input [N][3][H][W] -> im2col'ed input
 int launch_input_from_planar(const float* planar, const PreArgs& a, int nimages, cudaStream_t st);
 
+// ---- JPEG reconstruction (jpeg_gpu.cu): coefficient images of pe_jpeg_read_coefs -> BGR frames
+struct JpegArgs {
+    const uint8_t* coefs; long long coef_stride;    // [n] coefficient images (pe_jpeg_coef_header + int16), 256-byte aligned
+    uint8_t* planes; long long plane_stride;        // [n] component planes: byte 64 * b + k = sample k of block b (coefficient order)
+    uint8_t* dst;                                   // [n][H][W][3] uint8 BGR
+    int W, H, n;
+    long long max_blocks;                           // largest block count of a frame in the batch
+};
+int launch_jpeg_reconstruct(const JpegArgs& a, cudaStream_t st);   // dequantise + IDCT, then upsample + colour: 2 launches
+
 // ---- convolution / pooling (conv_simt.cu, conv_tc.cu, pool.cu)
 int launch_conv_simt(const ConvArgs& a, cudaStream_t st);
 struct PoolArgs {

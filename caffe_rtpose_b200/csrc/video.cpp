@@ -206,3 +206,22 @@ extern "C" int pe_video_read(const pe_video* v, int index, uint8_t* bgr, long lo
     }
     return PE_OK;
 }
+
+extern "C" long long pe_video_read_coefs(const pe_video* v, int index, void* buf, long long cap) {
+    if (!v) { g_video_error = "null argument"; return -PE_ERR_INVALID; }
+    if (!v->mjpeg) { g_video_error = v->path + ": not a Motion-JPEG video"; return -PE_ERR_INVALID; }
+    if (index < 0 || index >= (int)v->frames.size()) { g_video_error = "frame index outside the video"; return -PE_ERR_INVALID; }
+    while (index > 0 && v->frames[index].size == 0) index--;   // a zero-length chunk repeats the previous frame, as in pe_video_read
+    const FrameRef fr = v->frames[index];
+    if (fr.size == 0) { g_video_error = v->path + ": the video starts with an empty frame (pe_video_read gives it as black)"; return -PE_ERR_INVALID; }
+    std::vector<uint8_t> data;
+    try { data.resize(fr.size); } catch (...) { g_video_error = v->path + ": out of memory for a frame"; return -PE_ERR_IO; }
+    if (!v->read_at(fr.off, data.data(), fr.size)) { g_video_error = v->path + ": read error"; return -PE_ERR_IO; }
+    int jw = 0, jh = 0;
+    const int hrc = pe_decode_jpeg(data.data(), (long long)data.size(), &jw, &jh, nullptr, 0);   // frame header only
+    long long rc = hrc ? hrc : pe_jpeg_read_coefs(data.data(), (long long)data.size(), nullptr, 0);
+    if (rc > 0 && (jw != v->w || jh != v->h)) rc = -1;   // pe_video_read's rule: every frame has the video's size
+    if (rc > 0 && buf && cap >= rc && pe_jpeg_read_coefs(data.data(), (long long)data.size(), buf, cap) != rc) rc = -1;
+    if (rc <= 0) { g_video_error = v->path + ": frame " + std::to_string(index) + " is not a decodable JPEG"; return rc == -2 ? -PE_ERR_INVALID : -PE_ERR_IO; }
+    return rc;
+}

@@ -57,7 +57,7 @@ ABI_SYMBOLS = [
     "pe_caffemodel_last_error", "pe_create_from_prototxt", "pe_plan_describe", "pe_render_device", "pe_host_alloc", "pe_host_free", "pe_forward_camera_frames", "pe_broadcast_weights", "pe_render", "pe_encode_jpeg", "pe_decode_jpeg", "pe_decode_png",
     "pe_video_open", "pe_video_close", "pe_video_info", "pe_video_read", "pe_video_last_error",
     "pe_camera_open", "pe_camera_close", "pe_camera_info", "pe_camera_grab", "pe_camera_last_error", "pe_yuyv_to_bgr",
-    "pe_compare_results",
+    "pe_compare_results", "pe_jpeg_read_coefs", "pe_jpeg_coefs_to_bgr", "pe_forward_jpeg_coefs", "pe_video_read_coefs",
 ]
 
 
@@ -140,6 +140,10 @@ def lib():
     L.pe_encode_jpeg.restype = C.c_longlong
     L.pe_decode_jpeg.argtypes = [C.c_char_p, C.c_longlong, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p, C.c_longlong]
     L.pe_decode_png.argtypes = L.pe_decode_jpeg.argtypes
+    L.pe_jpeg_read_coefs.argtypes = [C.c_char_p, C.c_longlong, C.c_void_p, C.c_longlong]
+    L.pe_jpeg_read_coefs.restype = C.c_longlong
+    L.pe_jpeg_coefs_to_bgr.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong]
+    L.pe_forward_jpeg_coefs.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.POINTER(C.c_double)]
     if hasattr(L, "pe_video_open") or "PE_LIB" not in os.environ:   # an older A/B build (PE_LIB) may predate the video reader
         L.pe_video_open.argtypes = [C.c_char_p, C.POINTER(C.c_void_p)]
         L.pe_video_close.argtypes = [C.c_void_p]
@@ -348,6 +352,17 @@ class PoseEngine:
         self._keep = frames
         s = C.c_double()
         self._ck(lib().pe_forward_camera_frames(self._h, ptrs, len(frames), w, h, C.byref(s)))
+        return s.value
+
+    def forward_jpeg(self, jpegs):
+        """jpegs: list of JPEG files (bytes) of one common size.  Only the entropy stage runs on the host (read_jpeg_coefs); the
+        GPU reconstructs the pixels, byte-identical to decode_jpeg, and then runs as forward_frames (display size) or
+        forward_camera_frames (any other size).  Returns frame.scale."""
+        bufs = [j if isinstance(j, np.ndarray) else read_jpeg_coefs(j) for j in jpegs]
+        ptrs = (C.c_void_p * len(bufs))(*[b.ctypes.data for b in bufs])
+        self._keep = bufs
+        s = C.c_double()
+        self._ck(lib().pe_forward_jpeg_coefs(self._h, ptrs, len(bufs), C.byref(s)))
         return s.value
 
     def render(self, idx=0, part_to_show=0, googly_eyes=False, display_bgr=None, want_canvas=False):
@@ -615,6 +630,51 @@ def decode_jpeg(data):
     rc = lib().pe_decode_jpeg(data, len(data), C.byref(w), C.byref(h), out.ctypes.data, out.size)
     if rc != 0:
         raise PoseEngineError("pe_decode_jpeg failed (%d)" % rc)
+    return out
+
+
+def _jpeg_error(fn, rc):
+    return PoseEngineError("%s: %s" % (fn, "not a JPEG / truncated" if rc == -1 else "unsupported JPEG variant (arithmetic / lossless / 12-bit / CMYK / unusual sampling)"))
+
+
+def read_jpeg_coefs(data):
+    """Entropy stage of decode_jpeg: the coefficient image (pe_jpeg_coef_header + int16 coefficients, poseengine.h) as a uint8
+    array, the input of PoseEngine.forward_jpeg."""
+    n = lib().pe_jpeg_read_coefs(data, len(data), None, 0)
+    if n < 0:
+        raise _jpeg_error("pe_jpeg_read_coefs", n)
+    buf = np.zeros(n, np.uint8)
+    rc = lib().pe_jpeg_read_coefs(data, len(data), buf.ctypes.data, n)
+    if rc != n:
+        raise _jpeg_error("pe_jpeg_read_coefs", rc)
+    return buf
+
+
+def jpeg_coef_header(buf):
+    """The header fields of a coefficient image: dict with width, height, num_comps, hmax, vmax, total_bytes and comps, a list of
+    dicts (h, v, bw, bh, dw, dh, offset, quant) per component."""
+    b = np.asarray(buf, np.uint8)
+    i32, i64 = b[:32].view(np.int32), b[:32].view(np.int64)
+    out = {"magic": int(b[:4].view(np.uint32)[0]), "width": int(i32[1]), "height": int(i32[2]), "num_comps": int(i32[3]),
+           "hmax": int(i32[4]), "vmax": int(i32[5]), "total_bytes": int(i64[3]), "comps": []}
+    for k in range(out["num_comps"]):
+        c = b[32 + 160 * k:32 + 160 * (k + 1)]
+        f = c[:24].view(np.int32)
+        out["comps"].append({"h": int(f[0]), "v": int(f[1]), "bw": int(f[2]), "bh": int(f[3]), "dw": int(f[4]), "dh": int(f[5]),
+                             "offset": int(c[24:32].view(np.int64)[0]), "quant": c[32:].view(np.uint16).reshape(8, 8).copy()})
+    return out
+
+
+def jpeg_coefs_to_bgr(buf):
+    """Host reconstruction of a coefficient image with decode_jpeg's own IDCT / upsampling / colour code (the reference of the
+    GPU kernels)."""
+    buf = np.ascontiguousarray(buf, np.uint8)
+    if buf.size < 512 or jpeg_coef_header(buf)["total_bytes"] > buf.size:
+        raise PoseEngineError("pe_jpeg_coefs_to_bgr: truncated coefficient image")
+    hd = jpeg_coef_header(buf)
+    out =np.zeros((max(hd["height"], 0), max(hd["width"], 0), 3), np.uint8)
+    if lib().pe_jpeg_coefs_to_bgr(buf.ctypes.data, out.ctypes.data, out.size) != 0:
+        raise PoseEngineError("pe_jpeg_coefs_to_bgr: malformed coefficient image")
     return out
 
 

@@ -56,6 +56,9 @@ static void define_flags() {
     define("num_producers", "0", "[extension] decoder threads for --image_dir / --synthetic: 1 = the reference's single producer, 0 = automatic "
            "(with automatic --batch: 10 per GPU, at most 48 and the host's cores minus the worker threads - one H100 consumes 200-300 frames/s, a thread decodes ~100)");
     define("decode_bench", "false", "[extension] run only the producer stage (decode + queue), print frames/s, exit (no GPU)", true);
+    define("gpu_decode", "false", "[extension] JPEG sources (--image_dir .jpg files, Motion-JPEG --video): the producer threads run only the "
+           "entropy (Huffman) stage; dequantisation, IDCT, chroma upsampling and colour conversion run on the GPU (pixels identical to the host "
+           "decoder). Other files and JPEGs it does not take are decoded on the host as without it", true);
     define("frame_format", "jpg", "[extension] jpg (quality 98, as the reference) or bmp (lossless) for --write_frames");
     define("no_frame_drops", "false", "Dont drop frames.", true);
     define("write_json", "", "Write joint data with json format as prefix%06d.json");
@@ -151,6 +154,7 @@ struct Frame {
     double scale = 1.0;                      // display / original (rtpose.cpp:474-480), filled by the engine
     std::vector<uint8_t> bgr;                // display image, HWC BGR (decode buffer)
     std::shared_ptr<uint8_t> pinned;         // same image in page-locked memory (pe_host_alloc) for direct async DMA
+    bool coefs = false;                      // --gpu_decode: `pinned` holds the JPEG's coefficient image (pe_jpeg_read_coefs), not pixels
     std::string stem;                        // for <stem>.json with --image_dir
     int num_people = 0;
     std::vector<float> joints;
@@ -465,9 +469,49 @@ static int source_frame_count() {
     if (global.camera) return 0x7fffffff;   // until ESC / a capture error
     return (int)global.image_list.size();
 }
+// --gpu_decode: frame i of --image_dir / a Motion-JPEG --video as a coefficient image in a page-locked buffer of the pool (the
+// reconstruction runs on the GPU, pe_forward_jpeg_coefs).  false: not a JPEG, or one the coefficient stage refuses: the caller
+// decodes the frame on the host instead, which also reports what is wrong with it.
+static bool fetch_coefs(int i, Frame& fr) {
+    std::vector<uint8_t> data;
+    if (!global.video) {
+        FILE* f = fopen(global.image_list[i].c_str(), "rb");
+        if (!f) return false;
+        fseek(f, 0, SEEK_END);
+        const long n = ftell(f);
+        fseek(f, 0, SEEK_SET);
+        data.resize((size_t)std::max(n, 0L));
+        const bool rd = n > 4 && fread(data.data(), 1, (size_t)n, f) == (size_t)n;
+        fclose(f);
+        if (!rd || data[0] != 0xFF || data[1] != 0xD8) return false;
+    }
+    auto read = [&](void* buf, long long cap) {
+        return global.video ? pe_video_read_coefs(global.video, i, buf, cap) : pe_jpeg_read_coefs(data.data(), (long long)data.size(), buf, cap);
+    };
+    const long long n = read(nullptr, 0);
+    if (n <= (long long)sizeof(pe_jpeg_coef_header) || n > (3LL << 28)) return false;
+    uint8_t* ph = g_pinned.get((size_t)n);   // without page-locked memory the engine stages the copy (as for pixel frames)
+    if (ph) fr.pinned = std::shared_ptr<uint8_t>(ph, [n](uint8_t* q) { g_pinned.put(q, (size_t)n); });
+    else { fr.bgr.resize((size_t)n); ph = fr.bgr.data(); }
+    pe_jpeg_coef_header hd;
+    if (read(ph, n) != n) { fr.pinned.reset(); std::vector<uint8_t>().swap(fr.bgr); return false; }
+    memcpy(&hd, ph, sizeof hd);
+    fr.w = hd.width; fr.h = hd.height;
+    fr.coefs = true;
+    return true;
+}
+
 // frame i of the source (synthetic / --video / --image_dir) into fr; false: could not be decoded (message logged)
 static bool fetch_source_frame(int i, Frame& fr) {
     int w = global.disp_w, h = global.disp_h;
+    if (Fb("gpu_decode") && (global.video || !global.image_list.empty()) && !global.camera && Fi("synthetic") <= 0 && fetch_coefs(i, fr)) {
+        if (!global.video) {
+            const std::string& p = global.image_list[i];
+            const size_t slash = p.find_last_of('/'), dot = p.find_last_of('.');
+            fr.stem = p.substr(slash == std::string::npos ? 0 : slash + 1, dot - (slash == std::string::npos ? 0 : slash + 1));
+        }
+        return true;
+    }
     if (Fi("synthetic") > 0) {
         synthetic_frame(i, w, h, fr.bgr);
     } else if (global.camera) {   // cap >> image_uchar_orig from the capture device
@@ -712,7 +756,7 @@ static void worker(int tid, pe_engine* e, pe_engine* ref) {
                 global.dropped++;
                 continue;
             }
-            if (!frames.empty() && (fr.w != frames[0].w || fr.h != frames[0].h)) {   // one forward = one frame size
+            if (!frames.empty() && (fr.w != frames[0].w || fr.h != frames[0].h || fr.coefs != frames[0].coefs)) {   // one forward = one frame size and kind
                 pending = std::move(fr); pending_valid = true;
                 break;
             }
@@ -731,16 +775,18 @@ static void worker(int tid, pe_engine* e, pe_engine* ref) {
         }
         std::vector<const uint8_t*> ptrs;
         for (auto& f : frames) ptrs.push_back(f.pinned ? f.pinned.get() : f.bgr.data());
-        int frc;
         double scale = 1.0;
-        if (frames[0].w == global.disp_w && frames[0].h == global.disp_h) frc = pe_forward_frames(e, ptrs.data(), (int)ptrs.size());
-        else frc = pe_forward_camera_frames(e, ptrs.data(), (int)ptrs.size(), frames[0].w, frames[0].h, &scale);   // warpAffine on the GPU
+        auto forward = [&](pe_engine* h) {
+            if (frames[0].coefs) return pe_forward_jpeg_coefs(h, (const void* const*)ptrs.data(), (int)ptrs.size(), &scale);   // GPU JPEG reconstruction
+            if (frames[0].w == global.disp_w && frames[0].h == global.disp_h) return pe_forward_frames(h, ptrs.data(), (int)ptrs.size());
+            return pe_forward_camera_frames(h, ptrs.data(), (int)ptrs.size(), frames[0].w, frames[0].h, &scale);   // warpAffine on the GPU
+        };
+        int frc = forward(e);
         for (auto& f : frames) f.scale = scale;
         if (frc) { LOG_ERROR("GPU %d: %s", device, pe_last_error(e)); global.failed = global.quit = true; break; }
         const bool audit = audit_every > 0 && batches++ % audit_every == 0;
         if (audit) {   // the same frames through the parity handle; its results are only compared, never written
-            if (frames[0].w == global.disp_w && frames[0].h == global.disp_h) frc = pe_forward_frames(ref, ptrs.data(), (int)ptrs.size());
-            else frc = pe_forward_camera_frames(ref, ptrs.data(), (int)ptrs.size(), frames[0].w, frames[0].h, &scale);
+            frc = forward(ref);
             if (frc) { LOG_ERROR("GPU %d (audit): %s", device, pe_last_error(ref)); global.failed = global.quit = true; break; }
         }
         for (size_t i = 0; i < frames.size(); i++) {
@@ -998,6 +1044,10 @@ int main(int argc, char** argv) {
         for (uint8_t b : px) { hash ^= b; hash *= 1099511628211ull; }
         printf("%dx%d %016llx\n", w, h, (unsigned long long)hash);
         return 0;
+    }
+    if (Fb("gpu_decode") && (Fi("synthetic") > 0 || (F("video").empty() && F("image_dir").empty()))) {
+        LOG_ERROR("--gpu_decode reconstructs JPEG files on the GPU: it needs --image_dir or a Motion-JPEG --video (not --synthetic or a camera)");
+        return 1;
     }
     if (F("video").empty() && F("image_dir").empty() && Fi("synthetic") <= 0) {   // the camera (rtpose.cpp:401-405, 1694-1695)
         int cw = 0, ch = 0;

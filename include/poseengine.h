@@ -139,6 +139,11 @@ int pe_forward_frames(pe_engine* e, const uint8_t* const* frames, int n);
  * produced on the GPU (OpenCV's fixed-point arithmetic, bit-exact), then as pe_forward_frames.  *scale receives
  * frame.scale (the JSON writer multiplies joints by 1/scale, rtpose.cpp:1384,1399-1400). */
 int pe_forward_camera_frames(pe_engine* e, const uint8_t* const* frames, int n, int orig_w, int orig_h, double* scale);
+/* n JPEG frames of one size as coefficient images (pe_jpeg_read_coefs): copied to the GPU (asynchronously when they were allocated
+ * with pe_host_alloc), reconstructed there byte-identically to pe_decode_jpeg, then as pe_forward_frames when the frames are
+ * disp_w x disp_h (*scale = 1) and as pe_forward_camera_frames otherwise (GPU warpAffine, *scale = frame.scale).  pe_render
+ * with display_bgr == NULL draws on the reconstructed display frame. */
+int pe_forward_jpeg_coefs(pe_engine* e, const void* const* coefs, int n, double* scale);
 /* same, frames already resident in device memory (n consecutive disp_h*disp_w*3 images) */
 int pe_forward_frames_device(pe_engine* e, const void* d_frames, int n);
 /* HOST net input as the reference uploads it: n x num_scales x 3 x net_h x net_w fp32 planar
@@ -219,6 +224,36 @@ long long pe_encode_jpeg(const uint8_t* bgr, int w, int h, int quality, uint8_t*
  * cap >= w*h*3.  -1: not a JPEG / truncated; -2: arithmetic-coded, lossless, 12-bit, CMYK or unusual chroma sampling. */
 int pe_decode_jpeg(const uint8_t* data, long long size, int* w, int* h, uint8_t* bgr, long long cap);
 
+/* ---- JPEG decoding split between host and GPU: the host does only the entropy (Huffman) stage and hands the coefficient image
+ * to pe_forward_jpeg_coefs, whose kernels do dequantisation + islow IDCT, fancy chroma upsampling and YCbCr->BGR with
+ * pe_decode_jpeg's arithmetic (the pixels are byte-identical).
+ * Coefficient image = this 512-byte header followed by the components' int16 coefficients, one after the other (component k
+ * at comp[k].offset, comp[0].offset == sizeof(pe_jpeg_coef_header)), each [bh][bw][64] in natural (row-major) order over the
+ * MCU-padded block grid: exactly the values libjpeg's IDCT receives. */
+#define PE_JPEG_COEF_MAGIC 0x4345504Au /* "JPEC" */
+typedef struct pe_jpeg_coef_comp {
+    int32_t h, v;        /* sampling factors (1, 1 for a grey image) */
+    int32_t bw, bh;      /* blocks per row / column of the MCU-padded plane */
+    int32_t dw, dh;      /* real samples of the (downsampled) plane: ceil(width * h / hmax) x ceil(height * v / vmax) */
+    int64_t offset;      /* bytes from the start of the buffer to the coefficients */
+    uint16_t quant[64];  /* dequantisation table, natural order */
+} pe_jpeg_coef_comp;
+typedef struct pe_jpeg_coef_header {
+    uint32_t magic;      /* PE_JPEG_COEF_MAGIC */
+    int32_t width, height;
+    int32_t num_comps;   /* 1 (grey) or 3 (YCbCr) */
+    int32_t hmax, vmax;  /* largest sampling factors: the MCU is 8*hmax x 8*vmax pixels */
+    int64_t total_bytes; /* header + coefficients */
+    pe_jpeg_coef_comp comp[3];
+} pe_jpeg_coef_header;
+/* Entropy stage of pe_decode_jpeg: the coefficient image of a JPEG (host only, thread-safe).  Accepts exactly the files
+ * pe_decode_jpeg accepts.  buf == NULL: returns the size needed (parses up to the frame header only).  Otherwise returns the
+ * size written; -1 = not a JPEG / truncated / corrupt, or cap too small; -2 = a variant pe_decode_jpeg does not handle. */
+long long pe_jpeg_read_coefs(const uint8_t* data, long long size, void* buf, long long cap);
+/* host reconstruction of a coefficient image (the same IDCT / upsampling / colour code as pe_decode_jpeg): the reference the GPU
+ * kernels are tested against.  Returns 0 and writes width x height x 3 uint8 BGR when cap suffices; -1 = malformed buffer / cap. */
+int pe_jpeg_coefs_to_bgr(const void* coefs, uint8_t* bgr, long long cap);
+
 /* same for .png (the third format the reference lists, rtpose.cpp:1743): inflate + PNG filters / Adam7 / all colour types and
  * bit depths, converted as cv::imread(IMREAD_COLOR) does (8-bit BGR, alpha dropped, 16-bit -> high byte). */
 int pe_decode_png(const uint8_t* data, long long size, int* w, int* h, uint8_t* bgr, long long cap);
@@ -233,6 +268,10 @@ int pe_video_open(const char* path, pe_video** out);
 void pe_video_close(pe_video* v);
 int pe_video_info(const pe_video* v, int* w, int* h, double* fps, int* frame_count, char fourcc[5]);
 int pe_video_read(const pe_video* v, int index, uint8_t* bgr, long long cap);
+/* Motion-JPEG videos: frame `index` as a coefficient image (pe_jpeg_read_coefs) for pe_forward_jpeg_coefs.  Returns its size; it is
+ * written when buf != NULL and cap >= size (call again with a larger buffer otherwise).  -PE_ERR_INVALID: not a Motion-JPEG video,
+ * bad index, a JPEG variant the decoder does not handle; -PE_ERR_IO: unreadable / corrupt frame (text in pe_video_last_error()). */
+long long pe_video_read_coefs(const pe_video* v, int index, void* buf, long long cap);
 const char* pe_video_last_error(void);
 
 /* cv::VideoCapture on a camera index (rtpose.cpp:401-405 cap.open(FLAGS_camera) + CV_CAP_PROP_FRAME_WIDTH/HEIGHT from
