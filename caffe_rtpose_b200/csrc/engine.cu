@@ -17,6 +17,8 @@
 #include "kernels.h"
 #include "conv_tc.h"
 #include "jpeg_coefs.h"
+#include "jpeg_entropy.cuh"
+#include <climits>
 #include "prototxt.h"
 
 // NVTX ranges (header-only nvtx3: resolved at run time, no-ops without a profiler attached) around the phases of a forward, so that
@@ -90,6 +92,11 @@ struct pe_engine {
     // JPEG coefficient images (pe_forward_jpeg_coefs): device copies, pinned staging for pageable callers, component planes
     uint8_t* d_jcoef = nullptr; size_t jcoef_cap = 0; uint8_t* h_jcoef = nullptr; size_t h_jcoef_cap = 0;
     uint8_t* d_jplanes = nullptr; size_t jplanes_cap = 0;
+    // JPEG scan images (pe_forward_jpeg_scans): device copies, pinned staging, the decoder's work space, per-frame status
+    uint8_t* d_jscan = nullptr; size_t jscan_cap = 0; uint8_t* h_jscan = nullptr; size_t h_jscan_cap = 0;
+    uint8_t* d_jwork = nullptr; size_t jwork_cap = 0;
+    uint8_t* h_jstatus = nullptr; size_t h_jstatus_cap = 0;
+    int jstatus_n = 0;   // frames of the last forward whose status h_jstatus holds (0: the last forward was not from scan images)
     // renderers: canvas, uint8 image, heat-map scratch (allocated on first pe_render); display frames of the last forward
     float* d_canvas = nullptr; uint8_t* d_render_u8 = nullptr; uint8_t* d_render_src = nullptr; float* d_heat = nullptr; size_t heat_cap = 0;
     const uint8_t* last_frames = nullptr;
@@ -419,6 +426,7 @@ extern "C" void pe_destroy(pe_engine* e) {
     for (void* p : e->d_tabs) cudaFree(p);
     for (auto& t : e->tc) tc_layer_destroy(t);
     cudaFree(e->d_jcoef); cudaFreeHost(e->h_jcoef); cudaFree(e->d_jplanes);
+    cudaFree(e->d_jscan); cudaFreeHost(e->h_jscan); cudaFree(e->d_jwork); cudaFreeHost(e->h_jstatus);
     cudaFree(e->d_raw); cudaFreeHost(e->h_raw); cudaFree(e->d_wa); cudaFree(e->d_wb); cudaFree(e->d_wx0); cudaFree(e->d_wy0); cudaFree(e->d_wtab);
     e->packed_owner.reset(); cudaFree(e->d_range); cudaFree(e->d_frames); cudaFree(e->d_resized); cudaFree(e->d_planar); cudaFree(e->d_maps);
     cudaFreeHost(e->h_frames); cudaFreeHost(e->h_planar); cudaFreeHost(e->h_maps);
@@ -876,6 +884,7 @@ static int run_post_and_return(pe_engine* e, int n) {
     CK(e, cudaMemcpyAsync(e->h_peaks, e->post.peaks, sizeof(float) * (size_t)n * P * (MP + 1) * 3, cudaMemcpyDeviceToHost, e->stream));
     CK(e, cudaGetLastError());
     e->last_n = n;
+    e->jstatus_n = 0;
     return PE_OK;
 }
 
@@ -946,6 +955,7 @@ static int run_net(pe_engine* e, int n) {
         CK(e, cudaGraphLaunch(g.exec, e->stream));
         e->launches += g.launches;
         e->last_n = n;
+        e->jstatus_n = 0;
         return PE_OK;
     }
     if (g.seen++ == 0) return run_net_eager(e, n);   // first use of this batch size: eager (sets kernel attributes)
@@ -975,6 +985,7 @@ static int run_net(pe_engine* e, int n) {
     CK(e, cudaGraphLaunch(g.exec, e->stream));
     e->launches += g.launches;
     e->last_n = n;
+    e->jstatus_n = 0;
     return PE_OK;
 }
 
@@ -1139,6 +1150,8 @@ static int grow_buffer(pe_engine* e, uint8_t** p, size_t* cap, size_t need, bool
     return PE_OK;
 }
 
+static int reconstruct_and_forward(pe_engine* e, int n, int W, int H, size_t stride, long long max_blocks, double* scale);
+
 extern "C" int pe_forward_jpeg_coefs(pe_engine* e, const void* const* coefs, int n, double* scale) {
     NvtxRange r("pe_forward_jpeg_coefs (H2D + reconstruction)");
     int rc = check_n(e, n); if (rc) return rc;
@@ -1160,17 +1173,8 @@ extern "C" int pe_forward_jpeg_coefs(pe_engine* e, const void* const* coefs, int
         max_bytes = std::max(max_bytes, (long long)hd.total_bytes);
         max_blocks = std::max(max_blocks, (long long)(hd.total_bytes - (long long)sizeof hd) / 128);
     }
-    const bool display = W == e->cfg.disp_w && H == e->cfg.disp_h;
-    uint8_t* dst = e->d_frames;
-    if (!display) {   // reconstructed at the original size into the warpAffine source, as pe_forward_camera_frames uploads it
-        rc = prepare_warp(e, W, H); if (rc) return rc;
-        rc = grow_buffer(e, &e->d_raw, &e->raw_cap, (size_t)W * H * 3 * e->cfg.max_batch, false); if (rc) return rc;
-        dst = e->d_raw;
-    }
-    if (scale) *scale = display ? 1.0 : e->warp_scale;
-    const size_t stride = ((size_t)max_bytes + 255) & ~(size_t)255, pstride = ((size_t)max_blocks * 64 + 255) & ~(size_t)255;
+    const size_t stride = ((size_t)max_bytes + 255) & ~(size_t)255;
     rc = grow_buffer(e, &e->d_jcoef, &e->jcoef_cap, stride * n, false); if (rc) return rc;
-    rc = grow_buffer(e, &e->d_jplanes, &e->jplanes_cap, pstride * n, false); if (rc) return rc;
     // page-locked caller buffers (pe_host_alloc) are DMA'd directly; pageable ones are staged, which drains the stream
     bool pinned = true;
     for (int i = 0; i < n && pinned; i++) {
@@ -1185,6 +1189,22 @@ extern "C" int pe_forward_jpeg_coefs(pe_engine* e, const void* const* coefs, int
         for (int i = 0; i < n; i++) memcpy(e->h_jcoef + i * stride, coefs[i], bytes[i]);
         CK(e, cudaMemcpyAsync(e->d_jcoef, e->h_jcoef, stride * n, cudaMemcpyHostToDevice, e->stream));
     }
+    return reconstruct_and_forward(e, n, W, H, stride, max_blocks, scale);
+}
+
+// coefficient images in e->d_jcoef (n frames of W x H, `stride` bytes apart) -> display frames -> the net
+static int reconstruct_and_forward(pe_engine* e, int n, int W, int H, size_t stride, long long max_blocks, double* scale) {
+    int rc;
+    const bool display = W == e->cfg.disp_w && H == e->cfg.disp_h;
+    uint8_t* dst = e->d_frames;
+    if (!display) {   // reconstructed at the original size into the warpAffine source, as pe_forward_camera_frames uploads it
+        rc = prepare_warp(e, W, H); if (rc) return rc;
+        rc = grow_buffer(e, &e->d_raw, &e->raw_cap, (size_t)W * H * 3 * e->cfg.max_batch, false); if (rc) return rc;
+        dst = e->d_raw;
+    }
+    if (scale) *scale = display ? 1.0 : e->warp_scale;
+    const size_t pstride = ((size_t)max_blocks * 64 + 255) & ~(size_t)255;
+    rc = grow_buffer(e, &e->d_jplanes, &e->jplanes_cap, pstride * n, false); if (rc) return rc;
     JpegArgs ja;
     ja.coefs = e->d_jcoef; ja.coef_stride = (long long)stride; ja.planes = e->d_jplanes; ja.plane_stride = (long long)pstride;
     ja.dst = dst; ja.W = W; ja.H = H; ja.n = n; ja.max_blocks = max_blocks;
@@ -1196,6 +1216,101 @@ extern "C" int pe_forward_jpeg_coefs(pe_engine* e, const void* const* coefs, int
         e->launches += launch_warp_affine(w, n, e->stream);
     }
     return pe_forward_frames_device(e, e->d_frames, n);
+}
+
+// Scan images -> coefficient images in e->d_jcoef (the entropy kernels), the per-frame status queued into e->h_jstatus.  Everything the
+// kernels index with is checked here first; the launch shapes come from these sizes, so nothing waits for the device.
+static int decode_scans(pe_engine* e, const void* const* scans, int n, int S, int* W, int* H, size_t* cstride, long long* max_blocks) {
+    if (!scans) return fail(e, PE_ERR_INVALID, "null scan images");
+    if (S < 8 || S > (1 << 30)) return fail(e, PE_ERR_INVALID, "subsequence length %d bits outside [8, 2^30]", S);
+    long long max_scan = 0, max_coef = 0, max_seg = 0, max_sub = 0;
+    std::vector<long long> bytes(n);
+    for (int i = 0; i < n; i++) {
+        if (!scans[i]) return fail(e, PE_ERR_INVALID, "null scan image %d", i);
+        const pe_jpeg_scan_header& hd = *(const pe_jpeg_scan_header*)scans[i];
+        long long subs = 0;
+        if (!pe_jpeg::scan_header_valid(hd, S, &subs)) return fail(e, PE_ERR_INVALID, "scan image %d: not a pe_jpeg_read_scan image", i);
+        if (i == 0) { *W = hd.coef.width; *H = hd.coef.height; }
+        else if (hd.coef.width != *W || hd.coef.height != *H)
+            return fail(e, PE_ERR_INVALID, "scan image %d is %dx%d, frame 0 %dx%d: one size per call", i, hd.coef.width, hd.coef.height, *W, *H);
+        bytes[i] = hd.total_bytes;
+        max_scan = std::max(max_scan, (long long)hd.total_bytes);
+        max_coef = std::max(max_coef, (long long)hd.coef.total_bytes);
+        max_blocks[0] = std::max(max_blocks[0], (long long)(hd.coef.total_bytes - (long long)sizeof hd.coef) / 128);
+        max_seg = std::max(max_seg, (long long)hd.num_segments);
+        max_sub = std::max(max_sub, subs);
+    }
+    auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
+    const size_t sstride = al((size_t)max_scan);
+    *cstride = al((size_t)max_coef);
+    const int ctas = (int)((max_sub + pe_jpeg::SYNC_THREADS - 1) / pe_jpeg::SYNC_THREADS);
+    const size_t tab_b = al(jpeg_huff_tables_bytes() * n), seg_b = al((size_t)(max_seg + 1) * 4 * n), pub_b = al((size_t)ctas * 16 * n),
+                 flag_b = al((size_t)ctas * 4 * n), small_b = al((size_t)4 * n);
+    int rc = grow_buffer(e, &e->d_jcoef, &e->jcoef_cap, *cstride * n, false); if (rc) return rc;
+    rc = grow_buffer(e, &e->d_jscan, &e->jscan_cap, sstride * n, false); if (rc) return rc;
+    rc = grow_buffer(e, &e->d_jwork, &e->jwork_cap, tab_b + seg_b + pub_b + flag_b + 2 * small_b, false); if (rc) return rc;
+    rc = grow_buffer(e, &e->h_jstatus, &e->h_jstatus_cap, (size_t)4 * e->cfg.max_batch, true); if (rc) return rc;
+    bool pinned = true;   // page-locked caller buffers (pe_host_alloc) are DMA'd directly; pageable ones are staged, which drains the stream
+    for (int i = 0; i < n && pinned; i++) {
+        cudaPointerAttributes at;
+        if (cudaPointerGetAttributes(&at, scans[i]) != cudaSuccess || at.type != cudaMemoryTypeHost) { pinned = false; cudaGetLastError(); }
+    }
+    if (pinned) {
+        for (int i = 0; i < n; i++) CK(e, cudaMemcpyAsync(e->d_jscan + i * sstride, scans[i], bytes[i], cudaMemcpyHostToDevice, e->stream));
+    } else {
+        CK(e, cudaStreamSynchronize(e->stream));
+        rc = grow_buffer(e, &e->h_jscan, &e->h_jscan_cap, sstride * n, true); if (rc) return rc;
+        for (int i = 0; i < n; i++) memcpy(e->h_jscan + i * sstride, scans[i], bytes[i]);
+        CK(e, cudaMemcpyAsync(e->d_jscan, e->h_jscan, sstride * n, cudaMemcpyHostToDevice, e->stream));
+    }
+    CK(e, cudaMemsetAsync(e->d_jcoef, 0, *cstride * n, e->stream));
+    JpegScanArgs a;
+    a.scans = e->d_jscan; a.scan_stride = (long long)sstride;
+    a.coefs = e->d_jcoef; a.coef_stride = (long long)*cstride;
+    uint8_t* w = e->d_jwork;
+    a.tabs = w; w += tab_b;
+    a.seg_sub = (int*)w; a.seg_stride = max_seg + 1; w += seg_b;
+    a.pub = (unsigned long long*)w; w += pub_b;
+    a.flags = (int*)w; w += flag_b;
+    a.tickets = (int*)w; w += small_b;
+    a.status = (int*)w;
+    a.ctas_max = ctas; a.n = n; a.S = S;
+    e->launches += launch_jpeg_entropy(a, e->stream);
+    CK(e, cudaMemcpyAsync(e->h_jstatus, a.status, (size_t)4 * n, cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaGetLastError());
+    return PE_OK;
+}
+
+extern "C" int pe_forward_jpeg_scans(pe_engine* e, const void* const* scans, int n, double* scale) {
+    NvtxRange r("pe_forward_jpeg_scans (H2D + entropy decoding + reconstruction)");
+    int rc = check_n(e, n); if (rc) return rc;
+    CK(e, cudaSetDevice(e->cfg.device));
+    int W = 0, H = 0;
+    size_t stride = 0;
+    long long max_blocks = 0;
+    rc = decode_scans(e, scans, n, pe_jpeg::SUBSEQ_BITS, &W, &H, &stride, &max_blocks); if (rc) return rc;
+    rc = reconstruct_and_forward(e, n, W, H, stride, max_blocks, scale); if (rc) return rc;
+    e->jstatus_n = n;
+    return PE_OK;
+}
+
+extern "C" int pe_jpeg_decode_scans(pe_engine* e, const void* const* scans, int n, int subseq_bits, void* const* coefs_out, int* status_out) {
+    int rc = check_n(e, n); if (rc) return rc;
+    if (!coefs_out) return fail(e, PE_ERR_INVALID, "null output buffers");
+    CK(e, cudaSetDevice(e->cfg.device));
+    int W = 0, H = 0;
+    size_t stride = 0;
+    long long max_blocks = 0;
+    e->jstatus_n = 0;   // h_jstatus now holds this call's statuses, not those of the last forward
+    rc = decode_scans(e, scans, n, subseq_bits ? subseq_bits : pe_jpeg::SUBSEQ_BITS, &W, &H, &stride, &max_blocks); if (rc) return rc;
+    CK(e, cudaStreamSynchronize(e->stream));
+    for (int i = 0; i < n; i++) {
+        const pe_jpeg_scan_header& hd = *(const pe_jpeg_scan_header*)scans[i];
+        if (!coefs_out[i]) return fail(e, PE_ERR_INVALID, "null output buffer %d", i);
+        CK(e, cudaMemcpy(coefs_out[i], e->d_jcoef + i * stride, (size_t)hd.coef.total_bytes, cudaMemcpyDeviceToHost));
+        if (status_out) { int st; memcpy(&st, e->h_jstatus + 4 * i, 4); status_out[i] = st == INT_MAX ? 0 : 1 + st; }
+    }
+    return PE_OK;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1463,6 +1578,11 @@ extern "C" int pe_fetch(pe_engine* e, int idx, float* joints, int* num_people, f
     if (idx < 0 || idx >= e->last_n) return fail(e, PE_ERR_INVALID, "frame index %d outside the last forward (n=%d)", idx, e->last_n);
     int rc = pe_sync(e); if (rc) return rc;
     if (e->check_range && idx == 0) { rc = pe_range_status(e, nullptr, nullptr); if (rc) return rc; }   // PE_CHECK_RANGE=1: range problems are errors
+    if (idx < e->jstatus_n) {   // a frame from a scan image whose entropy-coded data the host entropy stage rejects
+        int mcu;
+        memcpy(&mcu, e->h_jstatus + 4 * idx, 4);
+        if (mcu != INT_MAX) return fail(e, PE_ERR_IO, "frame %d: corrupt JPEG data (DC category above 15) in MCU %d", idx, mcu);
+    }
     const int P = e->mt->num_parts, MP = e->mt->max_peaks;
     if (num_people) *num_people = e->h_num_people[idx];
     if (joints) memcpy(joints, e->h_joints + (size_t)idx * PE_MAX_PEOPLE * P * 3, sizeof(float) * PE_MAX_PEOPLE * P * 3);

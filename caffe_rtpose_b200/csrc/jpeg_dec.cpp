@@ -25,6 +25,7 @@
 // Host code, no GPU.
 #include "jpeg_tables.h"
 #include "jpeg_coefs.h"
+#include "jpeg_entropy.cuh"
 #include <stdint.h>
 #include <stdlib.h>
 #include <string.h>
@@ -567,7 +568,15 @@ struct CoefOut {
     short* coef(int k) const { return (short*)(buf + hdr.comp[k].offset); }
 };
 
-static int decode_impl(const uint8_t* data, long long size, int* w, int* h, uint8_t* bgr, long long cap, bool allow_fast, CoefOut* co = nullptr);
+// Scan output of pe_jpeg_read_scan: the fast route's scan recorded (tables, restart segments, entropy-coded bytes) instead of decoded
+struct ScanOut {
+    pe_jpeg_scan_header hdr;
+    std::vector<int64_t> seg;   // offset, length per segment, offsets from `data`
+    const uint8_t* data = nullptr;
+};
+
+static int decode_impl(const uint8_t* data, long long size, int* w, int* h, uint8_t* bgr, long long cap, bool allow_fast, CoefOut* co = nullptr,
+                       ScanOut* so = nullptr);
 static void reconstruct(std::vector<Comp>& comps, int hmax, int vmax, int W, int H, uint8_t* bgr);
 
 }  // namespace
@@ -580,7 +589,7 @@ extern "C" int pe_decode_jpeg(const uint8_t* data, long long size, int* w, int* 
 }
 
 namespace {
-static int decode_impl(const uint8_t* data, long long size, int* w, int* h, uint8_t* bgr, long long cap, bool allow_fast, CoefOut* co) {
+static int decode_impl(const uint8_t* data, long long size, int* w, int* h, uint8_t* bgr, long long cap, bool allow_fast, CoefOut* co, ScanOut* so) {
     if (!data || size < 4 || data[0] != 0xFF || data[1] != 0xD8) return -1;
     uint16_t quant[4][64];
     bool quant_set[4] = {false, false, false, false};
@@ -656,8 +665,10 @@ static int decode_impl(const uint8_t* data, long long size, int* w, int* h, uint
                 hd.magic = PE_JPEG_COEF_MAGIC; hd.width = W; hd.height = H; hd.num_comps = nc;
                 for (int i = 0; i < nc; i++) { hd.comp[i].h = comps[i].h; hd.comp[i].v = comps[i].v; }
                 if (!pe_jpeg::coef_layout(hd)) return -2;
-                if (!co->buf) return 0;
-                if (co->cap < hd.total_bytes) return -1;
+                if (!so) {   // (a scan image's size is known only after the whole file)
+                    if (!co->buf) return 0;
+                    if (co->cap < hd.total_bytes) return -1;
+                }
             }
             mcux = (W + 8 * hmax - 1) / (8 * hmax); mcuy = (H + 8 * vmax - 1) / (8 * vmax);
             for (auto& c : comps) {
@@ -718,13 +729,61 @@ static int decode_impl(const uint8_t* data, long long size, int* w, int* h, uint
                 if ((need_dc && sp.Ah == 0 && !dc[c->td].set) || (need_ac && !ac[c->ta].set)) return -1;
                 c->pred = 0;
             }
-            if (fast_done) return decode_impl(data, size, w, h, bgr, cap, false, co);   // more scans after a complete one: the general route decides
+            if (fast_done) return so ? -3 : decode_impl(data, size, w, h, bgr, cap, false, co);   // more scans after a complete one: the general route decides
             // interleaved: MCUs of h x v blocks per component over the padded grid; single component: its real blocks
             const int units_x = ns > 1 ? mcux : sc[0]->nbw, units_y = ns > 1 ? mcuy : sc[0]->nbh;
             bool distinct = true;   // a (corrupt) scan that names a component twice accumulates coefficients: general route only
             for (int i = 0; i < ns; i++)
                 for (int j = i + 1; j < ns; j++) distinct = distinct && sc[i] != sc[j];
-            if (allow_fast && !progressive && !any_scan && distinct && ns == (int)comps.size()) {
+            const bool fast_scan = !progressive && !any_scan && distinct && ns == (int)comps.size();
+            if (so && !fast_scan) return -3;   // valid so far, but not one interleaved sequential scan: the host entropy stage
+            if (so) {
+                // ---- scan output: record the scan instead of decoding it.  Segment boundaries are a property of the bytes:
+                //  * the sequential reader never consumes a marker (it stops at the first FF xx with xx != 00 and feeds zero bits), and
+                //    the restart search starts where the reader stopped, which is at or after the segment's start but never past the
+                //    first such FF.  So segment k begins right after the first FF D0..D7 pair at or after the start of segment k-1;
+                //  * a segment's data ends at the first FF xx (xx != 00) at or after its start - an FF as the file's last byte too;
+                //  * no RST pair where one is due: -1, as on both decoding routes.
+                // The marker loop then continues from the last segment's start: the bytes from there to where the reader would have
+                // stopped are data bytes and FF 00 pairs, which the loop skips, so it reaches the same next marker.
+                pe_jpeg_scan_header& sh = so->hdr;
+                const long long mcus = (long long)mcux * mcuy;
+                const long long nseg = restart ? (mcus + restart - 1) / restart : 1;
+                sh.magic = PE_JPEG_SCAN_MAGIC;
+                sh.num_scan_comps = ns;
+                for (int i = 0; i < ns; i++) {
+                    sh.scan_comp[i] = (int32_t)(sc[i] - comps.data());
+                    sh.dc_table[i] = sc[i]->td;
+                    sh.ac_table[i] = sc[i]->ta;
+                }
+                sh.restart_interval = restart;
+                sh.mcux = mcux; sh.mcuy = mcuy;
+                sh.num_segments = (int32_t)nseg;
+                for (int t = 0; t < 4; t++) {
+                    if (dc[t].set) { memcpy(sh.dc_bits[t], dc[t].bits + 1, 16); memcpy(sh.dc_vals[t], dc[t].vals, 256); }
+                    if (ac[t].set) { memcpy(sh.ac_bits[t], ac[t].bits + 1, 16); memcpy(sh.ac_vals[t], ac[t].vals, 256); }
+                }
+                const uint8_t* start = p + len;
+                so->data = start;
+                so->seg.assign((size_t)(2 * nseg), 0);
+                const uint8_t* q = start;
+                for (long long k = 0; k < nseg; k++) {
+                    if (k > 0) {
+                        while (q + 1 < end && !(q[0] == 0xFF && q[1] >= 0xD0 && q[1] <= 0xD7)) q++;
+                        if (q + 1 >= end) return -1;
+                        q += 2;
+                    }
+                    const uint8_t* e = q;
+                    while (e < end && !(e[0] == 0xFF && (e + 1 >= end || e[1] != 0))) e += e[0] == 0xFF ? 2 : 1;
+                    so->seg[2 * k] = q - start;
+                    so->seg[2 * k + 1] = e - q;
+                }
+                sh.data_bytes = so->seg[2 * nseg - 2] + so->seg[2 * nseg - 1];
+                fast_done = any_scan = true;
+                p = q;
+                continue;
+            }
+            if (allow_fast && fast_scan) {
                 // ---- fast route: one interleaved sequential scan, every block transformed as it leaves the entropy decoder
                 if (!co)
                     for (auto& c : comps) c.plane.resize((size_t)c.pw * c.ph);
@@ -812,6 +871,14 @@ static int decode_impl(const uint8_t* data, long long size, int* w, int* h, uint
             if (c.coef.empty()) memset(co->coef((int)k), 0, n * sizeof(short));
             else memcpy(co->coef((int)k), c.coef.data(), n * sizeof(short));
         }
+        if (so) {
+            pe_jpeg_scan_header& sh = so->hdr;
+            sh.coef = co->hdr;
+            sh.seg_table_offset = (int64_t)sizeof sh;
+            sh.data_offset = sh.seg_table_offset + (int64_t)(so->seg.size() * sizeof(int64_t));
+            sh.total_bytes = sh.data_offset + sh.data_bytes;
+            return 0;
+        }
         memcpy(co->buf, &co->hdr, sizeof co->hdr);
         return 0;
     }
@@ -853,6 +920,128 @@ extern "C" long long pe_jpeg_read_coefs(const uint8_t* data, long long size, voi
     memset(&co.hdr, 0, sizeof co.hdr);
     const int rc = decode_impl(data, size, nullptr, nullptr, nullptr, 0, !(env && env[0] == '0'), &co);
     return rc ? rc : co.hdr.total_bytes;
+}
+
+extern "C" long long pe_jpeg_read_scan(const uint8_t* data, long long size, void* buf, long long cap) {
+    CoefOut co;
+    co.buf = nullptr;
+    co.cap = 0;
+    memset(&co.hdr, 0, sizeof co.hdr);
+    ScanOut so;
+    memset(&so.hdr, 0, sizeof so.hdr);
+    const int rc = decode_impl(data, size, nullptr, nullptr, nullptr, 0, true, &co, &so);
+    if (rc) return rc;
+    const pe_jpeg_scan_header& sh = so.hdr;
+    if (!buf) return sh.total_bytes;
+    if (cap < sh.total_bytes) return -1;
+    uint8_t* out = (uint8_t*)buf;
+    memcpy(out, &sh, sizeof sh);
+    memcpy(out + sh.seg_table_offset, so.seg.data(), so.seg.size() * sizeof(int64_t));
+    memcpy(out + sh.data_offset, so.data, (size_t)sh.data_bytes);
+    return sh.total_bytes;
+}
+
+// The GPU entropy decoder (jpeg_entropy.cu) on the host: the same decode (jpeg_entropy.cuh), with loops over the threads of a CTA
+// in place of threads, the CTAs in order, and the rounds of the synchronisation exactly as the kernel runs them.
+extern "C" long long pe_jpeg_scan_to_coefs_host(const void* scan, void* coefs, long long cap, int subseq_bits) {
+    using namespace pe_jpeg;
+    if (!scan || !coefs || subseq_bits < 8) return -1;
+    const pe_jpeg_scan_header& h = *(const pe_jpeg_scan_header*)scan;
+    const long long S = subseq_bits;
+    long long nsub = 0;
+    if (!scan_header_valid(h, S, &nsub) || cap < h.coef.total_bytes) return -1;
+    std::vector<HuffDec> tabs(8);
+    for (int t = 0; t < 8; t++) {
+        HuffDec& d = tabs[t];
+        huff_canon(t < 4 ? h.dc_bits[t] : h.ac_bits[t - 4], d);
+        memcpy(d.vals, t < 4 ? h.dc_vals[t] : h.ac_vals[t - 4], 256);
+        for (int i = 0; i < (1 << LOOK_BITS); i++) d.look[i] = huff_look_entry(d, i);
+    }
+    const uint8_t* base = (const uint8_t*)scan;
+    ScanCtx c;
+    scan_slots(h, c);
+    c.data = base + h.data_offset;
+    c.seg = (const int64_t*)(base + h.seg_table_offset);
+    for (int k = 0; k < h.num_scan_comps; k++) { c.dc[k] = &tabs[h.dc_table[k]]; c.ac[k] = &tabs[4 + h.ac_table[k]]; }
+    c.zigzag = kZigzagNat;
+    uint8_t* out = (uint8_t*)coefs;
+    memset(out, 0, (size_t)h.coef.total_bytes);
+    memcpy(out, &h.coef, sizeof h.coef);
+    std::vector<long long> first_sub((size_t)c.num_segments + 1, 0);
+    for (int s = 0; s < c.num_segments; s++) first_sub[s + 1] = first_sub[s] + subseq_count(c.seg[2 * s + 1], S);
+    const int T = SYNC_THREADS;
+    long long err_mcu = -1;
+    State carry_state = 0;
+    long long carry_block = 0;
+    std::vector<int> seg(T);
+    std::vector<char> head(T), last(T);
+    std::vector<long long> stop(T), cnt(T), fb(T);
+    std::vector<State> start(T), ex(T), ns(T);
+    int s = 0;
+    for (long long g0 = 0; g0 < nsub; g0 += T) {
+        auto run = [&](int t) {
+            ex[t] = start[t];
+            const int64_t* sg = c.seg + 2 * seg[t];
+            cnt[t] = decode_run(c, c.data + sg[0], sg[1], &ex[t], stop[t], 1LL << 62, [](long long, int, int) {});
+        };
+        for (int t = 0; t < T; t++) {
+            const long long g = g0 + t;
+            head[t] = 1; last[t] = 1; seg[t] = 0; stop[t] = 0;
+            if (g >= nsub) { start[t] = ex[t] = 0; cnt[t] = 0; continue; }
+            while (first_sub[s + 1] <= g) s++;
+            const long long j = g - first_sub[s], n = c.seg[2 * s + 1];
+            seg[t] = s;
+            head[t] = j == 0;
+            last[t] = g == first_sub[s + 1] - 1;
+            stop[t] = last[t] ? n * 8 : (j + 1) * S;
+            start[t] = head[t] ? 0 : pack_state(canonical_pos(c.data + c.seg[2 * s], n, j * S), 0, 0);
+            run(t);
+        }
+        auto settle = [&]() {   // rounds: every thread takes its predecessor's exit of the previous round
+            for (;;) {
+                bool any = false;
+                for (int t = 0; t < T; t++) ns[t] = (!head[t] && t > 0) ? ex[t - 1] : start[t];
+                for (int t = 0; t < T; t++)
+                    if (ns[t] != start[t]) { start[t] = ns[t]; run(t); any = true; }
+                if (!any) break;
+            }
+        };
+        settle();
+        if (!head[0] && g0 > 0 && carry_state != start[0]) {   // the previous CTA's final exit state
+            start[0] = carry_state;
+            run(0);
+            settle();
+        }
+        for (int t = 0; t < T; t++) fb[t] = head[t] ? 0 : (t == 0 ? carry_block : fb[t - 1] + cnt[t - 1]);
+        carry_state = ex[T - 1];
+        carry_block = fb[T - 1] + cnt[T - 1];
+        for (int t = 0; t < T && g0 + t < nsub; t++) {
+            const long long limit = segment_mcus(c, seg[t]) * c.nslots - fb[t];
+            if (limit <= 0) continue;
+            const int64_t* sg = c.seg + 2 * seg[t];
+            State st = start[t];
+            const int sgi = seg[t];
+            const long long f = fb[t];
+            decode_run(c, c.data + sg[0], sg[1], &st, last[t] ? (1LL << 62) : stop[t], limit, [&](long long b, int zz, int v) {
+                long long mcu = 0;
+                const long long off = block_offset(h, c, sgi, f + b, &mcu);
+                if (zz == -2) { if (err_mcu < 0 || mcu < err_mcu) err_mcu = mcu; return; }
+                ((short*)(out + off))[zz < 0 ? 0 : c.zigzag[zz]] = (short)v;
+            });
+        }
+    }
+    // DC: per component a prefix sum of the differences that restarts with every segment, unsigned 32-bit as the host's pred
+    for (int sg = 0; sg < c.num_segments; sg++) {
+        unsigned pred[3] = {0, 0, 0};
+        const long long nb = segment_mcus(c, sg) * c.nslots;
+        for (long long b = 0; b < nb; b++) {
+            short* blk = (short*)(out + block_offset(h, c, sg, b, nullptr));
+            unsigned& pr = pred[c.slot_comp[b % c.nslots]];
+            pr += (unsigned)(int)blk[0];
+            blk[0] = (short)pr;
+        }
+    }
+    return err_mcu >= 0 ? -4 : h.coef.total_bytes;
 }
 
 extern "C" int pe_jpeg_coefs_to_bgr(const void* coefs, uint8_t* bgr, long long cap) {

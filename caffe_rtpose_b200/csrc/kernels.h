@@ -125,6 +125,20 @@ struct JpegArgs {
 };
 int launch_jpeg_reconstruct(const JpegArgs& a, cudaStream_t st);   // dequantise + IDCT, then upsample + colour: 2 launches
 
+// ---- JPEG entropy decoding (jpeg_entropy.cu): scan images of pe_jpeg_read_scan -> coefficient images
+struct JpegScanArgs {
+    const uint8_t* scans; long long scan_stride;    // [n] scan images (checked on the host), 256-byte aligned
+    uint8_t* coefs; long long coef_stride;          // [n] coefficient images, zeroed before the launch
+    void* tabs;                                     // [n][8] decoder tables (jpeg_huff_tables_bytes() per frame)
+    int* seg_sub; long long seg_stride;             // [n][num_segments + 1] first subsequence of every segment
+    unsigned long long* pub; int* flags; int ctas_max;   // [n][ctas_max] hand-over between the CTAs of a frame: state, block; flag
+    int* tickets;                                   // [n] CTA order
+    int* status;                                    // [n] first MCU with a DC category above 15, INT_MAX = none
+    int n, S;                                       // frames, subsequence bits
+};
+size_t jpeg_huff_tables_bytes();
+int launch_jpeg_entropy(const JpegScanArgs& a, cudaStream_t st);   // 3 launches
+
 // ---- convolution / pooling (conv_simt.cu, conv_tc.cu, pool.cu)
 int launch_conv_simt(const ConvArgs& a, cudaStream_t st);
 struct PoolArgs {

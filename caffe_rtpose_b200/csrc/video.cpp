@@ -207,7 +207,16 @@ extern "C" int pe_video_read(const pe_video* v, int index, uint8_t* bgr, long lo
     return PE_OK;
 }
 
+static long long read_jpeg_frame(const pe_video* v, int index, void* buf, long long cap,
+                                 long long (*reader)(const uint8_t*, long long, void*, long long));
 extern "C" long long pe_video_read_coefs(const pe_video* v, int index, void* buf, long long cap) {
+    return read_jpeg_frame(v, index, buf, cap, pe_jpeg_read_coefs);
+}
+extern "C" long long pe_video_read_scan(const pe_video* v, int index, void* buf, long long cap) {
+    return read_jpeg_frame(v, index, buf, cap, pe_jpeg_read_scan);
+}
+static long long read_jpeg_frame(const pe_video* v, int index, void* buf, long long cap,
+                                 long long (*reader)(const uint8_t*, long long, void*, long long)) {
     if (!v) { g_video_error = "null argument"; return -PE_ERR_INVALID; }
     if (!v->mjpeg) { g_video_error = v->path + ": not a Motion-JPEG video"; return -PE_ERR_INVALID; }
     if (index < 0 || index >= (int)v->frames.size()) { g_video_error = "frame index outside the video"; return -PE_ERR_INVALID; }
@@ -219,9 +228,10 @@ extern "C" long long pe_video_read_coefs(const pe_video* v, int index, void* buf
     if (!v->read_at(fr.off, data.data(), fr.size)) { g_video_error = v->path + ": read error"; return -PE_ERR_IO; }
     int jw = 0, jh = 0;
     const int hrc = pe_decode_jpeg(data.data(), (long long)data.size(), &jw, &jh, nullptr, 0);   // frame header only
-    long long rc = hrc ? hrc : pe_jpeg_read_coefs(data.data(), (long long)data.size(), nullptr, 0);
+    long long rc = hrc ? hrc : reader(data.data(), (long long)data.size(), nullptr, 0);
+    if (rc == -3) { g_video_error = v->path + ": frame " + std::to_string(index) + " needs the host entropy stage"; return -3; }
     if (rc > 0 && (jw != v->w || jh != v->h)) rc = -1;   // pe_video_read's rule: every frame has the video's size
-    if (rc > 0 && buf && cap >= rc && pe_jpeg_read_coefs(data.data(), (long long)data.size(), buf, cap) != rc) rc = -1;
+    if (rc > 0 && buf && cap >= rc && reader(data.data(), (long long)data.size(), buf, cap) != rc) rc = -1;
     if (rc <= 0) { g_video_error = v->path + ": frame " + std::to_string(index) + " is not a decodable JPEG"; return rc == -2 ? -PE_ERR_INVALID : -PE_ERR_IO; }
     return rc;
 }

@@ -58,6 +58,7 @@ ABI_SYMBOLS = [
     "pe_video_open", "pe_video_close", "pe_video_info", "pe_video_read", "pe_video_last_error",
     "pe_camera_open", "pe_camera_close", "pe_camera_info", "pe_camera_grab", "pe_camera_last_error", "pe_yuyv_to_bgr",
     "pe_compare_results", "pe_jpeg_read_coefs", "pe_jpeg_coefs_to_bgr", "pe_forward_jpeg_coefs", "pe_video_read_coefs",
+    "pe_jpeg_read_scan", "pe_jpeg_scan_to_coefs_host", "pe_forward_jpeg_scans", "pe_jpeg_decode_scans", "pe_video_read_scan",
 ]
 
 
@@ -144,6 +145,14 @@ def lib():
     L.pe_jpeg_read_coefs.restype = C.c_longlong
     L.pe_jpeg_coefs_to_bgr.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong]
     L.pe_forward_jpeg_coefs.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.POINTER(C.c_double)]
+    L.pe_jpeg_read_scan.argtypes = L.pe_jpeg_read_coefs.argtypes
+    L.pe_jpeg_read_scan.restype = C.c_longlong
+    L.pe_jpeg_scan_to_coefs_host.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong, C.c_int]
+    L.pe_jpeg_scan_to_coefs_host.restype = C.c_longlong
+    L.pe_forward_jpeg_scans.argtypes = L.pe_forward_jpeg_coefs.argtypes
+    L.pe_jpeg_decode_scans.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_int)]
+    L.pe_video_read_scan.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_longlong]
+    L.pe_video_read_scan.restype = C.c_longlong
     if hasattr(L, "pe_video_open") or "PE_LIB" not in os.environ:   # an older A/B build (PE_LIB) may predate the video reader
         L.pe_video_open.argtypes = [C.c_char_p, C.POINTER(C.c_void_p)]
         L.pe_video_close.argtypes = [C.c_void_p]
@@ -354,16 +363,34 @@ class PoseEngine:
         self._ck(lib().pe_forward_camera_frames(self._h, ptrs, len(frames), w, h, C.byref(s)))
         return s.value
 
-    def forward_jpeg(self, jpegs):
-        """jpegs: list of JPEG files (bytes) of one common size.  Only the entropy stage runs on the host (read_jpeg_coefs); the
-        GPU reconstructs the pixels, byte-identical to decode_jpeg, and then runs as forward_frames (display size) or
-        forward_camera_frames (any other size).  Returns frame.scale."""
-        bufs = [j if isinstance(j, np.ndarray) else read_jpeg_coefs(j) for j in jpegs]
+    def forward_jpeg(self, jpegs, entropy="host"):
+        """jpegs: list of JPEG files (bytes) of one common size.  entropy="host": only the entropy stage runs on the host
+        (read_jpeg_coefs); the GPU reconstructs the pixels, byte-identical to decode_jpeg, and then runs as forward_frames (display
+        size) or forward_camera_frames (any other size).  entropy="gpu": the host only parses the file (read_jpeg_scan) and the GPU
+        also decodes the Huffman data; for one interleaved sequential scan per file.  Arrays are taken as coefficient / scan images.
+        Returns frame.scale."""
+        if entropy not in ("host", "gpu"):
+            raise ValueError("entropy must be 'host' or 'gpu'")
+        read = read_jpeg_coefs if entropy == "host" else read_jpeg_scan
+        bufs = [j if isinstance(j, np.ndarray) else read(j) for j in jpegs]
         ptrs = (C.c_void_p * len(bufs))(*[b.ctypes.data for b in bufs])
         self._keep = bufs
         s = C.c_double()
-        self._ck(lib().pe_forward_jpeg_coefs(self._h, ptrs, len(bufs), C.byref(s)))
+        fn = lib().pe_forward_jpeg_coefs if entropy == "host" else lib().pe_forward_jpeg_scans
+        self._ck(fn(self._h, ptrs, len(bufs), C.byref(s)))
         return s.value
+
+    def decode_jpeg_scans(self, scans, subseq_bits=0):
+        """Test hook: scan images (read_jpeg_scan) -> coefficient images decoded on the GPU (subseq_bits 0 = the default
+        subsequence length).  Returns (list of coefficient images as uint8 arrays, list of statuses: 0, or 1 + the MCU of the
+        first data error)."""
+        scans = [np.ascontiguousarray(b, np.uint8) for b in scans]
+        outs = [np.zeros(jpeg_coef_header(b[:512])["total_bytes"], np.uint8) for b in scans]
+        ptrs = (C.c_void_p * len(scans))(*[b.ctypes.data for b in scans])
+        optrs = (C.c_void_p * len(outs))(*[o.ctypes.data for o in outs])
+        st = (C.c_int * len(scans))()
+        self._ck(lib().pe_jpeg_decode_scans(self._h, ptrs, len(scans), subseq_bits, optrs, st))
+        return outs, list(st)
 
     def render(self, idx=0, part_to_show=0, googly_eyes=False, display_bgr=None, want_canvas=False):
         """render() of rtpose.cpp:271-300 on frame idx of the last forward; returns the uint8 BGR image
@@ -648,6 +675,38 @@ def read_jpeg_coefs(data):
     if rc != n:
         raise _jpeg_error("pe_jpeg_read_coefs", rc)
     return buf
+
+
+def read_jpeg_scan(data):
+    """Scan image of a JPEG (pe_jpeg_scan_header + segment table + entropy-coded bytes, poseengine.h) as a uint8 array: the input of
+    PoseEngine.forward_jpeg(entropy="gpu").  Raises PoseEngineError for files that need the host entropy stage (progressive,
+    multi-scan) and for the codes of read_jpeg_coefs."""
+    n = lib().pe_jpeg_read_scan(data, len(data), None, 0)
+    if n == -3:
+        raise PoseEngineError("pe_jpeg_read_scan: not one interleaved sequential scan: needs the host entropy stage")
+    if n < 0:
+        raise _jpeg_error("pe_jpeg_read_scan", n)
+    buf = np.zeros(n, np.uint8)
+    rc = lib().pe_jpeg_read_scan(data, len(data), buf.ctypes.data, n)
+    if rc != n:
+        raise _jpeg_error("pe_jpeg_read_scan", rc)
+    return buf
+
+
+def jpeg_scan_to_coefs_host(scan, subseq_bits=1024):
+    """The GPU entropy decoder's algorithm run on the host: scan image -> (coefficient image, ok).  ok is False where
+    read_jpeg_coefs rejects the data (a DC category above 15)."""
+    scan = np.ascontiguousarray(scan, np.uint8)
+    if scan.size < 2784:
+        raise PoseEngineError("pe_jpeg_scan_to_coefs_host: truncated scan image")
+    n = jpeg_coef_header(scan[:512])["total_bytes"]
+    out = np.zeros(max(n, 0), np.uint8)
+    rc = lib().pe_jpeg_scan_to_coefs_host(scan.ctypes.data, out.ctypes.data, out.size, subseq_bits)
+    if rc == -1:
+        raise PoseEngineError("pe_jpeg_scan_to_coefs_host: malformed scan image")
+    if rc != n and rc != -4:
+        raise PoseEngineError("pe_jpeg_scan_to_coefs_host failed (%d)" % rc)
+    return out, rc == n
 
 
 def jpeg_coef_header(buf):

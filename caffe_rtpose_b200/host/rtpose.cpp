@@ -11,6 +11,7 @@
 // quality-98 .jpg files like the reference (pe_encode_jpeg; --frame_format bmp for lossless) with displayFrame's text overlays
 // (own bitmap font, --no_text turns them off).
 // Frames older than 0.1 s are dropped unless --no_frame_drops, as in processFrame (rtpose.cpp:1107-1124).
+#include <climits>
 #include <dirent.h>
 #include <math.h>
 #include <stdarg.h>
@@ -59,6 +60,9 @@ static void define_flags() {
     define("gpu_decode", "false", "[extension] JPEG sources (--image_dir .jpg files, Motion-JPEG --video): the producer threads run only the "
            "entropy (Huffman) stage; dequantisation, IDCT, chroma upsampling and colour conversion run on the GPU (pixels identical to the host "
            "decoder). Other files and JPEGs it does not take are decoded on the host as without it", true);
+    define("gpu_entropy", "false", "[extension] as --gpu_decode, and for sequential JPEGs (one interleaved scan: cameras, Motion-JPEG, "
+           "cv::imwrite) the producer threads only parse the file; the Huffman decoding runs on the GPU too. Progressive / multi-scan "
+           "JPEGs take the --gpu_decode route, other files the host decoder", true);
     define("frame_format", "jpg", "[extension] jpg (quality 98, as the reference) or bmp (lossless) for --write_frames");
     define("no_frame_drops", "false", "Dont drop frames.", true);
     define("write_json", "", "Write joint data with json format as prefix%06d.json");
@@ -154,7 +158,9 @@ struct Frame {
     double scale = 1.0;                      // display / original (rtpose.cpp:474-480), filled by the engine
     std::vector<uint8_t> bgr;                // display image, HWC BGR (decode buffer)
     std::shared_ptr<uint8_t> pinned;         // same image in page-locked memory (pe_host_alloc) for direct async DMA
-    bool coefs = false;                      // --gpu_decode: `pinned` holds the JPEG's coefficient image (pe_jpeg_read_coefs), not pixels
+    enum Kind { PIXELS, COEFS, SCAN };
+    Kind kind = PIXELS;                      // COEFS (--gpu_decode): `pinned` holds the JPEG's coefficient image (pe_jpeg_read_coefs);
+                                             // SCAN (--gpu_entropy): its scan image (pe_jpeg_read_scan)
     std::string stem;                        // for <stem>.json with --image_dir
     int num_people = 0;
     std::vector<float> joints;
@@ -394,6 +400,7 @@ struct Global {
     std::atomic<float> nms_threshold{0.05f}, connect_min_subset_score{0.4f}, connect_inter_threshold{0.05f};
     std::atomic<int> connect_min_subset_cnt{3}, connect_inter_min_above_threshold{9}, part_to_show{0}, params_version{0};
     std::atomic<int> dropped{0};
+    std::atomic<int> end_index{INT_MAX};   // --gpu_entropy: the run ends before this frame (a video frame the GPU could not decode)
     // global.uistate (rtpose.cpp:96-104): googly eyes, video pause / seek, driven by handle_key
     std::atomic<bool> googly_eyes{false}, video_paused{false};
     std::atomic<int> seek_delta{0};
@@ -416,6 +423,21 @@ static bool read_frame_image(const std::string& path, int& w, int& h, Frame& fr)
         fr.pinned = std::shared_ptr<uint8_t>(ph, [bytes](uint8_t* q) { g_pinned.put(q, bytes); });   // returned to the pool also when decoding failed
     }
     return ok;
+}
+
+static int num_producers();
+// --gpu_entropy: a frame whose entropy-coded data the GPU rejected (pe_fetch: PE_ERR_IO) is handled as the host route handles a file
+// it cannot decode, with the same message: it becomes a dropped index, and with the single --video reader the run ends there.
+static void undecodable_frame(const Frame& fr) {
+    std::lock_guard<std::mutex> l(global.mutex);
+    if (global.video) {
+        LOG_ERROR("%s: frame %d is not a decodable JPEG", F("video").c_str(), fr.video_frame_number);
+        int cur = global.end_index.load();
+        while (num_producers() == 1 && fr.index < cur && !global.end_index.compare_exchange_weak(cur, fr.index)) {}
+    } else {
+        LOG_ERROR("cannot decode %s (supported: .jpg, .png, 24-bit .bmp, P6 .ppm)", global.image_list[fr.video_frame_number].c_str());
+    }
+    global.dropped_index.push(fr.index);
 }
 
 static void pin_frame(Frame& fr) {
@@ -470,8 +492,9 @@ static int source_frame_count() {
     return (int)global.image_list.size();
 }
 // --gpu_decode: frame i of --image_dir / a Motion-JPEG --video as a coefficient image in a page-locked buffer of the pool (the
-// reconstruction runs on the GPU, pe_forward_jpeg_coefs).  false: not a JPEG, or one the coefficient stage refuses: the caller
-// decodes the frame on the host instead, which also reports what is wrong with it.
+// reconstruction runs on the GPU, pe_forward_jpeg_coefs); --gpu_entropy: as a scan image (pe_forward_jpeg_scans decodes the Huffman
+// data too), or as a coefficient image when the JPEG is not one sequential scan (-3).  false: not a JPEG, or one the coefficient
+// stage refuses: the caller decodes the frame on the host instead, which also reports what is wrong with it.
 static bool fetch_coefs(int i, Frame& fr) {
     std::vector<uint8_t> data;
     if (!global.video) {
@@ -485,10 +508,13 @@ static bool fetch_coefs(int i, Frame& fr) {
         fclose(f);
         if (!rd || data[0] != 0xFF || data[1] != 0xD8) return false;
     }
+    bool scan = Fb("gpu_entropy");
     auto read = [&](void* buf, long long cap) {
+        if (scan) return global.video ? pe_video_read_scan(global.video, i, buf, cap) : pe_jpeg_read_scan(data.data(), (long long)data.size(), buf, cap);
         return global.video ? pe_video_read_coefs(global.video, i, buf, cap) : pe_jpeg_read_coefs(data.data(), (long long)data.size(), buf, cap);
     };
-    const long long n = read(nullptr, 0);
+    long long n = read(nullptr, 0);
+    if (scan && n == -3) { scan = false; n = read(nullptr, 0); }   // progressive / multi-scan: the host entropy stage
     if (n <= (long long)sizeof(pe_jpeg_coef_header) || n > (3LL << 28)) return false;
     uint8_t* ph = g_pinned.get((size_t)n);   // without page-locked memory the engine stages the copy (as for pixel frames)
     if (ph) fr.pinned = std::shared_ptr<uint8_t>(ph, [n](uint8_t* q) { g_pinned.put(q, (size_t)n); });
@@ -496,15 +522,15 @@ static bool fetch_coefs(int i, Frame& fr) {
     pe_jpeg_coef_header hd;
     if (read(ph, n) != n) { fr.pinned.reset(); std::vector<uint8_t>().swap(fr.bgr); return false; }
     memcpy(&hd, ph, sizeof hd);
-    fr.w = hd.width; fr.h = hd.height;
-    fr.coefs = true;
+    fr.w = hd.width; fr.h = hd.height;   // (a scan image starts with the same header)
+    fr.kind = scan ? Frame::SCAN : Frame::COEFS;
     return true;
 }
 
 // frame i of the source (synthetic / --video / --image_dir) into fr; false: could not be decoded (message logged)
 static bool fetch_source_frame(int i, Frame& fr) {
     int w = global.disp_w, h = global.disp_h;
-    if (Fb("gpu_decode") && (global.video || !global.image_list.empty()) && !global.camera && Fi("synthetic") <= 0 && fetch_coefs(i, fr)) {
+    if ((Fb("gpu_decode") || Fb("gpu_entropy")) && (global.video || !global.image_list.empty()) && !global.camera && Fi("synthetic") <= 0 && fetch_coefs(i, fr)) {
         if (!global.video) {
             const std::string& p = global.image_list[i];
             const size_t slash = p.find_last_of('/'), dot = p.find_last_of('.');
@@ -564,6 +590,7 @@ static void producer() {
         Frame fr;
         fr.t_commit = now_s();    // frame.commit_time: taken when the frame is grabbed (rtpose.cpp:449)
         fr.index = global.produced; fr.video_frame_number = i;
+        if (fr.index >= global.end_index) break;   // --gpu_entropy: a video frame the GPU could not decode ends the run
         if (!fetch_source_frame(i, fr)) {
             if (global.video || global.camera) break;   // a broken frame ends a video / the capture (cap >> returns an empty Mat)
             continue;
@@ -595,7 +622,7 @@ static void producer_mt(int nthreads) {
     auto body = [&]() {
         while (!global.quit) {
             const int i = next++;
-            if (i >= total) break;
+            if (i >= total || i - start >= global.end_index) break;
             Frame fr;
             fr.t_commit = now_s();
             fr.index = i - start; fr.video_frame_number = i;
@@ -756,7 +783,7 @@ static void worker(int tid, pe_engine* e, pe_engine* ref) {
                 global.dropped++;
                 continue;
             }
-            if (!frames.empty() && (fr.w != frames[0].w || fr.h != frames[0].h || fr.coefs != frames[0].coefs)) {   // one forward = one frame size and kind
+            if (!frames.empty() && (fr.w != frames[0].w || fr.h != frames[0].h || fr.kind != frames[0].kind)) {   // one forward = one frame size and kind
                 pending = std::move(fr); pending_valid = true;
                 break;
             }
@@ -777,7 +804,8 @@ static void worker(int tid, pe_engine* e, pe_engine* ref) {
         for (auto& f : frames) ptrs.push_back(f.pinned ? f.pinned.get() : f.bgr.data());
         double scale = 1.0;
         auto forward = [&](pe_engine* h) {
-            if (frames[0].coefs) return pe_forward_jpeg_coefs(h, (const void* const*)ptrs.data(), (int)ptrs.size(), &scale);   // GPU JPEG reconstruction
+            if (frames[0].kind == Frame::COEFS) return pe_forward_jpeg_coefs(h, (const void* const*)ptrs.data(), (int)ptrs.size(), &scale);   // GPU JPEG reconstruction
+            if (frames[0].kind == Frame::SCAN) return pe_forward_jpeg_scans(h, (const void* const*)ptrs.data(), (int)ptrs.size(), &scale);   // + Huffman decoding
             if (frames[0].w == global.disp_w && frames[0].h == global.disp_h) return pe_forward_frames(h, ptrs.data(), (int)ptrs.size());
             return pe_forward_camera_frames(h, ptrs.data(), (int)ptrs.size(), frames[0].w, frames[0].h, &scale);   // warpAffine on the GPU
         };
@@ -791,7 +819,13 @@ static void worker(int tid, pe_engine* e, pe_engine* ref) {
         }
         for (size_t i = 0; i < frames.size(); i++) {
             int cnt = 0;
-            if (pe_fetch(e, (int)i, joints.data(), &cnt, audit ? peaks.data() : nullptr)) { LOG_ERROR("GPU %d: %s", device, pe_last_error(e)); global.failed = global.quit = true; break; }
+            const int frc_i = pe_fetch(e, (int)i, joints.data(), &cnt, audit ? peaks.data() : nullptr);
+            if (frc_i == PE_ERR_IO && frames[i].kind == Frame::SCAN) {   // corrupt entropy-coded data: as the host route treats the file
+                undecodable_frame(frames[i]);
+                frames[i].pinned.reset();
+                continue;
+            }
+            if (frc_i) { LOG_ERROR("GPU %d: %s", device, pe_last_error(e)); global.failed = global.quit = true; break; }
             if (audit && !audit_frame(e, ref, (int)i, joints, cnt, peaks)) {
                 LOG_ERROR("GPU %d (audit): %s", device, pe_last_error(ref)); global.failed = global.quit = true; break;
             }
@@ -1008,12 +1042,16 @@ static void orderer_and_writer(int num_workers) {
                 std::lock_guard<std::mutex> l(global.mutex);
                 while (!global.dropped_index.empty() && global.dropped_index.top() == next) { global.dropped_index.pop(); next++; }
             }
-            if (!heap.empty() && heap.top().index == next) { Frame top = heap.top(); heap.pop(); top.t_buffered = now_s(); emit(top); next++; }
+            if (!heap.empty() && heap.top().index == next) {
+                Frame top = heap.top(); heap.pop(); top.t_buffered = now_s();
+                if (top.index < global.end_index) emit(top);
+                next++;
+            }
             else break;
         }
         if (!got) {
             if (global.finished == num_workers && global.output_queue.size() == 0) {
-                while (!heap.empty()) { Frame top = heap.top(); heap.pop(); emit(top); }   // flush (frames lost to an error leave gaps)
+                while (!heap.empty()) { Frame top = heap.top(); heap.pop(); if (top.index < global.end_index) emit(top); }   // flush (frames lost to an error leave gaps)
                 break;
             }
             std::this_thread::sleep_for(std::chrono::microseconds(200));
@@ -1047,6 +1085,10 @@ int main(int argc, char** argv) {
     }
     if (Fb("gpu_decode") && (Fi("synthetic") > 0 || (F("video").empty() && F("image_dir").empty()))) {
         LOG_ERROR("--gpu_decode reconstructs JPEG files on the GPU: it needs --image_dir or a Motion-JPEG --video (not --synthetic or a camera)");
+        return 1;
+    }
+    if (Fb("gpu_entropy") && (Fi("synthetic") > 0 || (F("video").empty() && F("image_dir").empty()))) {
+        LOG_ERROR("--gpu_entropy decodes JPEG files on the GPU: it needs --image_dir or a Motion-JPEG --video (not --synthetic or a camera)");
         return 1;
     }
     if (F("video").empty() && F("image_dir").empty() && Fi("synthetic") <= 0) {   // the camera (rtpose.cpp:401-405, 1694-1695)

@@ -144,6 +144,14 @@ int pe_forward_camera_frames(pe_engine* e, const uint8_t* const* frames, int n, 
  * disp_w x disp_h (*scale = 1) and as pe_forward_camera_frames otherwise (GPU warpAffine, *scale = frame.scale).  pe_render
  * with display_bgr == NULL draws on the reconstructed display frame. */
 int pe_forward_jpeg_coefs(pe_engine* e, const void* const* coefs, int n, double* scale);
+/* the same from scan images (pe_jpeg_read_scan): the Huffman data is decoded on the GPU into coefficient images, then as
+ * pe_forward_jpeg_coefs.  A frame whose data the host entropy stage rejects (a DC category above 15) does not stop the batch:
+ * pe_fetch of that frame returns PE_ERR_IO (pe_last_error names the frame and the MCU), the other frames' results are unaffected. */
+int pe_forward_jpeg_scans(pe_engine* e, const void* const* scans, int n, double* scale);
+/* test hook: decode n scan images into coefficient images on the GPU with subsequences of subseq_bits bits (0 = the default) and
+ * copy them to coefs_out[i] (coef.total_bytes each).  Synchronous.  status_out[i] (optional): 0, or 1 + the MCU of the first data
+ * error of frame i.  The statuses of an earlier pe_forward_jpeg_scans are dropped: pe_fetch no longer reports them. */
+int pe_jpeg_decode_scans(pe_engine* e, const void* const* scans, int n, int subseq_bits, void* const* coefs_out, int* status_out);
 /* same, frames already resident in device memory (n consecutive disp_h*disp_w*3 images) */
 int pe_forward_frames_device(pe_engine* e, const void* d_frames, int n);
 /* HOST net input as the reference uploads it: n x num_scales x 3 x net_h x net_w fp32 planar
@@ -254,6 +262,41 @@ long long pe_jpeg_read_coefs(const uint8_t* data, long long size, void* buf, lon
  * kernels are tested against.  Returns 0 and writes width x height x 3 uint8 BGR when cap suffices; -1 = malformed buffer / cap. */
 int pe_jpeg_coefs_to_bgr(const void* coefs, uint8_t* bgr, long long cap);
 
+/* ---- JPEG entropy decoding on the GPU: the host parses the headers and finds the restart markers, the GPU decodes the Huffman data
+ * into the coefficient image pe_jpeg_read_coefs would write, bit for bit.
+ * Scan image = this header, then the segment table at seg_table_offset (num_segments x {int64 offset, int64 length}, offsets from
+ * data_offset), then the entropy-coded bytes of the scan at data_offset, still byte-stuffed, RST markers included.  One segment per
+ * restart interval (restart_interval == 0: one segment); a segment's bytes end at the first FF xx with xx != 00. */
+#define PE_JPEG_SCAN_MAGIC 0x4E43534Au /* "JSCN" */
+typedef struct pe_jpeg_scan_header {
+    pe_jpeg_coef_header coef; /* the header pe_jpeg_read_coefs writes for this file (geometry, quantisation tables) */
+    uint32_t magic;           /* PE_JPEG_SCAN_MAGIC */
+    int32_t num_scan_comps;   /* == coef.num_comps */
+    int32_t scan_comp[3];     /* SOF index of the scan's k-th component, in SOS order (the order of the blocks in an MCU) */
+    int32_t dc_table[3];      /* Huffman table slots of the scan's k-th component */
+    int32_t ac_table[3];
+    int32_t restart_interval; /* MCUs per segment, 0 = none */
+    int32_t mcux, mcuy;       /* MCU grid */
+    int32_t num_segments;
+    int32_t reserved;
+    int64_t seg_table_offset; /* bytes from the start of the buffer */
+    int64_t data_offset, data_bytes;
+    int64_t total_bytes;      /* header + segment table + data */
+    uint8_t dc_bits[4][16], ac_bits[4][16];   /* BITS (codes of length 1..16) of the four DC and four AC slots */
+    uint8_t dc_vals[4][256], ac_vals[4][256]; /* HUFFVAL; slots still undefined at the SOS hold the Annex K tables (slots 0, 1) or nothing */
+} pe_jpeg_scan_header;
+/* The scan image of a JPEG (host only, thread-safe), with pe_jpeg_read_coefs's size-query and cap protocol: buf == NULL returns the
+ * size (this parses the whole file).  It covers the streams of pe_jpeg_read_coefs's fast route: SOF0 / SOF1, one scan that names
+ * every component once.  -3: valid so far but another kind (progressive, multi-scan): needs the host entropy stage.  Otherwise
+ * pe_jpeg_read_coefs's codes; a data error the parser cannot see (a DC category above 15) is reported by the decoder.  Such a
+ * stream is one where the codes may differ: pe_jpeg_read_coefs stops at the scan with -1, this call goes on parsing and may
+ * return a later header's error instead (e.g. -2 for an SOF3 segment after the scan) or succeed; either way nothing is decoded. */
+long long pe_jpeg_read_scan(const uint8_t* data, long long size, void* buf, long long cap);
+/* Test hook: the GPU entropy decoder's algorithm run on the host (thread loops in place of threads), subsequences of subseq_bits
+ * bits (>= 8).  Writes the coefficient image; returns its size, -1 for a malformed scan image / cap, -4 for data the host entropy
+ * stage rejects (a DC category above 15: pe_jpeg_read_coefs returns -1) - the coefficient image is written all the same. */
+long long pe_jpeg_scan_to_coefs_host(const void* scan, void* coefs, long long cap, int subseq_bits);
+
 /* same for .png (the third format the reference lists, rtpose.cpp:1743): inflate + PNG filters / Adam7 / all colour types and
  * bit depths, converted as cv::imread(IMREAD_COLOR) does (8-bit BGR, alpha dropped, 16-bit -> high byte). */
 int pe_decode_png(const uint8_t* data, long long size, int* w, int* h, uint8_t* bgr, long long cap);
@@ -272,6 +315,9 @@ int pe_video_read(const pe_video* v, int index, uint8_t* bgr, long long cap);
  * written when buf != NULL and cap >= size (call again with a larger buffer otherwise).  -PE_ERR_INVALID: not a Motion-JPEG video,
  * bad index, a JPEG variant the decoder does not handle; -PE_ERR_IO: unreadable / corrupt frame (text in pe_video_last_error()). */
 long long pe_video_read_coefs(const pe_video* v, int index, void* buf, long long cap);
+/* the same as a scan image (pe_jpeg_read_scan) for pe_forward_jpeg_scans.  A frame that needs the host entropy stage (progressive,
+ * multi-scan) gives -3, as pe_jpeg_read_scan; this call never returns -PE_ERR_STATE, so -3 always has that meaning here. */
+long long pe_video_read_scan(const pe_video* v, int index, void* buf, long long cap);
 const char* pe_video_last_error(void);
 
 /* cv::VideoCapture on a camera index (rtpose.cpp:401-405 cap.open(FLAGS_camera) + CV_CAP_PROP_FRAME_WIDTH/HEIGHT from
