@@ -17,7 +17,7 @@
 //     row tiles form a thread block cluster: each CTA loads 1/TC_CLUSTER of every weight tile and multicasts it to all,
 //     and a slot of the weight ring is refilled once the consumers of every CTA in the cluster have released it.
 //   * Two consumer warpgroups (64 rows each) issue wgmma.mma_async m64nBNk16 from shared-memory descriptors,
-//     accumulators in registers, fp32.
+//     accumulators in registers, fp32, with one wgmma group of K steps in flight behind the one being issued.
 //   * Split precision: activations and weights are stored as P 16-bit "planes" whose sum is the fp32 value
 //     (hi / lo); the kernel issues the cross products with pa + pb < P on the tensor core.  The format (kernels.h,
 //     PlaneFmt): P=2 fp16 = parity mode, ~1e-5 over the whole net (DESIGN.md section 3); P=1 fp16 = fast mode, the
@@ -140,6 +140,7 @@ __device__ __forceinline__ uint64_t wg_desc(uint32_t saddr) {
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 
 // D(64 x N, fp32 registers) (+)= A(64 x 16) * B(N x 16)^T, both K-major in shared memory; scale_d = 0 overwrites D.
 // Register j of a thread holds row 16*(warp%4) + lane/4 + 8*((j/2)%2), column 8*(j/4) + 2*(lane%4) + j%2.
@@ -240,6 +241,14 @@ constexpr int TC_SMEM_BUDGET = 220 * 1024;   // of the 227 KB a block may use on
 // so the L2 -> shared-memory traffic of the weights, most of the kernel's, drops by this factor.  A windows stay per CTA.
 constexpr int TC_CLUSTER = 2;
 
+// A consumer warp has finished reading weight slot b (its wgmma groups have completed): tell the producer of every CTA in the
+// cluster, since each weight tile is written into all of them; and release window slot w after its last tap (w >= 0).
+__device__ __forceinline__ void tc_release(uint64_t* bempty, uint64_t* wempty, int b, int w, int lane) {
+    __syncwarp();
+    if (lane < TC_CLUSTER) mbar_arrive_cluster(&bempty[b], lane);
+    if (w >= 0 && lane == 0) mbar_arrive(&wempty[w]);
+}
+
 // Rows of the A window box: a 1x1 filter row is a single tap and reads only the tile's 128 rows.
 __host__ __device__ constexpr int tc_window_rows(int ksize) { return ksize == 1 ? TC_BM : TC_WROWS; }
 
@@ -339,45 +348,51 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     for (int j = 0; j < NACC; j++) { acc_h[j] = 0.f; sum_h[j] = 0.f; acc_c[j] = 0.f; }
     const int cs = a.chunk_iters;
     const uint32_t a_plane = tc_window_rows(ks) * 128;   // plane stride of the window as the TMA box lays it out
-    int it = 0, wc = 0;
-    for (int kb = 0; kb < a.kblocks_per_tap; kb++)
-        for (int r = 0; r < ks; r++, wc++) {
+    // K steps (it: one tap x 64 channels) in hi*hi chunks of cs steps, the last one possibly shorter.  One wgmma group stays
+    // in flight: step s is issued before step s - 1 is waited for, and only then are step s - 1's weight slot (and its
+    // window, after the window's last tap) released.  A chunk ends with wait_group 0 and the round-to-nearest chunk sum in
+    // straight-line code, so no accumulator is read while a group writing it is in flight.
+    int it = 0, wc = 0, q = 0;   // K step, window, tap within the window
+    for (int c0 = 0; c0 < num_k; c0 += cs) {
+        const int n = min(cs, num_k - c0);
+        int prev_b = 0, prev_w = -1;   // the previous step's weight slot, and its window slot if that was the window's last tap
+        for (int s = 0; s < n; s++, it++) {
             const int w = wc % WS;
-            mbar_wait(&wfull[w], (uint32_t)(wc / WS) & 1u);
-            const uint32_t wa = smem_u32(wring + (size_t)w * S::A_BYTES) + (uint32_t)(wg * 64 * 128);
-            for (int q = 0; q < ks; q++, it++) {
-                const int b = it % BS;
-                mbar_wait(&bfull[b], (uint32_t)(it / BS) & 1u);
-                const uint32_t sa = wa + (uint32_t)(q * 128);   // tap q: window rows [q + 64 wg, q + 64 wg + 64)
-                const uint32_t sb = smem_u32(bring + (size_t)b * S::B_BYTES);
-                const uint32_t h_acc = (it % cs) != 0;   // 0: hi*hi chunk starts from zero
-                wg_fence();
+            if (q == 0) mbar_wait(&wfull[w], (uint32_t)(wc / WS) & 1u);
+            const int b = it % BS;
+            mbar_wait(&bfull[b], (uint32_t)(it / BS) & 1u);
+            // tap q: window rows [q + 64 wg, q + 64 wg + 64)
+            const uint32_t sa = smem_u32(wring + (size_t)w * S::A_BYTES) + (uint32_t)(wg * 64 * 128) + (uint32_t)(q * 128);
+            const uint32_t sb = smem_u32(bring + (size_t)b * S::B_BYTES);
+            const uint32_t h_acc = s != 0;   // 0: hi*hi chunk starts from zero
+            wg_fence();
 #pragma unroll
-                for (int k = 0; k < TC_BK / 16; k++) {
-                    Wgmma<BN>::template mma<F16>(acc_h, wg_desc(sa + k * 32), wg_desc(sb + k * 32), (k != 0) | h_acc);
-                    if constexpr (PLANES > 1) {
+            for (int k = 0; k < TC_BK / 16; k++) {
+                Wgmma<BN>::template mma<F16>(acc_h, wg_desc(sa + k * 32), wg_desc(sb + k * 32), (k != 0) | h_acc);
+                if constexpr (PLANES > 1) {
 #pragma unroll
-                        for (int pa = 0; pa < PLANES; pa++)
+                    for (int pa = 0; pa < PLANES; pa++)
 #pragma unroll
-                            for (int pb = 0; pb < PLANES - pa; pb++) {
-                                if (pa + pb == 0) continue;
-                                const uint32_t first = it == 0 && k == 0 && pa + pb == 1 && pa == 0;
-                                Wgmma<BN>::template mma<F16>(acc_c, wg_desc(sa + pa * a_plane + k * 32),
-                                                             wg_desc(sb + pb * S::B_PLANE + k * 32), first ? 0u : 1u);
-                            }
-                    }
-                }
-                wg_commit();
-                wg_wait_all();
-                __syncwarp();
-                if (lane < TC_CLUSTER) mbar_arrive_cluster(&bempty[b], lane);   // this warp has read the weight tile: tell every producer
-                if ((it + 1) % cs == 0 || it + 1 == num_k) {
-#pragma unroll
-                    for (int j = 0; j < NACC; j++) sum_h[j] = __fadd_rn(sum_h[j], acc_h[j]);
+                        for (int pb = 0; pb < PLANES - pa; pb++) {
+                            if (pa + pb == 0) continue;
+                            const uint32_t first = it == 0 && k == 0 && pa + pb == 1 && pa == 0;
+                            Wgmma<BN>::template mma<F16>(acc_c, wg_desc(sa + pa * a_plane + k * 32),
+                                                         wg_desc(sb + pb * S::B_PLANE + k * 32), first ? 0u : 1u);
+                        }
                 }
             }
-            if (lane == 0) mbar_arrive(&wempty[w]);   // ... and of the window, after its last tap
+            wg_commit();
+            wg_wait_1();
+            if (s > 0) tc_release(bempty, wempty, prev_b, prev_w, lane);
+            prev_b = b;
+            prev_w = q == ks - 1 ? w : -1;
+            if (++q == ks) { q = 0; wc++; }
         }
+        wg_wait_all();
+        tc_release(bempty, wempty, prev_b, prev_w, lane);
+#pragma unroll
+        for (int j = 0; j < NACC; j++) sum_h[j] = __fadd_rn(sum_h[j], acc_h[j]);
+    }
 
     // ===== epilogue: sum, bias, ReLU, re-split into planes, store =====
     const int per_img = a.Hs * a.Wp;
