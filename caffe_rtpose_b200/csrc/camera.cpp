@@ -23,6 +23,7 @@
 #include <vector>
 
 #include "../../include/poseengine.h"
+#include "pixels.cuh"
 
 namespace {
 
@@ -34,24 +35,15 @@ int xioctl(int fd, unsigned long req, void* arg) {
     return r;
 }
 
-inline uint8_t sat8(int v) { return (uint8_t)(v < 0 ? 0 : (v > 255 ? 255 : v)); }
-
 }  // namespace
 
-// cv::cvtColor(src, dst, COLOR_YUV2BGR_YUYV) (imgproc color_yuv: ITU-R BT.601, studio range, 20-bit fixed point)
+// cv::cvtColor(src, dst, COLOR_YUV2BGR_YUYV) (imgproc color_yuv: ITU-R BT.601, studio range, 20-bit fixed point; pixels.cuh)
 extern "C" int pe_yuyv_to_bgr(const uint8_t* yuyv, int w, int h, long long stride, uint8_t* bgr) {
     if (!yuyv || !bgr || w <= 0 || h <= 0 || (w & 1) || stride < 2LL * w) return PE_ERR_INVALID;
-    constexpr int SHIFT = 20, CY = 1220542, CUB = 2116026, CUG = -409993, CVG = -852492, CVR = 1673527, HALF = 1 << (SHIFT - 1);
     for (int y = 0; y < h; y++) {
         const uint8_t* s = yuyv + (size_t)y * (size_t)stride;
         uint8_t* d = bgr + (size_t)y * w * 3;
-        for (int x = 0; x < w; x += 2, s += 4, d += 6) {
-            const int u = (int)s[1] - 128, v = (int)s[3] - 128;
-            const int ruv = HALF + CVR * v, guv = HALF + CVG * v + CUG * u, buv = HALF + CUB * u;
-            const int y0 = ((int)s[0] - 16 > 0 ? (int)s[0] - 16 : 0) * CY, y1 = ((int)s[2] - 16 > 0 ? (int)s[2] - 16 : 0) * CY;
-            d[0] = sat8((y0 + buv) >> SHIFT); d[1] = sat8((y0 + guv) >> SHIFT); d[2] = sat8((y0 + ruv) >> SHIFT);
-            d[3] = sat8((y1 + buv) >> SHIFT); d[4] = sat8((y1 + guv) >> SHIFT); d[5] = sat8((y1 + ruv) >> SHIFT);
-        }
+        for (int x = 0; x < w; x += 2, s += 4, d += 6) pe_pix::yuyv_pair(s, d);
     }
     return PE_OK;
 }

@@ -18,6 +18,7 @@
 #include "conv_tc.h"
 #include "jpeg_coefs.h"
 #include "jpeg_entropy.cuh"
+#include "pixels.cuh"
 #include <climits>
 #include "prototxt.h"
 
@@ -88,6 +89,9 @@ struct pe_engine {
     uint8_t* d_raw = nullptr; size_t raw_cap = 0; uint8_t* h_raw = nullptr; size_t h_raw_cap = 0;
     int warp_w = 0, warp_h = 0; double warp_scale = 1.0;
     int *d_wa = nullptr, *d_wb = nullptr, *d_wx0 = nullptr, *d_wy0 = nullptr; short* d_wtab = nullptr;
+    // decoder-format host frames (pe_forward_pixels) copied to the device before conversion; pe_stream_wait's event
+    uint8_t* d_pix = nullptr; size_t pix_cap = 0;
+    cudaEvent_t ev_wait = nullptr;
     bool input_lo_dirty = false;
     // JPEG coefficient images (pe_forward_jpeg_coefs): device copies, pinned staging for pageable callers, component planes
     uint8_t* d_jcoef = nullptr; size_t jcoef_cap = 0; uint8_t* h_jcoef = nullptr; size_t h_jcoef_cap = 0;
@@ -427,6 +431,7 @@ extern "C" void pe_destroy(pe_engine* e) {
     for (auto& t : e->tc) tc_layer_destroy(t);
     cudaFree(e->d_jcoef); cudaFreeHost(e->h_jcoef); cudaFree(e->d_jplanes);
     cudaFree(e->d_jscan); cudaFreeHost(e->h_jscan); cudaFree(e->d_jwork); cudaFreeHost(e->h_jstatus);
+    cudaFree(e->d_pix); if (e->ev_wait) cudaEventDestroy(e->ev_wait);
     cudaFree(e->d_raw); cudaFreeHost(e->h_raw); cudaFree(e->d_wa); cudaFree(e->d_wb); cudaFree(e->d_wx0); cudaFree(e->d_wy0); cudaFree(e->d_wtab);
     e->packed_owner.reset(); cudaFree(e->d_range); cudaFree(e->d_frames); cudaFree(e->d_resized); cudaFree(e->d_planar); cudaFree(e->d_maps);
     cudaFreeHost(e->h_frames); cudaFreeHost(e->h_planar); cudaFreeHost(e->h_maps);
@@ -1102,44 +1107,6 @@ static int prepare_warp(pe_engine* e, int ow, int oh) {
     return PE_OK;
 }
 
-extern "C" int pe_forward_camera_frames(pe_engine* e, const uint8_t* const* frames, int n, int orig_w, int orig_h, double* scale) {
-    int rc = check_n(e, n); if (rc) return rc;
-    if (!frames || orig_w <= 0 || orig_h <= 0) return fail(e, PE_ERR_INVALID, "bad raw frame arguments");
-    CK(e, cudaSetDevice(e->cfg.device));
-    rc = prepare_warp(e, orig_w, orig_h); if (rc) return rc;
-    if (scale) *scale = e->warp_scale;
-    const size_t fb = (size_t)orig_w * orig_h * 3;
-    if (e->raw_cap < fb * n) {
-        CK(e, cudaStreamSynchronize(e->stream));
-        cudaFree(e->d_raw); e->d_raw = nullptr;
-        CK(e, cudaMalloc(&e->d_raw, fb * e->cfg.max_batch));
-        e->raw_cap = fb * e->cfg.max_batch;
-    }
-    bool pinned = true;
-    for (int i = 0; i < n && pinned; i++) {
-        cudaPointerAttributes at;
-        if (!frames[i]) return fail(e, PE_ERR_INVALID, "null frame %d", i);
-        if (cudaPointerGetAttributes(&at, frames[i]) != cudaSuccess || at.type != cudaMemoryTypeHost) { pinned = false; cudaGetLastError(); }
-    }
-    if (pinned) {
-        for (int i = 0; i < n; i++) CK(e, cudaMemcpyAsync(e->d_raw + i * fb, frames[i], fb, cudaMemcpyHostToDevice, e->stream));
-    } else {
-        CK(e, cudaStreamSynchronize(e->stream));
-        if (e->h_raw_cap < fb * n) {
-            cudaFreeHost(e->h_raw); e->h_raw = nullptr;
-            CK(e, cudaMallocHost(&e->h_raw, fb * e->cfg.max_batch));
-            e->h_raw_cap = fb * e->cfg.max_batch;
-        }
-        for (int i = 0; i < n; i++) memcpy(e->h_raw + i * fb, frames[i], fb);
-        CK(e, cudaMemcpyAsync(e->d_raw, e->h_raw, fb * n, cudaMemcpyHostToDevice, e->stream));
-    }
-    WarpArgs w;
-    w.src = e->d_raw; w.dst = e->d_frames; w.sw = orig_w; w.sh = orig_h; w.dw = e->cfg.disp_w; w.dh = e->cfg.disp_h;
-    w.adelta = e->d_wa; w.bdelta = e->d_wb; w.x0 = e->d_wx0; w.y0 = e->d_wy0; w.tab = e->d_wtab;
-    e->launches += launch_warp_affine(w, n, e->stream);
-    return pe_forward_frames_device(e, e->d_frames, n);
-}
-
 // (re)allocates *p to hold at least `need` bytes; the stream is drained first because queued work may still use the old buffer
 static int grow_buffer(pe_engine* e, uint8_t** p, size_t* cap, size_t need, bool host) {
     if (*cap >= need) return PE_OK;
@@ -1147,6 +1114,107 @@ static int grow_buffer(pe_engine* e, uint8_t** p, size_t* cap, size_t need, bool
     if (host) { cudaFreeHost(*p); *p = nullptr; CK(e, cudaMallocHost((void**)p, need)); }
     else { cudaFree(*p); *p = nullptr; CK(e, cudaMalloc((void**)p, need)); }
     *cap = need;
+    return PE_OK;
+}
+
+// Where the routes that read frames of any size (pixels, camera, JPEG) build their W x H BGR frames: the display frames themselves
+// at the display size (*scale = 1), else the warpAffine source d_raw (*scale = frame.scale).  finish_frames warps d_raw into the
+// display frames when needed and runs the net.
+static int frame_target(pe_engine* e, int W, int H, uint8_t** dst, double* scale) {
+    if (W == e->cfg.disp_w && H == e->cfg.disp_h) {
+        *dst = e->d_frames;
+        if (scale) *scale = 1.0;
+        return PE_OK;
+    }
+    int rc = prepare_warp(e, W, H); if (rc) return rc;
+    rc = grow_buffer(e, &e->d_raw, &e->raw_cap, (size_t)W * H * 3 * e->cfg.max_batch, false); if (rc) return rc;
+    *dst = e->d_raw;
+    if (scale) *scale = e->warp_scale;
+    return PE_OK;
+}
+static int finish_frames(pe_engine* e, int n, int W, int H) {
+    if (W != e->cfg.disp_w || H != e->cfg.disp_h) {
+        WarpArgs w;
+        w.src = e->d_raw; w.dst = e->d_frames; w.sw = W; w.sh = H; w.dw = e->cfg.disp_w; w.dh = e->cfg.disp_h;
+        w.adelta = e->d_wa; w.bdelta = e->d_wb; w.x0 = e->d_wx0; w.y0 = e->d_wy0; w.tab = e->d_wtab;
+        e->launches += launch_warp_affine(w, n, e->stream);
+    }
+    return pe_forward_frames_device(e, e->d_frames, n);
+}
+
+extern "C" int pe_forward_pixels(pe_engine* e, const pe_pixel_format* fmt, const void* const* frames, int n, double* scale) {
+    NvtxRange r("pe_forward_pixels");
+    int rc = check_n(e, n); if (rc) return rc;
+    pe_pix::Layout L;
+    std::string why;
+    if (!pe_pix::layout_of(fmt, &L, &why)) return fail(e, PE_ERR_INVALID, "%s", why.c_str());
+    if (!frames) return fail(e, PE_ERR_INVALID, "null frames");
+    CK(e, cudaSetDevice(e->cfg.device));
+    enum { DEVICE, PINNED, PAGEABLE };
+    int kind[PIX_MAX_FRAMES];
+    bool any_host = false, any_pageable = false;
+    for (int i = 0; i < n; i++) {
+        if (!frames[i]) return fail(e, PE_ERR_INVALID, "null frame %d", i);
+        cudaPointerAttributes at;
+        if (cudaPointerGetAttributes(&at, frames[i]) != cudaSuccess) { cudaGetLastError(); at.type = cudaMemoryTypeUnregistered; }
+        if (at.type == cudaMemoryTypeDevice && at.device != e->cfg.device)
+            return fail(e, PE_ERR_INVALID, "frame %d is device memory of GPU %d, the engine runs on GPU %d", i, at.device, e->cfg.device);
+        kind[i] = at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged ? DEVICE : at.type == cudaMemoryTypeHost ? PINNED : PAGEABLE;
+        any_host |= kind[i] != DEVICE;
+        any_pageable |= kind[i] == PAGEABLE;
+    }
+    uint8_t* dst;
+    rc = frame_target(e, L.w, L.h, &dst, scale); if (rc) return rc;
+    const bool bgr = L.format == PE_PIX_BGR;
+    const size_t fb = (size_t)L.w * L.h * 3, span = (size_t)L.span, stride = (span + 255) & ~(size_t)255;
+    // Pageable frames are staged in h_raw, which the queued work may still be reading: the stream is drained first.  Host frames
+    // other than BGR are copied whole to d_pix, and the kernel converts them there.
+    if (any_pageable) {
+        rc = grow_buffer(e, &e->h_raw, &e->h_raw_cap, stride * e->cfg.max_batch, true); if (rc) return rc;
+        CK(e, cudaStreamSynchronize(e->stream));
+    }
+    if (any_host && !bgr) { rc = grow_buffer(e, &e->d_pix, &e->pix_cap, stride * e->cfg.max_batch, false); if (rc) return rc; }
+    PixArgs a;
+    a.dst = dst; a.pitch = L.pitch; a.chroma = L.chroma; a.format = L.format; a.w = L.w; a.h = L.h;
+    for (int i = 0; i < n; i++) {
+        const uint8_t* src = (const uint8_t*)frames[i];
+        if (kind[i] == PAGEABLE) { memcpy(e->h_raw + i * stride, src, span); src = e->h_raw + i * stride; }
+        if (bgr) {   // BGR needs no conversion: the copy into place drops the pitch
+            CK(e, cudaMemcpy2DAsync(dst + i * fb, (size_t)L.w * 3, src, (size_t)L.pitch, (size_t)L.w * 3, L.h, cudaMemcpyDefault, e->stream));
+        } else if (kind[i] == DEVICE) {
+            a.src[i] = src;
+        } else {
+            CK(e, cudaMemcpyAsync(e->d_pix + i * stride, src, span, cudaMemcpyHostToDevice, e->stream));
+            a.src[i] = e->d_pix + i * stride;
+        }
+    }
+    if (!bgr) e->launches += launch_pixels_to_bgr(a, n, e->stream);
+    return finish_frames(e, n, L.w, L.h);
+}
+
+extern "C" int pe_forward_camera_frames(pe_engine* e, const uint8_t* const* frames, int n, int orig_w, int orig_h, double* scale) {
+    const pe_pixel_format f = {PE_PIX_BGR, orig_w, orig_h, 0, 0};
+    return pe_forward_pixels(e, &f, (const void* const*)frames, n, scale);
+}
+
+extern "C" int pe_stream_wait(pe_engine* e, void* cuda_stream) {
+    if (!e) return PE_ERR_INVALID;
+    CK(e, cudaSetDevice(e->cfg.device));
+    if (!e->ev_wait) CK(e, cudaEventCreateWithFlags(&e->ev_wait, cudaEventDisableTiming));
+    CK(e, cudaEventRecord(e->ev_wait, cuda_stream ? (cudaStream_t)cuda_stream : cudaStreamLegacy));
+    CK(e, cudaStreamWaitEvent(e->stream, e->ev_wait, 0));
+    return PE_OK;
+}
+
+extern "C" int pe_pixels_to_bgr(const pe_pixel_format* fmt, const void* frame, uint8_t* bgr, long long cap) {
+    pe_pix::Layout L;
+    std::string why;
+    if (!pe_pix::layout_of(fmt, &L, &why)) return fail(nullptr, PE_ERR_INVALID, "%s", why.c_str());
+    if (!frame || !bgr) return fail(nullptr, PE_ERR_INVALID, "null frame or output");
+    if (cap < 3LL * L.w * L.h) return fail(nullptr, PE_ERR_INVALID, "cap %lld is below the %lld bytes of the BGR frame", cap, 3LL * L.w * L.h);
+    PixArgs a;
+    a.src[0] = (const uint8_t*)frame; a.dst = bgr; a.pitch = L.pitch; a.chroma = L.chroma; a.format = L.format; a.w = L.w; a.h = L.h;
+    pixels_to_bgr_host(a);
     return PE_OK;
 }
 
@@ -1194,28 +1262,15 @@ extern "C" int pe_forward_jpeg_coefs(pe_engine* e, const void* const* coefs, int
 
 // coefficient images in e->d_jcoef (n frames of W x H, `stride` bytes apart) -> display frames -> the net
 static int reconstruct_and_forward(pe_engine* e, int n, int W, int H, size_t stride, long long max_blocks, double* scale) {
-    int rc;
-    const bool display = W == e->cfg.disp_w && H == e->cfg.disp_h;
-    uint8_t* dst = e->d_frames;
-    if (!display) {   // reconstructed at the original size into the warpAffine source, as pe_forward_camera_frames uploads it
-        rc = prepare_warp(e, W, H); if (rc) return rc;
-        rc = grow_buffer(e, &e->d_raw, &e->raw_cap, (size_t)W * H * 3 * e->cfg.max_batch, false); if (rc) return rc;
-        dst = e->d_raw;
-    }
-    if (scale) *scale = display ? 1.0 : e->warp_scale;
+    uint8_t* dst;
+    int rc = frame_target(e, W, H, &dst, scale); if (rc) return rc;
     const size_t pstride = ((size_t)max_blocks * 64 + 255) & ~(size_t)255;
     rc = grow_buffer(e, &e->d_jplanes, &e->jplanes_cap, pstride * n, false); if (rc) return rc;
     JpegArgs ja;
     ja.coefs = e->d_jcoef; ja.coef_stride = (long long)stride; ja.planes = e->d_jplanes; ja.plane_stride = (long long)pstride;
     ja.dst = dst; ja.W = W; ja.H = H; ja.n = n; ja.max_blocks = max_blocks;
     e->launches += launch_jpeg_reconstruct(ja, e->stream);
-    if (!display) {
-        WarpArgs w;
-        w.src = e->d_raw; w.dst = e->d_frames; w.sw = W; w.sh = H; w.dw = e->cfg.disp_w; w.dh = e->cfg.disp_h;
-        w.adelta = e->d_wa; w.bdelta = e->d_wb; w.x0 = e->d_wx0; w.y0 = e->d_wy0; w.tab = e->d_wtab;
-        e->launches += launch_warp_affine(w, n, e->stream);
-    }
-    return pe_forward_frames_device(e, e->d_frames, n);
+    return finish_frames(e, n, W, H);
 }
 
 // Scan images -> coefficient images in e->d_jcoef (the entropy kernels), the per-frame status queued into e->h_jstatus.  Everything the

@@ -139,6 +139,17 @@ struct JpegScanArgs {
 size_t jpeg_huff_tables_bytes();
 int launch_jpeg_entropy(const JpegScanArgs& a, cudaStream_t st);   // 3 launches
 
+// ---- decoder-format frames (pixels.cu): pe_pixel_format frames -> tight uint8 BGR
+constexpr int PIX_MAX_FRAMES = 64;                  // = the largest max_batch: the pointer table travels in the kernel parameters
+struct PixArgs {
+    const uint8_t* src[PIX_MAX_FRAMES];             // [n] frame starts (device pointers; the host reference reads src[0])
+    uint8_t* dst;                                   // [n][h][w][3]
+    long long pitch, chroma;                        // a checked pe_pix::Layout's
+    int format, w, h;
+};
+int launch_pixels_to_bgr(const PixArgs& a, int n, cudaStream_t st);   // PE_PIX_RGB, _YUYV, _NV12, _I420
+void pixels_to_bgr_host(const PixArgs& a);                         // every format, frame src[0]
+
 // ---- convolution / pooling (conv_simt.cu, conv_tc.cu, pool.cu)
 int launch_conv_simt(const ConvArgs& a, cudaStream_t st);
 struct PoolArgs {

@@ -22,6 +22,8 @@ PREC_FP32_SIMT, PREC_BF16X1, PREC_BF16X2, PREC_BF16X3 = 0, 1, 2, 3
 PREC_F16X2 = PREC_BF16X2   # the parity mode: 2 fp16 planes, chunked round-to-nearest accumulation (poseengine.h)
 PREC_F16X1 = 4             # the fast mode: the parity mode's hi plane alone, one MMA per MAC (poseengine.h)
 MAX_PEOPLE = 96
+# pixel formats of forward_pixels / pixels_to_bgr (PE_PIX_*, poseengine.h)
+PIX_BGR, PIX_RGB, PIX_YUYV, PIX_NV12, PIX_I420 = 0, 1, 2, 3, 4
 
 _f32p = np.ctypeslib.ndpointer(dtype=np.float32, flags="C_CONTIGUOUS")
 
@@ -30,6 +32,10 @@ class _Config(C.Structure):
     _fields_ = [("device", C.c_int), ("model", C.c_int), ("net_w", C.c_int), ("net_h", C.c_int), ("disp_w", C.c_int),
                 ("disp_h", C.c_int), ("num_scales", C.c_int), ("start_scale", C.c_double), ("scale_gap", C.c_double),
                 ("max_batch", C.c_int), ("precision", C.c_int)]
+
+
+class _PixelFormat(C.Structure):
+    _fields_ = [("format", C.c_int), ("width", C.c_int), ("height", C.c_int), ("pitch", C.c_longlong), ("chroma_offset", C.c_longlong)]
 
 
 class PoseEngineError(RuntimeError):
@@ -59,6 +65,7 @@ ABI_SYMBOLS = [
     "pe_camera_open", "pe_camera_close", "pe_camera_info", "pe_camera_grab", "pe_camera_last_error", "pe_yuyv_to_bgr",
     "pe_compare_results", "pe_jpeg_read_coefs", "pe_jpeg_coefs_to_bgr", "pe_forward_jpeg_coefs", "pe_video_read_coefs",
     "pe_jpeg_read_scan", "pe_jpeg_scan_to_coefs_host", "pe_forward_jpeg_scans", "pe_jpeg_decode_scans", "pe_video_read_scan",
+    "pe_forward_pixels", "pe_stream_wait", "pe_pixels_to_bgr",
 ]
 
 
@@ -152,6 +159,9 @@ def lib():
     L.pe_forward_jpeg_scans.argtypes = L.pe_forward_jpeg_coefs.argtypes
     L.pe_jpeg_decode_scans.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_int)]
     L.pe_video_read_scan.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_longlong]
+    L.pe_forward_pixels.argtypes = [C.c_void_p, C.POINTER(_PixelFormat), C.POINTER(C.c_void_p), C.c_int, C.POINTER(C.c_double)]
+    L.pe_stream_wait.argtypes = [C.c_void_p, C.c_void_p]
+    L.pe_pixels_to_bgr.argtypes = [C.POINTER(_PixelFormat), C.c_void_p, C.c_void_p, C.c_longlong]
     L.pe_video_read_scan.restype = C.c_longlong
     if hasattr(L, "pe_video_open") or "PE_LIB" not in os.environ:   # an older A/B build (PE_LIB) may predate the video reader
         L.pe_video_open.argtypes = [C.c_char_p, C.POINTER(C.c_void_p)]
@@ -287,11 +297,13 @@ class PoseEngine:
         self.resize_layer = ImResizeLayer(self)
         self.model_descriptor = ModelDescriptorFactory.createModelDescriptor(model)
         self._keep = None
+        self._held = []   # frames forward_pixels reads asynchronously: released by the next fetch, sync or close
 
     def close(self):
         if getattr(self, "_h", None):
             lib().pe_destroy(self._h)
             self._h = None
+        self._held = []
 
     def __del__(self):
         try:
@@ -380,6 +392,28 @@ class PoseEngine:
         self._ck(fn(self._h, ptrs, len(bufs), C.byref(s)))
         return s.value
 
+    def forward_pixels(self, frames, fmt, chroma_offset=None):
+        """frames: numpy arrays or torch tensors (host or CUDA) of one format and size, in cv2's shapes: (h*3/2, w) for PIX_NV12 /
+        PIX_I420, (h, w, 2) for PIX_YUYV, (h, w, 3) for PIX_RGB / PIX_BGR.  The row stride is the pitch, so a column slice of a
+        wider allocation is read in place (an I420 array of that shape is copied unless tight: its chroma rows are not pitch/2
+        apart).  chroma_offset (NV12 / I420): the frames are the (h, w) luma planes, the row stride is the pitch, and the chroma plane
+        starts chroma_offset bytes after each frame's start, e.g. pitch * 1088 in a 1080p NVDEC surface; the caller vouches that
+        the allocation reaches that far.  Converted to BGR on the GPU
+        as cv2.cvtColor does, then as forward_camera_frames.  CUDA frames are read on the engine's stream after the work queued so
+        far on torch's current stream.  Returns frame.scale."""
+        views = [_pixel_view(f, fmt, chroma_offset) for f in frames]
+        pf = views[0][1]
+        if any((v[1].width, v[1].height, v[1].pitch) != (pf.width, pf.height, pf.pitch) for v in views):
+            raise ValueError("forward_pixels: the frames of one call share their size and row stride")
+        for dev in {v[3] for v in views if v[3] is not None and v[3].index == self.cfg.device}:
+            import torch
+            self._ck(lib().pe_stream_wait(self._h, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+        self._held.extend(v[2] for v in views)
+        ptrs = (C.c_void_p * len(views))(*[v[0] for v in views])
+        s = C.c_double()
+        self._ck(lib().pe_forward_pixels(self._h, C.byref(pf), ptrs, len(views), C.byref(s)))
+        return s.value
+
     def decode_jpeg_scans(self, scans, subseq_bits=0):
         """Test hook: scan images (read_jpeg_scan) -> coefficient images decoded on the GPU (subseq_bits 0 = the default
         subsequence length).  Returns (list of coefficient images as uint8 arrays, list of statuses: 0, or 1 + the MCU of the
@@ -436,12 +470,14 @@ class PoseEngine:
 
     def sync(self):
         self._ck(lib().pe_sync(self._h))
+        self._held = []
 
     def fetch(self, idx=0):
         joints = np.zeros((MAX_PEOPLE, self.num_parts, 3), np.float32)
         peaks = np.zeros((self.num_parts, self.max_peaks + 1, 3), np.float32)
         n = C.c_int()
         self._ck(lib().pe_fetch(self._h, idx, joints, C.byref(n), peaks.ctypes.data_as(C.c_void_p)))
+        self._held = []
         return n.value, joints[:n.value].copy(), peaks
 
     def fetch_maps(self, n=1):
@@ -796,6 +832,54 @@ class VideoCapture:
             self.release()
         except Exception:
             pass
+
+
+def _pixel_view(frame, fmt, chroma_offset=None):
+    """(data pointer, _PixelFormat, the object that owns the pixels, torch device of a CUDA tensor or None) of a uint8 frame in
+    forward_pixels's shapes.  Frames whose pixels or channels are not adjacent in memory are copied first."""
+    if fmt not in (PIX_BGR, PIX_RGB, PIX_YUYV, PIX_NV12, PIX_I420):
+        raise ValueError("pixel format %r is not one of PIX_BGR .. PIX_I420" % (fmt,))
+    planar = fmt in (PIX_NV12, PIX_I420)
+    ch = 1 if planar else (2 if fmt == PIX_YUYV else 3)
+    is_np = isinstance(frame, np.ndarray)
+    if not is_np:
+        import torch
+        if not torch.is_tensor(frame):
+            raise TypeError("frames are numpy arrays or torch tensors")
+    if (frame.dtype != np.uint8) if is_np else (frame.dtype != torch.uint8):
+        raise TypeError("frames are uint8, not %s" % frame.dtype)
+    shape = tuple(frame.shape)
+    if shape[2:] != (() if planar else (ch,)) or len(shape) < 2:
+        raise ValueError("frame shape %s does not fit format %d" % (shape, fmt))
+
+    def strides(f):
+        return tuple(f.strides) if is_np else tuple(f.stride())
+    h, w = shape[0], shape[1]
+    st = strides(frame)
+    # In cv2's (h*3/2, w) I420 array one row holds two chroma rows, so only a tight one has the layout's pitch/2 chroma rows
+    tight_i420 = fmt == PIX_I420 and chroma_offset is None
+    if (w > 1 and st[1] != ch) or (not planar and st[2] != 1) or (h > 1 and st[0] < w * ch) or (tight_i420 and h > 1 and st[0] != w):
+        frame = np.ascontiguousarray(frame) if is_np else frame.contiguous()
+        st = strides(frame)
+    if planar and chroma_offset is None:
+        if h % 3:
+            raise ValueError("a %s frame has h*3/2 rows, not %d" % ("NV12" if fmt == PIX_NV12 else "I420", h))
+        h = h * 2 // 3
+    pitch = st[0] if shape[0] > 1 else w * ch
+    ptr = frame.ctypes.data if is_np else frame.data_ptr()
+    dev = None if is_np or not frame.is_cuda else frame.device
+    return ptr, _PixelFormat(fmt, w, h, pitch, chroma_offset or 0), frame, dev
+
+
+def pixels_to_bgr(frame, fmt):
+    """cv2.cvtColor of a host frame in forward_pixels's shapes to uint8 BGR (h, w, 3): the host reference of the GPU conversion."""
+    ptr, pf, frame, dev = _pixel_view(frame, fmt)
+    if dev is not None:
+        raise ValueError("pixels_to_bgr takes host frames")
+    out = np.empty((pf.height, pf.width, 3), np.uint8)
+    if lib().pe_pixels_to_bgr(C.byref(pf), ptr, out.ctypes.data, out.size) != 0:
+        raise PoseEngineError("pe_pixels_to_bgr: %s" % lib().pe_last_error(None).decode())
+    return out
 
 
 def yuyv_to_bgr(yuyv):
