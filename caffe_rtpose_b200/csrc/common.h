@@ -21,6 +21,9 @@ namespace pe {
 // stride-1 convolution with zero padding is a CONSTANT ROW SHIFT (r-pad)*Wp + (s-pad) of the whole
 // matrix: the implicit-GEMM A operand of every tap is a plain 2-D tile (one TMA box), and Caffe's
 // zero padding (im2col.cpp:35-46) falls out of the zero gap rows / TMA out-of-bounds fill.
+// That holds only while pad <= gap: a larger pad reaches into the previous / next row or image.  So the
+// plan sets each level's gap to max(1, largest pad of a convolution at that level) (NetPlan::gap; 1, 1, 1, 3
+// for the built-in graphs, whose VGG levels run 3x3 and whose stride-8 stages run 7x7).
 // ---------------------------------------------------------------------------------------------
 struct Geo {
     int W, H, gap, Wp, Hs, N;
@@ -74,6 +77,7 @@ struct NetPlan {
     std::vector<OpRef> order;
     std::vector<BlobRef> blobs;
     int input_act = 0;
+    int gap[4] = {1, 1, 1, 1};   // per level: max(1, largest conv pad at that level), see Geo
 };
 struct NetDef;
 // plan from a parsed prototxt / built-in definition; -1 and a message when the graph is outside the supported family

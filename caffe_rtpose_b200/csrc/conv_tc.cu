@@ -450,8 +450,9 @@ static EncodeTiledFn get_encode() {
     return fn;
 }
 
+// Never below cout: the packed weights, the biases and the grid's N tiles all span cout_pad channels.
 int tc_cout_pad(int cout) {
-    if (cout >= 128) return (cout + 127) / 128 * 128;
+    if (cout > 64) return (cout + 127) / 128 * 128;
     if (cout > 48) return 64;
     if (cout > 32) return 48;
     if (cout > 16) return 32;

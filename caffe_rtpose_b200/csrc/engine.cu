@@ -238,7 +238,8 @@ static void set_post_params(pe_engine* e) {
 
 // Host-only view of the execution plan a prototxt (or, with path == NULL, the built-in graph of `model`) produces: one
 // line per op, "conv <name> cout cin k relu level in_act in_cused out_act out_coff planar_coff", "pool <name> in out",
-// "copy src dst channels", then "nms threshold max_peaks num_parts" and "resize start_scale scale_gap".  No GPU needed.
+// "copy src dst channels", then "gap level g" per resolution level (the flat layout's gap, common.h), "nms threshold
+// max_peaks num_parts" and "resize start_scale scale_gap".  No GPU needed.
 extern "C" int pe_plan_describe(int model, const char* prototxt_path, char* buf, int cap) {
     NetDef net;
     std::string err;
@@ -262,6 +263,10 @@ extern "C" int pe_plan_describe(int model, const char* prototxt_path, char* buf,
         } else {
             snprintf(t, sizeof t, "copy %d %d %d\n", p.copies[op.idx].src_act, p.copies[op.idx].dst_act, p.copies[op.idx].channels);
         }
+        s += t;
+    }
+    for (int l = 0; l < 4; l++) {
+        snprintf(t, sizeof t, "gap %d %d\n", l, p.gap[l]);
         s += t;
     }
     snprintf(t, sizeof t, "nms %g %d %d\nresize %g %g\n", p.nms_threshold, p.nms_max_peaks, p.nms_num_parts, p.resize_start_scale, p.resize_scale_gap);
@@ -334,14 +339,15 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
     CKC(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
     for (int i = 0; i < 16; i++) CKC(cudaEventCreate(&e->ev[i]));
 
+    // the plan first: each level's gap is the largest pad of its convolutions (common.h)
+    e->plan = prototxt_path ? proto_plan : build_plan(cfg->model, e->fmt.planes ? 64 : 32, e->fmt.planes ? 64 : 16);
     const int N = cfg->max_batch * cfg->num_scales;
     int w = cfg->net_w, h = cfg->net_h;
     for (int l = 0; l < 4; l++) {
-        e->geo[l] = make_geo(w, h, l == 3 ? 3 : 1, N);
+        e->geo[l] = make_geo(w, h, e->plan.gap[l], N);
         w = pooled(w); h = pooled(h);
     }
     if (e->geo[3].W * 8 != cfg->net_w || e->geo[3].H * 8 != cfg->net_h) { fail(e, PE_ERR_INVALID, "net size not divisible by 8 after pooling"); return bail(PE_ERR_INVALID); }
-    e->plan = prototxt_path ? proto_plan : build_plan(cfg->model, e->fmt.planes ? 64 : 32, e->fmt.planes ? 64 : 16);
     e->hw.resize(e->plan.convs.size());
     if (e->fmt.planes && setup_lanes(e)) return bail(PE_ERR_CUDA);
     // FLOPs (SURVEY.md section 8d): 2*Cout*Cin*k^2*Hout*Wout per conv and image

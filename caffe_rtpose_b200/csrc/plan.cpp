@@ -307,6 +307,8 @@ int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, s
         }
     }
     if (p.convs.empty() || !p.convs[0].im2col_input) return fail("the first layer must be a convolution on the net input");
+    // A tap is a constant row shift of the flat padded layout only while pad <= gap (common.h, Geo)
+    for (const ConvSpec& c : p.convs) p.gap[c.level] = std::max(p.gap[c.level], c.pad);
     // Every forward runs the whole order, so a blob whose channels a later op writes (a stage output in a ping-pong concat
     // buffer that a later stage reuses) holds that op's data after the forward: record the first such op.
     for (BlobRef& b : p.blobs)

@@ -14,7 +14,7 @@ there, and those tests ran with zero biases.  Here each layer L is checked alone
 The pixels: every pixel of the first and the last 128-row M tile (the last one partial), of every tile that straddles two
 images of a batch, the image borders (x, y in {0, 1, W-2, W-1} / {0, 1, H-2, H-1}, where the zero padding comes from gap rows
 and TMA out-of-bounds fill) and 1000 random ones.  Tiles are located in the flat padded layout of common.h: row
-m = (n*Hs + y)*Wp + x, Wp = W + gap, Hs = H + gap, gap 1 on the VGG levels and 3 at stride 8.
+m = (n*Hs + y)*Wp + x, Wp = W + gap, Hs = H + gap, with the plan's gap (plan_gaps: 1 on the VGG levels and 3 at stride 8).
 
 Error model (u = 2^-24; derived from the code, per product a*w and relative to mag):
   P=2 (fp16 hi + lo planes, conv_tc.cu)
@@ -52,6 +52,7 @@ Measured on one H100 80GB HBM3 (700 W power limit), largest |got - ref| / mag ov
   conv1_1 direct (fp32 CUDA cores, P=2 output): 2.92e-7.  Calibrated range nets at 160x96 (P=2, half width): within the P=2 row.
   P=1       7.18e-4 (BN 128) 1.87e-3/1.39e-3  3.02e-3 (BN 128)                   4.67e-3 (B = 7.9e-3; held to B only)
 """
+import functools
 import json
 import os
 
@@ -170,9 +171,10 @@ def netspec(model):
         return json.load(f)
 
 
-def conv_layers(model):
-    """[dict(name, bottom, top, k, relu, level)] in prototxt order, plus the Concat layers by top and the final concat."""
-    spec = netspec(model)
+def conv_layers(model, spec=None):
+    """[dict(name, bottom, top, k, relu, level)] in prototxt order, plus the Concat layers by top and the final concat.
+    spec: a layer table in the netspec format (default: the shipped graph of `model`)."""
+    spec = spec or netspec(model)
     layers = spec["layers"]
     relu = {l["bottom"][0] for l in layers if l["type"] == "ReLU"}
     concat = {l["top"][0]: l["bottom"] for l in layers if l["type"] == "Concat"}
@@ -208,7 +210,7 @@ def checked_layers(model):
 
 # Restated from conv_tc.cu (tc_cout_pad, tc_bn, tc_layer_launch): the tile width a layer runs at.
 def tc_cout_pad(cout):
-    if cout >= 128:
+    if cout > 64:
         return (cout + 127) // 128 * 128
     return 64 if cout > 48 else 48 if cout > 32 else 32 if cout > 16 else 16
 
@@ -225,11 +227,20 @@ def tc_instance(cout, ksize, M, planes, nsm, share=2):
     return bn, planes, 128 if ksize == 1 else 136
 
 
-def level_geo(net_w, net_h, level):
+@functools.lru_cache(maxsize=None)
+def plan_gaps(model=engine.COCO_18, prototxt=None):
+    """[gap of level 0..3] of the flat padded layout, as the plan prints it (`gap <level> <g>` lines of pe_plan_describe)."""
+    text = engine.plan_describe(model=None if prototxt else model, prototxt=prototxt)
+    gaps = {int(l.split()[1]): int(l.split()[2]) for l in text.splitlines() if l.startswith("gap ")}
+    return [gaps[l] for l in range(4)]
+
+
+def level_geo(net_w, net_h, level, gaps=None):
+    """(W, H, gap) of a resolution level; gaps: plan_gaps() of the net (default: the built-in graphs, both the same)."""
     w, h = net_w, net_h
     for _ in range(level):
         w, h = (w + 1) // 2, (h + 1) // 2
-    return w, h, 3 if level == 3 else 1
+    return w, h, (gaps or plan_gaps())[level]
 
 
 # ------------------------------------------------------------------------------------------ GPU configurations
@@ -294,11 +305,11 @@ def frames_for(n, disp_w, disp_h):
 
 
 class Blobs:
-    """Blobs of the engine's last forward (first nimg images), fetched once each."""
+    """Blobs of the engine's last forward (first nimg images), fetched once each.  spec: as conv_layers."""
 
-    def __init__(self, eng, nimg, model, W):
+    def __init__(self, eng, nimg, model, W, spec=None):
         self.eng, self.nimg, self.cache = eng, nimg, {}
-        _, self.concat, final = conv_layers(model)
+        _, self.concat, final = conv_layers(model, spec)
         self.final_off, off = {}, 0
         for b in self.concat[final]:      # the last stage's outputs: channel slices of the planar maps (concat_stage7)
             c = W[b][0].shape[0]

@@ -35,7 +35,7 @@ CLUSTER = 2   # conv_tc.cu TC_CLUSTER: CTAs along M that share each weight tile 
 
 
 def tc_cout_pad(cout):
-    if cout >= 128:
+    if cout > 64:
         return (cout + 127) // 128 * 128
     return 64 if cout > 48 else 48 if cout > 32 else 32 if cout > 16 else 16
 
@@ -59,6 +59,7 @@ def l2_smem_bytes(cout, cin, k, H, W, gap, nimg, planes=2, cluster=CLUSTER):
 def layer_bytes(model, nimg):
     """{conv name: L2 -> shared-memory bytes} of one forward of nimg frames at the benchmark's net size."""
     out = {}
+    gaps = {int(l.split()[1]): int(l.split()[2]) for l in engine.plan_describe(model=model).splitlines() if l.startswith("gap ")}
     for name, co, ci, k in synth.conv_table(model):
         level = 0 if name.startswith("conv1") else 1 if name.startswith("conv2") else 2 if name.startswith("conv3") else 3
         w, h = NET_W, NET_H
@@ -66,7 +67,7 @@ def layer_bytes(model, nimg):
             w, h = (w + 1) // 2, (h + 1) // 2
         if name == "conv1_1":   # runs on the im2col'ed input: a 1x1 conv over 27 channels, padded to 64
             ci, k = 27, 1
-        out[name] = l2_smem_bytes(co, ci, k, h, w, 3 if level == 3 else 1, nimg)
+        out[name] = l2_smem_bytes(co, ci, k, h, w, gaps[level], nimg)
     return out
 
 
