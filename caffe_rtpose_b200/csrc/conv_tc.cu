@@ -463,11 +463,6 @@ int tc_cout_pad(int cout) {
 // Three planes (bf16x3, kept for A/B comparisons) stay at 64.
 static int tc_bn(int cout_pad, int planes) { return std::min(cout_pad, planes == 3 ? 64 : 128); }
 
-static int env_int(const char* name, int dflt) {
-    const char* v = getenv(name);
-    return v ? atoi(v) : dflt;
-}
-
 template <int BN, int PLANES, bool F16>
 static int launch_inst(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap) {
     auto kern = conv_wg_kernel<BN, PLANES, F16>;
@@ -497,7 +492,7 @@ template <int BN>
 static int launch_bn(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap) {
     const PlaneFmt f = l.d.fmt;
     if (f.planes == 1) return f.f16 ? launch_inst<BN, 1, true>(l, a, grid, st, bmap) : launch_inst<BN, 1, false>(l, a, grid, st, bmap);
-    if (f.planes == 2 && f.f16 == PARITY_F16) return launch_inst<BN, 2, PARITY_F16>(l, a, grid, st, bmap);
+    if (f.planes == 2 && f.f16) return launch_inst<BN, 2, true>(l, a, grid, st, bmap);
     if constexpr (BN <= 64) { if (f.planes == 3 && !f.f16) return launch_inst<BN, 3, false>(l, a, grid, st, bmap); }
     return -1;   // no kernel for this tile width and plane format (tc_bn never picks one)
 }
@@ -566,9 +561,8 @@ int tc_layer_launch(const TcLayer& l, int nimg, cudaStream_t st, int share) {
     // efficiency of the shape) is larger.  share: layers running concurrently on other streams take their part of the SMs.
     const long long mt = (a.M + TC_BM - 1) / TC_BM;
     const long long sms = std::max(1, nsm / (share < 1 ? 1 : share));
-    static const int narrow_env = env_int("PE_TC_NARROW", 1);
     int bn = l.bn, bmap = 1;
-    if (narrow_env && l.bn >= 64) {
+    if (l.bn >= 64) {
         const double sfull = (double)std::min<long long>(mt * (d.cout_pad / l.bn), sms) * 1.00;
         const double shalf = (double)std::min<long long>(mt * (d.cout_pad / (l.bn / 2)), sms) * 0.80;
         if (shalf > sfull) { bn = l.bn / 2; bmap = 2; }

@@ -55,12 +55,6 @@ struct pe_engine {
     unsigned* d_range = nullptr;
     bool calibrated = false, check_range = false;
     std::vector<size_t> w_off, b_off;
-    size_t w11_off = 0;             // fp32 [27][64] weights + 64 biases of conv1_1 for the direct kernel (0: not packed)
-    float w11_scale = 1.f;          // activation scale currently folded into that copy
-    bool conv11_direct = false;     // PE_CONV11_DIRECT=1: conv1_1 by conv1_1_direct_kernel (fp32 CUDA cores, no im2col'ed input) instead of
-                                    // the im2col + implicit-GEMM path (the tensor path is the default)
-    bool input_from_frames = false; // the last forward came from uint8 frames: d_resized holds conv1_1's input
-    bool input_act_stale = false;   // ... and the im2col'ed input activation was not produced (conv1_1 direct)
     std::vector<int> cout_pad, cin_pad;
     std::vector<TcLayer> tc;        // wgmma per-conv launch state
     // io
@@ -92,7 +86,7 @@ struct pe_engine {
     // decoder-format host frames (pe_forward_pixels) copied to the device before conversion; pe_stream_wait's event
     uint8_t* d_pix = nullptr; size_t pix_cap = 0;
     cudaEvent_t ev_wait = nullptr;
-    bool input_lo_dirty = false;
+    bool input_lo_dirty = false;   // the planar-input path wrote non-zero lo planes / channels >= 32 of the input buffer
     // JPEG coefficient images (pe_forward_jpeg_coefs): device copies, pinned staging for pageable callers, component planes
     uint8_t* d_jcoef = nullptr; size_t jcoef_cap = 0; uint8_t* h_jcoef = nullptr; size_t h_jcoef_cap = 0;
     uint8_t* d_jplanes = nullptr; size_t jplanes_cap = 0;
@@ -109,7 +103,7 @@ struct pe_engine {
     // any setter whose value is baked into kernel arguments.
     struct GraphEntry { cudaGraphExec_t exec = nullptr; long long launches = 0; int seen = 0; };
     std::map<int, GraphEntry> graphs;
-    bool use_graphs = true;   // the planar-input path wrote non-zero lo planes / channels >= 32 of the input buffer
+    bool use_graphs = true;   // cleared when capture or instantiation fails: every later forward runs eagerly
     long long launches = 0;
     std::string err;
     double flops_per_scale = 0;
@@ -334,8 +328,6 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
     if (prototxt_path) e->mt_own.max_peaks = proto_plan.nms_max_peaks;   // nms_param.max_peaks (NmsLayer::GetMaxPeaks, rtpose.cpp:195)
     e->mt = &e->mt_own;
     e->fmt = plane_fmt(cfg->precision);
-    if (const char* g = getenv("PE_GRAPH")) e->use_graphs = atoi(g) != 0;
-    if (const char* g = getenv("PE_CONV11_DIRECT")) e->conv11_direct = atoi(g) != 0;
     if (const char* g = getenv("PE_CHECK_RANGE")) e->check_range = atoi(g) != 0;
     e->elem = e->fmt.planes == 0 ? 4 : 2;
     e->start_scale_f = (float)cfg->start_scale;  // ImResizeLayer::SetStartScale(float)
@@ -566,11 +558,6 @@ static size_t packed_layout(pe_engine* e) {
         e->b_off[i] = total;
         total = align256(total + (size_t)(e->cout_pad[i] + 1) * 4);   // bias[cout_pad] + the layer's epilogue scale
     }
-    e->w11_off = 0;
-    if (nc && e->plan.convs[0].im2col_input && e->plan.convs[0].cout == 64 && e->plan.convs[0].k == 3) {
-        e->w11_off = total;                                   // travels with the packed buffer (weight broadcast)
-        total = align256(total + (27 * 64 + 64) * sizeof(float));
-    }
     return total;
 }
 
@@ -692,18 +679,10 @@ extern "C" int pe_commit_weights(pe_engine* e) {
     }
     const size_t total = packed_layout(e);
     e->bias_true.assign(nc, std::vector<float>());
-    e->w11_scale = 1.f; e->calibrated = false;
+    e->calibrated = false;
     e->wsi.assign(nc, 1.f);
     e->conv_scale.assign(nc, 1.f);
     std::vector<uint8_t> host(total, 0);
-    if (e->w11_off) {   // wT[k][co], k = c*9 + kh*3 + kw: Caffe's im2col row order (im2col.cpp:19-55)
-        float* wT = (float*)(host.data() + e->w11_off);
-        const HostWeights& h0 = e->hw[0];
-        for (int co = 0; co < 64; co++) {
-            for (int k = 0; k < 27; k++) wT[k * 64 + co] = h0.w[(size_t)co * 27 + k];
-            wT[27 * 64 + co] = h0.b[co];
-        }
-    }
     for (size_t i = 0; i < nc; i++) {
         pack_conv_weights(e, (int)i, host.data() + e->w_off[i]);
         e->bias_true[i] = e->hw[i].b;
@@ -869,14 +848,6 @@ static int run_op(pe_engine* e, const OpRef& op, int nimg, cudaStream_t st = nul
         const ConvSpec& c = e->plan.convs[op.idx];
         const Geo& g = e->geo[c.level];
         const long long M = (long long)nimg * g.Hs * g.Wp;
-        if (op.idx == 0 && c.im2col_input && e->conv11_direct && e->input_from_frames && e->w11_off && c.out_act >= 0) {
-            PreArgs a = e->pre;
-            a.nframes = nimg / e->cfg.num_scales;
-            const float* wT = (const float*)((const char*)e->d_packed + e->w11_off);
-            e->launches += launch_conv1_1_direct(a, wT, wT + 27 * 64, e->acts[c.out_act], e->plan.acts[c.out_act].C, e->act_plane[c.out_act],
-                                                 c.relu, nimg, st);
-            return PE_OK;
-        }
         if (e->fmt.planes) {
             const int n = tc_layer_launch(e->tc[op.idx], nimg, st, share);
             if (n < 0) return fail(e, PE_ERR_CUDA, "conv %s: tensor-core launch failed or no kernel fits the tile (%s)", c.name.c_str(), cudaGetErrorString(cudaGetLastError()));
@@ -955,7 +926,6 @@ static int setup_lanes(pe_engine* e) {
     e->conv_done.assign(nc, nullptr);
     e->last_lane1_conv = -1;
     e->two_lanes = false;
-    if (const char* g = getenv("PE_TWO_LANES")) { if (atoi(g) == 0) return PE_OK; }
     std::vector<int> conv_lane(nc, 0);
     int n1 = 0;
     for (size_t i = 0; i < nc; i++) {
@@ -1043,11 +1013,7 @@ extern "C" int pe_forward_frames_device(pe_engine* e, const void* d_frames, int 
         CK(e, cudaMemsetAsync(e->acts[e->plan.input_act], 0, bytes, e->stream));
         e->input_lo_dirty = false;
     }
-    const bool direct = e->conv11_direct && e->w11_off && e->plan.convs[0].out_act >= 0;
-    e->launches += launch_preprocess(a, e->stream, !direct);
-    if (!e->input_from_frames) drop_graphs(e);   // graphs captured on the planar-input path hold the other conv1_1 kernel
-    e->input_from_frames = true;
-    e->input_act_stale = direct;
+    e->launches += launch_preprocess(a, e->stream);
     e->last_frames = (const uint8_t*)d_frames;
     return run_net(e, n);
 }
@@ -1438,51 +1404,38 @@ extern "C" int pe_calibrate(pe_engine* e, const uint8_t* const* frames, int n) {
         return fail(e, PE_ERR_STATE, "this handle received its weights by broadcast / sharing: calibrate the source handle before replicating");
     CK(e, cudaSetDevice(e->cfg.device));
     drop_graphs(e);
-    // frames -> device -> net input (the im2col path: conv1_1 is calibrated like every other layer)
+    // frames -> device -> net input
     const size_t fb = (size_t)e->cfg.disp_w * e->cfg.disp_h * 3;
     CK(e, cudaStreamSynchronize(e->stream));
     for (int i = 0; i < n; i++) { if (!frames[i]) return fail(e, PE_ERR_INVALID, "null frame %d", i); memcpy(e->h_frames + i * fb, frames[i], fb); }
     CK(e, cudaMemcpyAsync(e->d_frames, e->h_frames, fb * n, cudaMemcpyHostToDevice, e->stream));
     PreArgs a = e->pre;
     a.frames = e->d_frames; a.nframes = n;
-    const bool direct_was = e->conv11_direct;
-    e->conv11_direct = false;
-    e->launches += launch_preprocess(a, e->stream, true);
-    e->input_from_frames = true; e->input_act_stale = false; e->last_frames = e->d_frames;
+    e->launches += launch_preprocess(a, e->stream);
+    e->last_frames = e->d_frames;
     const int nimg = n * e->cfg.num_scales;
-    auto restore = [&](int code) { e->conv11_direct = direct_was; return code; };
     for (const OpRef& op : e->plan.order) {
-        if (op.type != 0) { if ((rc = run_op(e, op, nimg))) return restore(rc); continue; }
+        if (op.type != 0) { if ((rc = run_op(e, op, nimg))) return rc; continue; }
         const int i = op.idx;
         const ConvSpec& c = e->plan.convs[i];
         // the producers of this layer's input are final: fold their scales into the weights if they are not all equal to what is packed
         bool mixed = false;
         const float s_ref = input_ref_scale(e, c);
         for (int pc : c.cin_prod) if (pc >= 0 && e->conv_scale[pc] != s_ref) mixed = true;
-        if (mixed || e->calibrated) { if ((rc = upload_weights(e, i))) return restore(rc); }
+        if (mixed || e->calibrated) { if ((rc = upload_weights(e, i))) return rc; }
         if (c.out_act >= 0) {
             e->conv_scale[i] = 1.f;               // measure the true output range: fp32 epilogue values, before the fp16 split
-            if ((rc = upload_fields(e, i))) return restore(rc);
+            if ((rc = upload_fields(e, i))) return rc;
             CK(e, cudaMemsetAsync(e->d_range + i, 0, sizeof(unsigned), e->stream));
-            if ((rc = run_op(e, op, nimg))) return restore(rc);
+            if ((rc = run_op(e, op, nimg))) return rc;
             unsigned bits = 0;
             CK(e, cudaMemcpyAsync(&bits, e->d_range + i, sizeof bits, cudaMemcpyDeviceToHost, e->stream));
             CK(e, cudaStreamSynchronize(e->stream));
             float m; memcpy(&m, &bits, 4);
             if (m > 0.f && m < 3e38f) { int ex = 0; frexpf(m, &ex); e->conv_scale[i] = ldexpf(1.f, std::max(-100, std::min(100, 6 - ex))); }   // m * s in [32, 64)
         }
-        if ((rc = upload_fields(e, i))) return restore(rc);
-        if ((rc = run_op(e, op, nimg))) return restore(rc);
-    }
-    e->conv11_direct = direct_was;
-    if (e->w11_off) {   // the direct conv1_1 kernel has its own fp32 copy of the layer: fold the output scale into it
-        const float s_out = e->conv_scale[0];
-        std::vector<float> w(27 * 64 + 64);
-        CK(e, cudaMemcpy(w.data(), (char*)e->d_packed + e->w11_off, w.size() * sizeof(float), cudaMemcpyDeviceToHost));
-        const float rel = s_out / e->w11_scale;
-        for (float& v : w) v *= rel;
-        CK(e, cudaMemcpy((char*)e->d_packed + e->w11_off, w.data(), w.size() * sizeof(float), cudaMemcpyHostToDevice));
-        e->w11_scale = s_out;
+        if ((rc = upload_fields(e, i))) return rc;
+        if ((rc = run_op(e, op, nimg))) return rc;
     }
     CK(e, cudaMemsetAsync(e->d_range, 0, nc * sizeof(unsigned), e->stream));
     e->calibrated = true;
@@ -1539,9 +1492,6 @@ extern "C" int pe_forward_net_input(pe_engine* e, const float* net_input, int n)
     e->launches += launch_input_from_planar(e->d_planar, a, n * e->cfg.num_scales, e->stream);
     e->input_lo_dirty = e->fmt.planes > 0;
     e->last_frames = nullptr;
-    if (e->input_from_frames) drop_graphs(e);   // the captured graphs hold the other conv1_1 kernel
-    e->input_from_frames = false;
-    e->input_act_stale = false;
     return run_net(e, n);
 }
 extern "C" int pe_forward_maps(pe_engine* e, const float* maps8, int n) {
@@ -1701,12 +1651,6 @@ extern "C" int pe_fetch_blob(pe_engine* e, const char* blob_name, float* out, si
         if (w) *w = g.W;
         if (!out) return PE_OK;
         if (cnt > cap) return fail(e, PE_ERR_INVALID, "blob %s needs %zu floats", blob_name, cnt);
-        if (b.act == e->plan.input_act && e->input_act_stale) {   // conv1_1 ran from the uint8 images: materialise the net input on demand
-            PreArgs a = e->pre;
-            a.nframes = std::max(e->last_n, 1);
-            e->launches += launch_im2col_u8(a, e->stream);
-            e->input_act_stale = false;
-        }
         float* d = nullptr;
         CK(e, cudaMalloc(&d, cnt * sizeof(float)));
         // stored value = true value * conv_scale[producer] (pools pass their producer's scale through; the net input has none)

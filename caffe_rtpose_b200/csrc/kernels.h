@@ -10,15 +10,10 @@ namespace pe {
 // vs 3e-6 for fp16).  The fast mode (F16X1) is the parity mode's hi plane alone.  fp16's range (65504) needs the per-layer
 // power-of-two range scales of pe_calibrate for nets outside O(1e-2 .. 1e3); the bf16 modes (BF16X1, BF16X3) have fp32's range.
 struct PlaneFmt { int planes; bool f16; };
-#ifdef PE_PARITY_PLANES_BF16   // A/B build: parity mode on bf16 planes (8 + 8 bits, 2.1e-5 over the net), see DESIGN.md section 3
-constexpr bool PARITY_F16 = false;
-#else
-constexpr bool PARITY_F16 = true;
-#endif
 inline PlaneFmt plane_fmt(int precision) {   // PE_PREC_* -> format
     switch (precision) {
         case PE_PREC_BF16X1: return {1, false};
-        case PE_PREC_F16X2: return {2, PARITY_F16};
+        case PE_PREC_F16X2: return {2, true};
         case PE_PREC_BF16X3: return {3, false};
         case PE_PREC_F16X1: return {1, true};
         default: return {0, false};   // PE_PREC_FP32_SIMT
@@ -102,11 +97,7 @@ struct PreArgs {
     void* out; int kp; long long out_plane; PlaneFmt fmt;
     int Wp, Hs;
 };
-int launch_preprocess(const PreArgs& a, cudaStream_t st, bool with_im2col = true);
-int launch_im2col_u8(const PreArgs& a, cudaStream_t st);   // resized uint8 images -> im2col'ed input activation (second half of launch_preprocess)
-// conv1_1 from the resized uint8 images (fp32 CUDA cores); wT = [27][64] weights in (c, kh, kw) order, k-major
-int launch_conv1_1_direct(const PreArgs& a, const float* wT, const float* bias, void* out, int out_pitch, long long out_plane, int relu,
-                          int nimages, cudaStream_t st);
+int launch_preprocess(const PreArgs& a, cudaStream_t st);
 struct WarpArgs {
     const uint8_t* src; uint8_t* dst; int sw, sh, dw, dh;
     const int* adelta; const int* bdelta; const int* x0; const int* y0;   // OpenCV's fixed-point coordinate tables

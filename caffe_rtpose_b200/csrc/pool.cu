@@ -95,7 +95,7 @@ int launch_pool(const PoolArgs& a, cudaStream_t st) {
         const dim3 grid((per + 255) / 256, a.N);
         if (f.planes == 1 && f.f16) pool_planes_kernel<1, true><<<grid, 256, 0, st>>>(a);
         else if (f.planes == 1) pool_planes_kernel<1, false><<<grid, 256, 0, st>>>(a);
-        else if (f.planes == 2) pool_planes_kernel<2, PARITY_F16><<<grid, 256, 0, st>>>(a);
+        else if (f.planes == 2) pool_planes_kernel<2, true><<<grid, 256, 0, st>>>(a);
         else pool_planes_kernel<3, false><<<grid, 256, 0, st>>>(a);
     }
     return 1;

@@ -231,7 +231,7 @@ __global__ void __launch_bounds__(256) input_im2col_u8_kernel(PreArgs a) {
                           (uint32_t)k[q * 8 + 4] | ((uint32_t)k[q * 8 + 5] << 16), (uint32_t)k[q * 8 + 6] | ((uint32_t)k[q * 8 + 7] << 16));
 }
 
-int launch_im2col_u8(const PreArgs& a, cudaStream_t st) {
+static int launch_im2col_u8(const PreArgs& a, cudaStream_t st) {
     if (a.fmt.planes > 0 && a.kp >= 32) {
         const dim3 g((a.net_w + 31) / 32, (a.net_h + 7) / 8, a.nframes * a.S), b(32, 8);
         if (a.fmt.f16) input_im2col_u8_kernel<true><<<g, b, 0, st>>>(a);
@@ -242,120 +242,10 @@ int launch_im2col_u8(const PreArgs& a, cudaStream_t st) {
     input_im2col_kernel<0><<<dim3((work + 255) / 256, a.nframes * a.S), 256, 0, st>>>(a, nullptr, a.nframes * a.S);
     return 1;
 }
-int launch_preprocess(const PreArgs& a, cudaStream_t st, bool with_im2col) {
+int launch_preprocess(const PreArgs& a, cudaStream_t st) {
     dim3 g((a.net_w * a.net_h + 255) / 256, a.S, a.nframes);
     area_resize_kernel<<<g, 256, 0, st>>>(a);
-    if (!with_im2col) return 1;   // conv1_1 reads the resized uint8 images itself (conv1_1_direct_kernel)
     return 1 + launch_im2col_u8(a, st);
-}
-
-// ------------------------------------------------------------------------------------------------
-// conv1_1 (3 -> 64 channels, 3x3) straight from the resized uint8 images, fp32 FFMA on the CUDA cores.
-// As a tensor-core GEMM this layer is all memory traffic: K = 27 padded to 64 channels in two planes made it read
-// 560 MB of (mostly zero) im2col'ed input per 9-frame step to do 7.5 GFLOP (ncu r1n: 247 us, tensor pipe 10 %), after a
-// 160 us kernel had written that input.  Here one lane owns one pixel and all 64 output channels: the 27 patch values
-// come from a shared-memory tile of the normalised image (pad + v/256 - 0.5 as process_and_pad_image, rtpose.cpp:239-269;
-// zero outside the image = Caffe's conv padding), the weights are broadcast float4 loads, sums run in Caffe's im2col
-// order (c, kh, kw) in fp32 - exact fp32 products, so closer to the reference than the split-fp16 path - and the
-// result leaves as coalesced 512-byte rows (staged per warp through swizzled shared memory).
-// ------------------------------------------------------------------------------------------------
-template <int PLANES, bool F16>   // PLANES 0: fp32 activations, otherwise the plane format (kernels.h, PlaneFmt)
-__global__ void __launch_bounds__(256) conv1_1_direct_kernel(PreArgs a, const float* __restrict__ wT /*[27][64]*/, const float* __restrict__ bias,
-                                                              void* out, int out_pitch, long long out_plane, int relu) {
-    constexpr int TX = 32, TY = 8;
-    __shared__ float tile[3][TY + 2][TX + 2];
-    __shared__ __align__(16) float s_w[27 * 64];
-    __shared__ float s_b[64];
-    __shared__ __align__(1024) uint8_t s_stage[8][4096];
-    const int n = blockIdx.z;                      // image = frame * S + scale
-    const int s = n % a.S;
-    const AreaTab& t = a.tab[s];
-    const uint8_t* img = a.resized + (size_t)n * a.net_h * a.net_w * 3;
-    const int x0 = blockIdx.x * TX, y0 = blockIdx.y * TY;
-    const int tid = threadIdx.y * 32 + threadIdx.x;
-    for (int i = tid; i < 27 * 64; i += 256) s_w[i] = wT[i];
-    if (tid < 64) s_b[tid] = bias[tid];
-    for (int i = tid; i < 3 * (TY + 2) * (TX + 2); i += 256) {
-        const int c = i / ((TY + 2) * (TX + 2)), rem = i % ((TY + 2) * (TX + 2));
-        const int yy = y0 + rem / (TX + 2) - 1, xx = x0 + rem % (TX + 2) - 1;
-        float v = 0.f;
-        if (yy >= 0 && yy < a.net_h && xx >= 0 && xx < a.net_w) {
-            const int oy = yy - t.padh, ox = xx - t.padw;
-            if (oy >= 0 && oy < t.th && ox >= 0 && ox < t.tw)
-                v = __fsub_rn(__fmul_rn((float)img[((size_t)oy * t.tw + ox) * 3 + c], 0.00390625f), 0.5f);   // x/256 - 0.5, exact
-        }
-        tile[c][rem / (TX + 2)][rem % (TX + 2)] = v;
-    }
-    __syncthreads();
-    const int lx = threadIdx.x, ly = threadIdx.y;
-    const int y = y0 + ly;
-    float acc[64];
-#pragma unroll
-    for (int j = 0; j < 64; j++) acc[j] = 0.f;
-#pragma unroll 1
-    for (int c = 0; c < 3; c++)
-#pragma unroll
-        for (int rs = 0; rs < 9; rs++) {
-            const float v = tile[c][ly + rs / 3][lx + rs % 3];
-            const float4* w4 = (const float4*)(s_w + (c * 9 + rs) * 64);
-#pragma unroll
-            for (int j = 0; j < 16; j++) {
-                const float4 w = w4[j];
-                acc[4 * j] = __fmaf_rn(v, w.x, acc[4 * j]); acc[4 * j + 1] = __fmaf_rn(v, w.y, acc[4 * j + 1]);
-                acc[4 * j + 2] = __fmaf_rn(v, w.z, acc[4 * j + 2]); acc[4 * j + 3] = __fmaf_rn(v, w.w, acc[4 * j + 3]);
-            }
-        }
-#pragma unroll
-    for (int j = 0; j < 64; j++) {
-        float v = __fadd_rn(acc[j], s_b[j]);
-        if (relu) v = fmaxf(v, 0.f);
-        acc[j] = v;
-    }
-    if (y >= a.net_h) return;                      // whole warp (a warp is one image row of the tile)
-    const int nvalid = min(TX, a.net_w - x0);      // pixels of this warp inside the image
-    const long long m0 = ((long long)n * a.Hs + y) * a.Wp + x0;
-    if (PLANES == 0) {
-        if (lx < nvalid) {
-            float4* o = (float4*)((float*)out + (size_t)(m0 + lx) * out_pitch);
-#pragma unroll
-            for (int j = 0; j < 16; j++) o[j] = make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]);
-        }
-        return;
-    }
-    uint8_t* stage = s_stage[ly];
-#pragma unroll 1
-    for (int p = 0; p < PLANES; p++) {
-        // this plane of the lane's 64 channels -> 8 chunks of 16 bytes, SWIZZLE_128B order (conflict-free), residual stays in acc
-#pragma unroll
-        for (int ch = 0; ch < 8; ch++) {
-            uint32_t pk[4];
-#pragma unroll
-            for (int j = 0; j < 4; j++) pk[j] = split_pair<F16>(acc[ch * 8 + 2 * j], acc[ch * 8 + 2 * j + 1]);
-            *(uint4*)(stage + lx * 128 + ((ch ^ (lx & 7)) * 16)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-        }
-        __syncwarp();
-        // read back row-major: one instruction stores 4 complete 128-byte rows
-#pragma unroll
-        for (int i = 0; i < 8; i++) {
-            const int row = i * 4 + (lx >> 3), ch = lx & 7;
-            const uint4 v = *(const uint4*)(stage + row * 128 + ((ch ^ (row & 7)) * 16));
-            if (row < nvalid)
-                *(uint4*)((uint8_t*)out + ((size_t)p * out_plane + (size_t)(m0 + row) * out_pitch) * 2 + ch * 16) = v;
-        }
-        __syncwarp();
-    }
-}
-
-int launch_conv1_1_direct(const PreArgs& a, const float* wT, const float* bias, void* out, int out_pitch, long long out_plane, int relu,
-                          int nimages, cudaStream_t st) {
-    dim3 g((a.net_w + 31) / 32, (a.net_h + 7) / 8, nimages), b(32, 8);
-    const PlaneFmt f = a.fmt;
-    if (f.planes == 0) conv1_1_direct_kernel<0, false><<<g, b, 0, st>>>(a, wT, bias, out, out_pitch, out_plane, relu);
-    else if (f.planes == 1 && f.f16) conv1_1_direct_kernel<1, true><<<g, b, 0, st>>>(a, wT, bias, out, out_pitch, out_plane, relu);
-    else if (f.planes == 1) conv1_1_direct_kernel<1, false><<<g, b, 0, st>>>(a, wT, bias, out, out_pitch, out_plane, relu);
-    else if (f.planes == 2) conv1_1_direct_kernel<2, PARITY_F16><<<g, b, 0, st>>>(a, wT, bias, out, out_pitch, out_plane, relu);
-    else conv1_1_direct_kernel<3, false><<<g, b, 0, st>>>(a, wT, bias, out, out_pitch, out_plane, relu);
-    return 1;
 }
 
 int launch_input_from_planar(const float* planar, const PreArgs& a, int nimages, cudaStream_t st) {

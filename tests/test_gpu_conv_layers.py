@@ -32,7 +32,6 @@ Error model (u = 2^-24; derived from the code, per product a*w and relative to m
   P=1 (bf16, unit roundoff 2^-8): weights and output rounded to bf16 (2^-8 each), one truncating chain of <= 588 steps
       (2^-13.8): B = 2^-7 + 2^-11.
   SIMT fp32: fmaf over K = k*k*Cin products, then the bias: gamma_{K+1} = (K+1)u / (1 - (K+1)u).
-  conv1_1 direct (fp32 FMA over 27 taps + bias, stored as fp16 hi + lo at P=2): gamma_28 + 4u.
 The fetched input is the exact sum of the planes, so the rounding of the activations does not enter.  floor: at P=2 the
 output's lo plane can be an fp16 subnormal (spacing 2^-24 of the stored value = true value x the layer's range scale s):
 2^-24 / s.  Uncalibrated s = 1; after pe_calibrate s >= 32 / max|output|, so the floor is 2^-24 max|output| / 32.  (Weights
@@ -49,7 +48,7 @@ Measured on one H100 80GB HBM3 (700 W power limit), largest |got - ref| / mag ov
   P=2       1.08e-7/1.04e-7  3.07e-7/2.80e-7  3.42e-7 / 3.31e-7 / 2.6e-7-2.8e-7   2.64e-7 (BN 64)
   P=3       6.96e-8 (BN 64)  2.17e-7 (64)     2.14e-7 (64), 1.80e-7 (32)         8.33e-8
   SIMT      4.11e-7          3.25e-7          2.99e-7                            2.20e-7
-  conv1_1 direct (fp32 CUDA cores, P=2 output): 2.92e-7.  Calibrated range nets at 160x96 (P=2, half width): within the P=2 row.
+  Calibrated range nets at 160x96 (P=2, half width): within the P=2 row.
   P=1       7.18e-4 (BN 128) 1.87e-3/1.39e-3  3.02e-3 (BN 128)                   4.67e-3 (B = 7.9e-3; held to B only)
 """
 import functools
@@ -275,29 +274,22 @@ def weights_with_biases(model, kind="he", grow=1.0):
     return {k: (W0[k][0], Wb[k][1]) for k in W0}
 
 
-# name -> (model, net_w, net_h, precision, frame counts to run, env, calibrate with weights kind/grow)
+# name -> (model, net_w, net_h, precision, frame counts to run, calibrate with weights kind/grow)
 CONFIGS = {
-    "coco_p2": (engine.COCO_18, 656, 368, engine.PREC_F16X2, (1, 2), {}, None),
-    "mpi_p2": (engine.MPI_15, 496, 368, engine.PREC_F16X2, (1, 3), {}, None),
-    "coco_p3": (engine.COCO_18, 656, 368, engine.PREC_BF16X3, (2,), {}, None),
-    "coco_p1": (engine.COCO_18, 656, 368, engine.PREC_BF16X1, (2,), {}, None),
-    "coco_simt": (engine.COCO_18, 656, 368, engine.PREC_FP32_SIMT, (2,), {}, None),
-    "coco_conv11_direct": (engine.COCO_18, 656, 368, engine.PREC_F16X2, (1,), {"PE_CONV11_DIRECT": "1"}, None),
-    "range_caffe_filler": (engine.COCO_18, 160, 96, engine.PREC_F16X2, (1,), {}, ("caffe", 1.0)),
-    "range_growing": (engine.COCO_18, 160, 96, engine.PREC_F16X2, (1,), {}, ("he", 1.6)),
+    "coco_p2": (engine.COCO_18, 656, 368, engine.PREC_F16X2, (1, 2), None),
+    "mpi_p2": (engine.MPI_15, 496, 368, engine.PREC_F16X2, (1, 3), None),
+    "coco_p3": (engine.COCO_18, 656, 368, engine.PREC_BF16X3, (2,), None),
+    "coco_p1": (engine.COCO_18, 656, 368, engine.PREC_BF16X1, (2,), None),
+    "coco_simt": (engine.COCO_18, 656, 368, engine.PREC_FP32_SIMT, (2,), None),
+    "range_caffe_filler": (engine.COCO_18, 160, 96, engine.PREC_F16X2, (1,), ("caffe", 1.0)),
+    "range_growing": (engine.COCO_18, 160, 96, engine.PREC_F16X2, (1,), ("he", 1.6)),
 }
 # largest |got - ref| / mag per layer class, 2-2.5x the H100's measured values (module docstring); P=1 is held to B only
 MEASURED_MAX = {
-    engine.PREC_F16X2: {"7x7": 2.5e-7, "3x3": 7e-7, "1x1": 8e-7, "im2col": 6e-7, "direct": 7e-7},
+    engine.PREC_F16X2: {"7x7": 2.5e-7, "3x3": 7e-7, "1x1": 8e-7, "im2col": 6e-7},
     engine.PREC_BF16X3: {"7x7": 1.6e-7, "3x3": 5e-7, "1x1": 5e-7, "im2col": 2e-7},
     engine.PREC_FP32_SIMT: {"7x7": 1e-6, "3x3": 8e-7, "1x1": 7e-7, "im2col": 5e-7},
 }
-
-
-def layers_for(cfg):
-    model = CONFIGS[cfg][0]
-    layers = checked_layers(model)
-    return [l for l in layers if l["name"] == "conv1_1"] if CONFIGS[cfg][5].get("PE_CONV11_DIRECT") else layers
 
 
 def frames_for(n, disp_w, disp_h):
@@ -331,23 +323,21 @@ class Blobs:
         return self.cache[name]
 
 
-def bound(prec, layer, cin, direct):
+def bound(prec, layer, cin):
     K = layer["k"] ** 2 * cin
-    if direct:
-        return 28 * U / (1 - 28 * U) + 4 * U
     if prec == engine.PREC_FP32_SIMT:
         return (K + 1) * U / (1 - (K + 1) * U)
     return B_P1 if prec == engine.PREC_BF16X1 else B_P2
 
 
-def check_layer(layer, blobs, W, prec, pts, calibrated, direct):
+def check_layer(layer, blobs, W, prec, pts, calibrated):
     w, b = W[layer["name"]]
     x = blobs.get(layer["bottom"])
     y = blobs.get(layer["top"])
     ref, mag = conv_ref(x, w, b, pts, layer["relu"])
     got = y[pts[:, 0], :, pts[:, 1], pts[:, 2]].astype(np.float64)
     err = np.abs(got - ref)
-    B = bound(prec, layer, w.shape[1], direct)
+    B = bound(prec, layer, w.shape[1])
     floor = 0.0
     if prec == engine.PREC_F16X2:
         floor = U * (float(np.abs(y).max()) / 32 if calibrated else 1.0)
@@ -364,10 +354,8 @@ def layer_class(layer):
     return "im2col" if layer["name"] == "conv1_1" else "%dx%d" % (layer["k"], layer["k"])
 
 
-def run_config(cfg, monkeypatch):
-    model, net_w, net_h, prec, counts, env, cal = CONFIGS[cfg]
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
+def run_config(cfg):
+    model, net_w, net_h, prec, counts, cal = CONFIGS[cfg]
     W = weights_with_biases(model, *(cal or ("he", 1.0)))
     disp_w, disp_h = 2 * net_w, 2 * net_h
     eng = engine.PoseEngine(model, net_w, net_h, disp_w, disp_h, precision=prec, max_batch=max(counts))
@@ -381,13 +369,11 @@ def run_config(cfg, monkeypatch):
             eng.calibrate(frames)
         eng.forward_frames(frames)
         blobs = Blobs(eng, n, model, W)
-        for layer in layers_for(cfg):
+        for layer in checked_layers(model):
             w_, h_, gap = level_geo(net_w, net_h, layer["level"])
             pts = sample_pixels(n, h_, w_, gap, rng)
-            r = check_layer(layer, blobs, W, prec, pts, cal is not None, bool(env.get("PE_CONV11_DIRECT")))
-            if env.get("PE_CONV11_DIRECT"):
-                width = "direct"
-            elif prec == engine.PREC_FP32_SIMT:
+            r = check_layer(layer, blobs, W, prec, pts, cal is not None)
+            if prec == engine.PREC_FP32_SIMT:
                 width = "simt"
             else:
                 ks = 1 if layer["name"] == "conv1_1" else layer["k"]
@@ -400,15 +386,15 @@ def run_config(cfg, monkeypatch):
         print("  %-7s %-7s %.3e" % (key[0], key[1], worst[key]))
     if prec in MEASURED_MAX:
         lim = MEASURED_MAX[prec]
-        over = {k: v for k, v in worst.items() if v > lim["direct" if k[1] == "direct" else k[0]]}
+        over = {k: v for k, v in worst.items() if v > lim[k[0]]}
         assert not over, "accumulation error above what this kernel measured: %s" % over
     return worst
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("cfg", list(CONFIGS))
-def test_conv_layers_vs_float64(cfg, monkeypatch):
-    run_config(cfg, monkeypatch)
+def test_conv_layers_vs_float64(cfg):
+    run_config(cfg)
 
 
 @pytest.mark.gpu
@@ -417,12 +403,12 @@ def test_width_rule_covers_every_instance():
     has, each filter size at full and half width, and a partial last row tile at every level."""
     nsm = torch.cuda.get_device_properties(0).multi_processor_count
     seen, partial = set(), set()
-    for cfg, (model, net_w, net_h, prec, counts, env, _) in CONFIGS.items():
-        if prec == engine.PREC_FP32_SIMT or env.get("PE_CONV11_DIRECT"):
+    for model, net_w, net_h, prec, counts, _ in CONFIGS.values():
+        if prec == engine.PREC_FP32_SIMT:
             continue
         W = synth.make_weights(model)
         for n in counts:
-            for layer in layers_for(cfg):
+            for layer in checked_layers(model):
                 w_, h_, gap = level_geo(net_w, net_h, layer["level"])
                 M = n * (h_ + gap) * (w_ + gap)
                 ks = 1 if layer["name"] == "conv1_1" else layer["k"]
@@ -505,5 +491,5 @@ def test_fetch_blob_refuses_overwritten_stage_outputs():
     layer = [l for l in checked_layers(model) if l["name"] == "Mconv7_stage5_L1"][0]
     blobs = Blobs(eng, 1, model, W)
     w_, h_, gap = level_geo(net_w, net_h, 3)
-    check_layer(layer, blobs, W, engine.PREC_F16X2, sample_pixels(1, h_, w_, gap, np.random.default_rng(3)), False, False)
+    check_layer(layer, blobs, W, engine.PREC_F16X2, sample_pixels(1, h_, w_, gap, np.random.default_rng(3)), False)
     eng.close()

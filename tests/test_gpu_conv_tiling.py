@@ -84,7 +84,7 @@ def test_batched_frames_match_frames_alone_and_float64(model):
         for layer in layers:
             w_, h_, gap = level_geo(NET_W, NET_H, layer["level"])
             pts = np.unique(np.concatenate([sample_pixels(n, h_, w_, gap, rng, 200), image_tile_pixels(n, h_, w_, gap)]), axis=0)
-            r = check_layer(layer, blobs, W, prec, pts, False, False)
+            r = check_layer(layer, blobs, W, prec, pts, False)
             key = layer_class(layer)
             worst[key] = max(worst.get(key, 0.0), r)
             ks = 1 if layer["name"] == "conv1_1" else layer["k"]
