@@ -1,0 +1,30 @@
+// The e4m3 instances of the wgmma / TMA convolution (PE_PREC_E4M3X1), in a translation unit of their own so that conv_tc.cu
+// keeps exactly its 16-bit instances.  The kernel is conv_wg_kernel (conv_tc_kernel.cuh) at ELEM = e4m3: 128-channel K blocks
+// in the same 128-byte swizzle rows, wgmma m64nBNk32 e4m3 x e4m3 -> fp32 with the fp16 fast mode's chunked round-to-nearest
+// accumulation, and an epilogue that rounds to e4m3 with cvt.rn.satfinite.  conv1_1 keeps its fp16 im2col input: its instance
+// reads fp16 and writes e4m3.
+#include "conv_tc_kernel.cuh"
+
+namespace pe {
+
+template <int BN>
+static int launch_e4m3_bn(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap) {
+    const PlaneFmt f = l.d.fmt;
+    if (f.planes != 1) return -1;
+    if (f.e4m3()) return launch_inst<BN, 1, ELEM_E4M3, ELEM_E4M3>(l, a, grid, st, bmap);
+    if (f.f16() && l.d.out_e4m3) return launch_inst<BN, 1, ELEM_F16, ELEM_E4M3>(l, a, grid, st, bmap);
+    return -1;
+}
+
+int launch_e4m3(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap, int bn) {
+    switch (bn) {
+        case 128: return launch_e4m3_bn<128>(l, a, grid, st, bmap);
+        case 64: return launch_e4m3_bn<64>(l, a, grid, st, bmap);
+        case 48: return launch_e4m3_bn<48>(l, a, grid, st, bmap);
+        case 32: return launch_e4m3_bn<32>(l, a, grid, st, bmap);
+        case 16: return launch_e4m3_bn<16>(l, a, grid, st, bmap);
+        default: return -1;
+    }
+}
+
+}  // namespace pe

@@ -8,15 +8,16 @@
 namespace pe {
 
 struct TcLayerDesc {
-    const void* in; int in_pitch, in_cused; long long in_plane;   // 16-bit planes [P][M][pitch]
-    const void* w;                                                // 16-bit planes [P][cout_pad][K]
+    const void* in; int in_pitch, in_cused; long long in_plane;   // planes [P][M][pitch] of fmt's element kind
+    const void* w;                                                // planes [P][cout_pad][K] of fmt's element kind
     const float* bias;
     int cout, cout_pad, ksize, pad, relu;
-    PlaneFmt fmt;                                                 // plane count and fp16 / bf16 (kernels.h)
+    PlaneFmt fmt;                                                 // plane count and element kind of in and w (kernels.h)
+    bool out_e4m3 = false;                                        // out holds e4m3 (with fmt fp16: conv1_1 of PE_PREC_E4M3X1)
     const float* out_scale = nullptr;                             // device: epilogue factor 2^-k (weights packed with 2^k)
     unsigned* range = nullptr;                                    // device: running max |stored value| (float bits), or null
     Geo geo;                                                      // geo.N = max images
-    void* out; int out_pitch, out_coff; long long out_plane;      // 16-bit planes, or
+    void* out; int out_pitch, out_coff; long long out_plane;      // planes (e4m3 when fmt or out_e4m3 says so), or
     float* planar; int planar_C, planar_coff;                     // final fp32 maps (N, planar_C, H, W)
 };
 struct TcLayer {

@@ -16,6 +16,7 @@
 #include "common.h"
 #include "kernels.h"
 #include "conv_tc.h"
+#include "e4m3.h"
 #include "jpeg_coefs.h"
 #include "jpeg_entropy.cuh"
 #include "pixels.cuh"
@@ -39,8 +40,7 @@ struct pe_engine {
     const ModelTables* mt = nullptr;
     ModelTables mt_own;     // model tables with the prototxt's nms max_peaks
     Geo geo[4];
-    PlaneFmt fmt = {0, false};   // storage of activations and packed weights (kernels.h): 0 planes = fp32 SIMT
-    int elem = 4;
+    PlaneFmt fmt = {0, ELEM_BF16};   // storage of activations and packed weights (kernels.h): 0 planes = fp32 SIMT
     std::vector<void*> acts;        // device
     std::vector<long long> act_plane;  // elements per plane
     std::vector<HostWeights> hw;    // per conv
@@ -48,7 +48,7 @@ struct pe_engine {
     // packed weights (one device buffer): per conv offsets (bytes)
     void* d_packed = nullptr; size_t packed_bytes = 0;
     std::shared_ptr<void> packed_owner;   // frees d_packed when the last handle using it goes (pe_share_weights)
-    // fp16-plane range management (F16X2, F16X1): per-conv-output power-of-two scale s (stored value = true value * s), the true
+    // range management of the fp16 and e4m3 modes (F16X2, F16X1, E4M3X1): per-conv-output power-of-two scale s (stored value = true value * s), the true
     // biases / weight-scale inverses the packed epilogue fields derive from, and the kernels' running max |stored value| per conv
     std::vector<float> conv_scale, wsi;   // per conv: scale of its stored output; inverse of the power of two folded into its weights
     std::vector<std::vector<float>> bias_true;
@@ -111,6 +111,18 @@ struct pe_engine {
 
 static void drop_graphs(pe_engine* e);
 static int setup_lanes(pe_engine* e);
+
+// Storage of activation i and of conv i's packed weights: the engine's format, except that E4M3X1 keeps the im2col'ed net input,
+// and so conv1_1's weights, in one fp16 plane (kernels.h)
+static PlaneFmt act_fmt(const pe_engine* e, int i) {
+    return e->fmt.e4m3() && i == e->plan.input_act ? PlaneFmt{1, ELEM_F16} : e->fmt;
+}
+static PlaneFmt conv_wfmt(const pe_engine* e, int i) { return act_fmt(e, e->plan.convs[i].in_act); }
+// channel granularity of the activations (common.h): 16 (fp32 SIMT), 64 (16-bit planes), 128 (e4m3: one K block, conv_tc_kernel.cuh)
+static int act_cpad(int precision) { return precision == PE_PREC_FP32_SIMT ? 16 : precision == PE_PREC_E4M3X1 ? 128 : 64; }
+// Concat slot granularity (common.h, build_plan_from_net): 16 bytes of e4m3, 8 channels otherwise
+static int slot_align(int precision) { return precision == PE_PREC_E4M3X1 ? 16 : 8; }
+static size_t fmt_bytes(PlaneFmt f) { return (size_t)f.elem_bytes() * (f.planes ? f.planes : 1); }   // bytes per element, all planes
 
 static int fail(pe_engine* e, int code, const char* fmt, ...) {
     char buf[1024];
@@ -300,7 +312,7 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
     if (prototxt_path) {
         std::string perr;
         if (parse_prototxt_file(prototxt_path, netdef, perr)) return fail(nullptr, PE_ERR_IO, "%s: %s", prototxt_path, perr.c_str());
-        if (build_plan_from_net(netdef, cfg->precision ? 64 : 32, cfg->precision ? 64 : 16, proto_plan, perr))
+        if (build_plan_from_net(netdef, cfg->precision ? 64 : 32, act_cpad(cfg->precision), proto_plan, perr, slot_align(cfg->precision)))
             return fail(nullptr, PE_ERR_INVALID, "%s: %s", prototxt_path, perr.c_str());
         if (cfg->model >= 0 && cfg->model != proto_plan.model)
             return fail(nullptr, PE_ERR_INVALID, "%s describes the %s model (nms num_parts %d), the configuration asks for model %d", prototxt_path,
@@ -314,7 +326,7 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
     if (cfg->max_batch < 1 || cfg->max_batch > 64) return fail(nullptr, PE_ERR_INVALID, "max_batch %d out of [1,64]", cfg->max_batch);
     if (check_resize_scales(nullptr, (float)cfg->start_scale, (float)cfg->scale_gap, cfg->num_scales)) return PE_ERR_INVALID;
     if (cfg->disp_w <= 0 || cfg->disp_h <= 0) return fail(nullptr, PE_ERR_INVALID, "bad display resolution");
-    if (cfg->precision < 0 || cfg->precision > 4) return fail(nullptr, PE_ERR_INVALID, "unknown precision %d", cfg->precision);
+    if (cfg->precision < 0 || cfg->precision > PE_PREC_E4M3X1) return fail(nullptr, PE_ERR_INVALID, "unknown precision %d", cfg->precision);
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
         return fail(nullptr, PE_ERR_CUDA, "no CUDA device visible: the pose engine has no CPU fallback");
@@ -329,7 +341,6 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
     e->mt = &e->mt_own;
     e->fmt = plane_fmt(cfg->precision);
     if (const char* g = getenv("PE_CHECK_RANGE")) e->check_range = atoi(g) != 0;
-    e->elem = e->fmt.planes == 0 ? 4 : 2;
     e->start_scale_f = (float)cfg->start_scale;  // ImResizeLayer::SetStartScale(float)
     e->scale_gap_f = (float)cfg->scale_gap;
     auto bail = [&](int rc) { g_create_error = e->err; pe_destroy(e); return rc; };
@@ -345,7 +356,7 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
     for (int i = 0; i < 16; i++) CKC(cudaEventCreate(&e->ev[i]));
 
     // the plan first: each level's gap is the largest pad of its convolutions (common.h)
-    e->plan = prototxt_path ? proto_plan : build_plan(cfg->model, e->fmt.planes ? 64 : 32, e->fmt.planes ? 64 : 16);
+    e->plan = prototxt_path ? proto_plan : build_plan(cfg->model, e->fmt.planes ? 64 : 32, act_cpad(cfg->precision), slot_align(cfg->precision));
     const int N = cfg->max_batch * cfg->num_scales;
     int w = cfg->net_w, h = cfg->net_h;
     for (int l = 0; l < 4; l++) {
@@ -369,7 +380,7 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
         const ActSpec& a = e->plan.acts[i];
         const Geo& g = e->geo[a.level];
         e->act_plane[i] = g.M * a.C;
-        const size_t bytes = (size_t)e->act_plane[i] * e->elem * (e->fmt.planes ? e->fmt.planes : 1);
+        const size_t bytes = (size_t)e->act_plane[i] * fmt_bytes(act_fmt(e, (int)i));
         CKC(cudaMalloc(&e->acts[i], bytes));
         CKC(cudaMemsetAsync(e->acts[i], 0, bytes, e->stream));
     }
@@ -388,7 +399,7 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
     if (build_pre_tables(e)) return bail(PE_ERR_INVALID);
     e->pre.frames = e->d_frames; e->pre.resized = e->d_resized;
     e->pre.out = e->acts[e->plan.input_act]; e->pre.kp = e->plan.kp_input;
-    e->pre.out_plane = e->act_plane[e->plan.input_act]; e->pre.fmt = e->fmt;
+    e->pre.out_plane = e->act_plane[e->plan.input_act]; e->pre.fmt = act_fmt(e, e->plan.input_act);
     e->pre.Wp = e->geo[0].Wp; e->pre.Hs = e->geo[0].Hs;
 
     // post-processing state
@@ -554,7 +565,7 @@ static size_t packed_layout(pe_engine* e) {
         e->cout_pad[i] = e->fmt.planes ? tc_cout_pad(c.cout) : (c.cout + 63) / 64 * 64;
         const size_t K = (size_t)(c.im2col_input ? 1 : c.k * c.k) * e->cin_pad[i];
         e->w_off[i] = total;
-        total = align256(total + K * e->cout_pad[i] * e->elem * (e->fmt.planes ? e->fmt.planes : 1));
+        total = align256(total + K * e->cout_pad[i] * fmt_bytes(conv_wfmt(e, (int)i)));
         e->b_off[i] = total;
         total = align256(total + (size_t)(e->cout_pad[i] + 1) * 4);   // bias[cout_pad] + the layer's epilogue scale
     }
@@ -601,9 +612,10 @@ static void pack_conv_weights(pe_engine* e, int i, uint8_t* dst) {
         if (ci < 0) return 0.f;
         return hw.w[((size_t)co * c.cin + ci) * c.k * c.k + tap] * chan[ec];
     };
-    memset(dst, 0, K * cop * e->elem * (e->fmt.planes ? e->fmt.planes : 1));
+    const PlaneFmt wf = conv_wfmt(e, i);
+    memset(dst, 0, K * cop * fmt_bytes(wf));
     float wscale_inv = 1.f;
-    if (e->fmt.planes == 0) {  // fp32 [K][cout_pad]
+    if (wf.planes == 0) {  // fp32 [K][cout_pad]
         float* W = (float*)dst;
         for (size_t kk = 0; kk < K; kk++)
             for (int co = 0; co < c.cout; co++) W[kk * cop + co] = src(co, (int)kk);
@@ -611,23 +623,30 @@ static void pack_conv_weights(pe_engine* e, int i, uint8_t* dst) {
         uint16_t* W = (uint16_t*)dst;
         const size_t plane = (size_t)cop * K;
         // fp16 planes: scale the layer by 2^k so that max|w| lands in [2^13, 2^14) - small weights would otherwise
-        // put their lo plane into fp16 subnormals.  Exact (power of two); the epilogue multiplies by 2^-k.
+        // put their lo plane into fp16 subnormals.  e4m3: into [128, 256), below the largest finite 448, so that
+        // weights down to max|w| * 2^-13 stay normal.  Exact (power of two); the epilogue multiplies by 2^-k.
         float wscale = 1.f;
-        if (e->fmt.f16) {
+        if (wf.f16() || wf.e4m3()) {
             float mx = 0.f;
             for (int co = 0; co < c.cout; co++)
                 for (size_t kk = 0; kk < K; kk++) mx = fmaxf(mx, fabsf(src(co, (int)kk)));
             int ex = 0;
-            if (mx > 0.f && mx < 3e38f) { frexpf(mx, &ex); wscale = ldexpf(1.f, std::max(-100, std::min(100, 14 - ex))); }
+            const int top = wf.e4m3() ? 8 : 14;
+            if (mx > 0.f && mx < 3e38f) { frexpf(mx, &ex); wscale = ldexpf(1.f, std::max(-100, std::min(100, top - ex))); }
         }
         wscale_inv = 1.f / wscale;
-        for (int co = 0; co < c.cout; co++)
-            for (size_t kk = 0; kk < K; kk++) {
-                uint16_t h[3];
-                if (e->fmt.f16) split_fp16(src(co, (int)kk) * wscale, e->fmt.planes, h);
-                else split_bf16(src(co, (int)kk), e->fmt.planes, h);
-                for (int p = 0; p < e->fmt.planes; p++) W[p * plane + (size_t)co * K + kk] = h[p];
-            }
+        if (wf.e4m3()) {   // one byte per weight, [cout_pad][K]
+            for (int co = 0; co < c.cout; co++)
+                for (size_t kk = 0; kk < K; kk++) dst[(size_t)co * K + kk] = float_to_e4m3(src(co, (int)kk) * wscale);
+        } else {
+            for (int co = 0; co < c.cout; co++)
+                for (size_t kk = 0; kk < K; kk++) {
+                    uint16_t h[3];
+                    if (wf.f16()) split_fp16(src(co, (int)kk) * wscale, wf.planes, h);
+                    else split_bf16(src(co, (int)kk), wf.planes, h);
+                    for (int p = 0; p < wf.planes; p++) W[p * plane + (size_t)co * K + kk] = h[p];
+                }
+        }
     }
     e->wsi[i] = wscale_inv;
 }
@@ -635,7 +654,7 @@ static void pack_conv_weights(pe_engine* e, int i, uint8_t* dst) {
 // per-layer launch state (TMA descriptors) over the packed buffer the handle currently points at
 static int bind_packed(pe_engine* e) {
     const size_t nc = e->plan.convs.size();
-    if (e->fmt.f16 && !e->d_range) {
+    if (e->fmt.ranged() && !e->d_range) {
         CK(e, cudaMalloc(&e->d_range, nc * sizeof(unsigned)));
         CK(e, cudaMemset(e->d_range, 0, nc * sizeof(unsigned)));
     }
@@ -649,8 +668,9 @@ static int bind_packed(pe_engine* e) {
             d.in = e->acts[c.in_act]; d.in_pitch = e->plan.acts[c.in_act].C; d.in_cused = c.in_cused; d.in_plane = e->act_plane[c.in_act];
             d.w = (char*)e->d_packed + e->w_off[i]; d.bias = (const float*)((char*)e->d_packed + e->b_off[i]);
             d.cout = c.cout; d.cout_pad = e->cout_pad[i]; d.ksize = c.im2col_input ? 1 : c.k; d.pad = c.im2col_input ? 0 : c.pad;
-            d.relu = c.relu; d.fmt = e->fmt; d.geo = g; d.out_scale = d.bias + e->cout_pad[i];
-            d.range = (e->fmt.f16 && e->d_range) ? e->d_range + i : nullptr;
+            d.relu = c.relu; d.fmt = conv_wfmt(e, (int)i); d.geo = g; d.out_scale = d.bias + e->cout_pad[i];
+            d.out_e4m3 = e->fmt.e4m3();
+            d.range = (e->fmt.ranged() && e->d_range) ? e->d_range + i : nullptr;
             if (c.out_act >= 0) {
                 d.out = e->acts[c.out_act]; d.out_pitch = e->plan.acts[c.out_act].C; d.out_coff = c.out_coff; d.out_plane = e->act_plane[c.out_act];
                 d.planar = nullptr; d.planar_C = 0; d.planar_coff = 0;
@@ -877,7 +897,7 @@ static int run_op(pe_engine* e, const OpRef& op, int nimg, cudaStream_t st = nul
         const Geo& g = e->geo[3];
         CopyArgs a;
         a.src = e->acts[c.src_act]; a.dst = e->acts[c.dst_act]; a.pitch = e->plan.acts[c.src_act].C; a.channels = c.channels;
-        a.elem_bytes = e->elem; a.M = (long long)nimg * g.Hs * g.Wp; a.plane = e->act_plane[c.src_act]; a.fmt = e->fmt;
+        a.elem_bytes = e->fmt.elem_bytes(); a.M = (long long)nimg * g.Hs * g.Wp; a.plane = e->act_plane[c.src_act]; a.fmt = e->fmt;
         e->launches += launch_copy_channels(a, st);
     }
     return PE_OK;
@@ -1009,7 +1029,7 @@ extern "C" int pe_forward_frames_device(pe_engine* e, const void* d_frames, int 
     PreArgs a = e->pre;
     a.frames = (const uint8_t*)d_frames; a.nframes = n;
     if (e->input_lo_dirty) {   // the uint8 path only writes the hi plane; drop what the planar path left behind
-        const size_t bytes = (size_t)e->act_plane[e->plan.input_act] * e->elem * (e->fmt.planes ? e->fmt.planes : 1);
+        const size_t bytes = (size_t)e->act_plane[e->plan.input_act] * fmt_bytes(act_fmt(e, e->plan.input_act));
         CK(e, cudaMemsetAsync(e->acts[e->plan.input_act], 0, bytes, e->stream));
         e->input_lo_dirty = false;
     }
@@ -1387,7 +1407,7 @@ static int upload_fields(pe_engine* e, int i) {
 static int upload_weights(pe_engine* e, int i) {   // re-pack layer i with the current input scales (host fp32 copy needed)
     const ConvSpec& c = e->plan.convs[i];
     const size_t K = (size_t)(c.im2col_input ? 1 : c.k * c.k) * e->cin_pad[i];
-    std::vector<uint8_t> buf(K * e->cout_pad[i] * e->elem * (e->fmt.planes ? e->fmt.planes : 1));
+    std::vector<uint8_t> buf(K * e->cout_pad[i] * fmt_bytes(conv_wfmt(e, i)));
     pack_conv_weights(e, i, buf.data());
     CK(e, cudaMemcpyAsync((char*)e->d_packed + e->w_off[i], buf.data(), buf.size(), cudaMemcpyHostToDevice, e->stream));
     CK(e, cudaStreamSynchronize(e->stream));
@@ -1398,7 +1418,7 @@ extern "C" int pe_calibrate(pe_engine* e, const uint8_t* const* frames, int n) {
     int rc = check_n(e, n); if (rc) return rc;
     if (!frames) return fail(e, PE_ERR_INVALID, "null frames");
     if (!e->committed) return fail(e, PE_ERR_STATE, "pe_commit_weights has not been called");
-    if (!e->fmt.f16) return PE_OK;   // fp32 / bf16 modes have fp32's exponent range
+    if (!e->fmt.ranged()) return PE_OK;   // fp32 / bf16 modes have fp32's exponent range
     const size_t nc = e->plan.convs.size();
     if (e->bias_true.size() != nc || e->bias_true[0].empty() || e->hw[0].w.empty())
         return fail(e, PE_ERR_STATE, "this handle received its weights by broadcast / sharing: calibrate the source handle before replicating");
@@ -1432,7 +1452,10 @@ extern "C" int pe_calibrate(pe_engine* e, const uint8_t* const* frames, int n) {
             CK(e, cudaMemcpyAsync(&bits, e->d_range + i, sizeof bits, cudaMemcpyDeviceToHost, e->stream));
             CK(e, cudaStreamSynchronize(e->stream));
             float m; memcpy(&m, &bits, 4);
-            if (m > 0.f && m < 3e38f) { int ex = 0; frexpf(m, &ex); e->conv_scale[i] = ldexpf(1.f, std::max(-100, std::min(100, 6 - ex))); }   // m * s in [32, 64)
+            // m * s in [32, 64) for fp16 (1000x headroom to 65504); in [64, 128) for e4m3 (3.5-7x headroom to 448, and values
+            // down to m * s * 2^-12 stay normal)
+            const int top = e->fmt.e4m3() ? 7 : 6;
+            if (m > 0.f && m < 3e38f) { int ex = 0; frexpf(m, &ex); e->conv_scale[i] = ldexpf(1.f, std::max(-100, std::min(100, top - ex))); }
         }
         if ((rc = upload_fields(e, i))) return rc;
         if ((rc = run_op(e, op, nimg))) return rc;
@@ -1442,8 +1465,10 @@ extern "C" int pe_calibrate(pe_engine* e, const uint8_t* const* frames, int n) {
     return run_post_and_return(e, n);
 }
 
-// Largest |stored value| / 65504 over the conv layers since the last call (PE_ERR_RANGE when a layer reached the fp16 limit, or when
-// a layer's maximum fell below 2^-10 - its lo plane then lives in fp16 subnormals and parity is lost); *layer64 names the worst one.
+// Largest |stored value| / the format's largest finite value (65504 for fp16, 448 for e4m3) over the conv layers since the last
+// call.  PE_ERR_RANGE when a layer reached that limit, or when a layer's maximum fell below a floor: fp16 2^-10 (its lo plane then
+// lives in fp16 subnormals and parity is lost); e4m3 2^-2, 16x above the smallest normal 2^-6, so that values a sixteenth of
+// the maximum - the bulk of a layer's outputs - are still normal.  *layer64 names the worst layer.
 extern "C" int pe_range_status(pe_engine* e, float* worst_ratio, char* layer64) {
     if (!e) return PE_ERR_INVALID;
     if (worst_ratio) *worst_ratio = 0.f;
@@ -1455,25 +1480,28 @@ extern "C" int pe_range_status(pe_engine* e, float* worst_ratio, char* layer64) 
     std::vector<unsigned> bits(nc);
     CK(e, cudaMemcpy(bits.data(), e->d_range, nc * sizeof(unsigned), cudaMemcpyDeviceToHost));
     CK(e, cudaMemset(e->d_range, 0, nc * sizeof(unsigned)));
+    const bool e4 = e->fmt.e4m3();
+    const float limit = e4 ? 448.f : 65504.f, floor_ = e4 ? 0.25f : 9.765625e-4f;
+    const char* what = e4 ? "the e4m3 planes" : "the fp16 planes";
     float worst = 0.f, smallest = 3e38f;
     int iw = -1, is = -1;
     for (size_t i = 0; i < nc; i++) {
         if (e->plan.convs[i].out_act < 0) continue;   // fp32 maps
         float m; memcpy(&m, &bits[i], 4);
         if (bits[i] == 0) continue;                   // layer did not run since the last call
-        if (!(m <= 3e38f) || m / 65504.f > worst) { worst = (m <= 3e38f) ? m / 65504.f : 2.f; iw = (int)i; }
+        if (!(m <= 3e38f) || m / limit > worst) { worst = (m <= 3e38f) ? m / limit : 2.f; iw = (int)i; }
         if (m < smallest) { smallest = m; is = (int)i; }
     }
     if (worst_ratio) *worst_ratio = worst;
     if (worst >= 1.f) {
         if (layer64) snprintf(layer64, 64, "%s", e->plan.convs[iw].name.c_str());
-        return fail(e, PE_ERR_RANGE, "layer %s produced values outside the range of the fp16 planes (max |v| = %.3g x scale): run pe_calibrate",
-                    e->plan.convs[iw].name.c_str(), worst * 65504.f);
+        return fail(e, PE_ERR_RANGE, "layer %s produced values outside the range of %s (max |v| = %.3g x scale): run pe_calibrate",
+                    e->plan.convs[iw].name.c_str(), what, worst * limit);
     }
-    if (is >= 0 && smallest < 9.765625e-4f) {
+    if (is >= 0 && smallest < floor_) {
         if (layer64) snprintf(layer64, 64, "%s", e->plan.convs[is].name.c_str());
-        return fail(e, PE_ERR_RANGE, "layer %s: largest stored value %.3g is below 2^-10, the fp16 planes lose precision: run pe_calibrate",
-                    e->plan.convs[is].name.c_str(), smallest);
+        return fail(e, PE_ERR_RANGE, "layer %s: largest stored value %.3g is below %s, %s lose precision: run pe_calibrate",
+                    e->plan.convs[is].name.c_str(), smallest, e4 ? "2^-2" : "2^-10", what);
     }
     if (layer64 && iw >= 0) snprintf(layer64, 64, "%s", e->plan.convs[iw].name.c_str());
     return PE_OK;
@@ -1655,7 +1683,7 @@ extern "C" int pe_fetch_blob(pe_engine* e, const char* blob_name, float* out, si
         CK(e, cudaMalloc(&d, cnt * sizeof(float)));
         // stored value = true value * conv_scale[producer] (pools pass their producer's scale through; the net input has none)
         const float inv = (b.prod >= 0 && b.prod < (int)e->conv_scale.size()) ? 1.f / e->conv_scale[b.prod] : 1.f;
-        e->launches += launch_act_to_nchw(e->acts[b.act], e->plan.acts[b.act].C, b.coff, b.c, e->act_plane[b.act], e->fmt, g, inv, d,
+        e->launches += launch_act_to_nchw(e->acts[b.act], e->plan.acts[b.act].C, b.coff, b.c, e->act_plane[b.act], act_fmt(e, b.act), g, inv, d,
                                           e->stream);
         CK(e, cudaMemcpyAsync(out, d, cnt * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
         CK(e, cudaStreamSynchronize(e->stream));

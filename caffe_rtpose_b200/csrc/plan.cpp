@@ -65,7 +65,7 @@ static const int kMaxChannels = 16384;   // a user's prototxt is untrusted input
 // "same"-padded convolutions, in-place ReLU, 2x2/2 MAX pooling, channel Concat, ImResize(factor 8), Nms, any number
 // of stages.  Anything else is reported as an error (the reference would run it through generic Caffe layers).
 // ---------------------------------------------------------------------------------------------
-int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, std::string& err) {
+int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, std::string& err, int slot_align) {
     p = NetPlan();
     const int NL = (int)net.layers.size();
     auto fail = [&](const std::string& m) { err = m; return -1; };
@@ -176,7 +176,7 @@ int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, s
         int eoff = 0;
         for (int pass = 0; pass < 2; pass++)        // shared blobs first
             for (Slot& sdef : sl)
-                if (sdef.shared == (pass == 0)) { sdef.eng_off = eoff; eoff += round_up(sdef.c, 8); }
+                if (sdef.shared == (pass == 0)) { sdef.eng_off = eoff; eoff += round_up(sdef.c, slot_align); }
         const int total = round_up(eoff, cpad);
         if (j == 0) cc_c = total;
         else {   // the physical buffers are reused: every concat must have the layout of the first
@@ -260,7 +260,7 @@ int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, s
                 p.blobs.push_back({top, c.out_act, sdef.eng_off, sdef.c, (int)p.convs.size(), (int)p.order.size()});
                 if (sdef.shared || consumers[top].size() > 1) {   // also read directly by convolutions (conv4_4_CPM feeds stage 1)
                     if (sdef.eng_off != 0) return fail("blob " + top + ": a directly consumed Concat bottom must be first in the buffer");
-                    Loc o; o.act = c.out_act; o.coff = 0; o.cused = round_up(sdef.c, 64); o.cmap = ident(sdef.c, o.cused);
+                    Loc o; o.act = c.out_act; o.coff = 0; o.cused = round_up(sdef.c, std::max(64, cpad)); o.cmap = ident(sdef.c, o.cused);
                     o.prod.assign(o.cused, -1);
                     for (int q = 0; q < sdef.c; q++) o.prod[q] = (int)p.convs.size();
                     if (o.cused > cc_c) return fail("blob " + top + ": too narrow concat buffer");
@@ -278,7 +278,7 @@ int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, s
             p.convs.push_back(c);
             p.order.push_back({0, (int)p.convs.size() - 1});
             if (concat_slot.count(top) && slots[concat_slot[top].first][concat_slot[top].second].shared && nbuf == 2) {
-                p.copies.push_back({cc[0], cc[1], round_up(channels[top], 8)});
+                p.copies.push_back({cc[0], cc[1], round_up(channels[top], slot_align)});   // whole 16-byte chunks, inside the slot
                 p.order.push_back({2, (int)p.copies.size() - 1});
             }
         } else if (l.type == "Pooling") {
@@ -329,10 +329,14 @@ int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, s
     return 0;
 }
 
-NetPlan build_plan(int model, int kp_input, int cpad) {
+int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, std::string& err) {
+    return build_plan_from_net(net, kp_input, cpad, p, err, 8);
+}
+
+NetPlan build_plan(int model, int kp_input, int cpad, int slot_align) {
     NetPlan p;
     std::string err;
-    if (build_plan_from_net(builtin_netdef(model, 6), kp_input, cpad, p, err)) fprintf(stderr, "poseengine: built-in plan: %s\n", err.c_str());
+    if (build_plan_from_net(builtin_netdef(model, 6), kp_input, cpad, p, err, slot_align)) fprintf(stderr, "poseengine: built-in plan: %s\n", err.c_str());
     return p;
 }
 

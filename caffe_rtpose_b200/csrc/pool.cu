@@ -1,9 +1,9 @@
 // 2x2 stride-2 MAX pooling (ceil dims), channel-slice copy and layout conversion on the flat padded layout.
 //
 // Pooling semantics: src/caffe/layers/pooling_layer.cpp:90-93 (ceil), :128-187 (max over the window clipped
-// to the image).  Activations are either fp32 [M][C] or 16-bit "planes" whose SUM is the value (split
-// precision for the wgmma conv, see conv_tc.cu); the max is taken on the reconstructed value and the
-// winner's planes are copied, which keeps the split exact.
+// to the image).  Activations are either fp32 [M][C], 16-bit "planes" whose SUM is the value (split
+// precision for the wgmma conv, see conv_tc.cu), or one e4m3 plane; the max is taken on the reconstructed
+// value and the winner's planes are copied, which keeps the split exact.
 #include "common.h"
 #include "kernels.h"
 
@@ -84,16 +84,57 @@ __global__ void __launch_bounds__(256) pool_planes_kernel(PoolArgs a) {
         *((uint4*)((__nv_bfloat16*)a.out + (size_t)p * a.out_plane + mo * a.C) + g) = o[p];
 }
 
+// e4m3 (one byte per channel): 16 channels per thread.  Rounding is monotone, so the max of the stored values is the stored
+// max: the winner's byte is copied.
+__global__ void __launch_bounds__(256) pool_e4m3_kernel(PoolArgs a) {
+    const unsigned cv = a.C / 16;
+    const int n = blockIdx.y;
+    const unsigned per_img = (unsigned)a.Hso * (unsigned)a.Wpo;
+    const unsigned idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= per_img * cv) return;
+    const int g = (int)(idx % cv);
+    const unsigned rem = idx / cv;
+    const int yo = (int)(rem / (unsigned)a.Wpo), xo = (int)(rem % (unsigned)a.Wpo);
+    if (xo >= a.Wo || yo >= a.Ho) return;
+    const long long mo = (long long)n * per_img + rem;
+    uint4 v[4];
+    bool ok[4];
+#pragma unroll
+    for (int w = 0; w < 4; w++) {
+        const int yi = 2 * yo + (w >> 1), xi = 2 * xo + (w & 1);
+        ok[w] = yi < a.Hi && xi < a.Wi;
+        const long long mi = ((long long)n * a.Hsi + (ok[w] ? yi : 2 * yo)) * a.Wpi + (ok[w] ? xi : 2 * xo);
+        v[w] = __ldg((const uint4*)((const uint8_t*)a.in + mi * a.C) + g);
+    }
+    uint4 o;
+#pragma unroll
+    for (int j = 0; j < 16; j++) {
+        uint8_t b = ((const uint8_t*)&v[0])[j];
+        float best = e4m3_to_float(b);
+#pragma unroll
+        for (int w = 1; w < 4; w++) {
+            const uint8_t c = ((const uint8_t*)&v[w])[j];
+            const float f = e4m3_to_float(c);
+            if (ok[w] && f > best) { best = f; b = c; }
+        }
+        ((uint8_t*)&o)[j] = b;
+    }
+    *((uint4*)((uint8_t*)a.out + mo * a.C) + g) = o;
+}
+
 int launch_pool(const PoolArgs& a, cudaStream_t st) {
     const long long rows_out = (long long)a.N * a.Hso * a.Wpo;
     const PlaneFmt f = a.fmt;
     if (f.planes == 0) {
         const long long total = rows_out * (a.C / 4);
         pool_f32_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(a);
+    } else if (f.e4m3()) {
+        const unsigned per = (unsigned)a.Hso * a.Wpo * (a.C / 16);
+        pool_e4m3_kernel<<<dim3((per + 255) / 256, a.N), 256, 0, st>>>(a);
     } else {
         const unsigned per = (unsigned)a.Hso * a.Wpo * (a.C / 8);
         const dim3 grid((per + 255) / 256, a.N);
-        if (f.planes == 1 && f.f16) pool_planes_kernel<1, true><<<grid, 256, 0, st>>>(a);
+        if (f.planes == 1 && f.f16()) pool_planes_kernel<1, true><<<grid, 256, 0, st>>>(a);
         else if (f.planes == 1) pool_planes_kernel<1, false><<<grid, 256, 0, st>>>(a);
         else if (f.planes == 2) pool_planes_kernel<2, true><<<grid, 256, 0, st>>>(a);
         else pool_planes_kernel<3, false><<<grid, 256, 0, st>>>(a);
@@ -101,7 +142,8 @@ int launch_pool(const PoolArgs& a, cudaStream_t st) {
     return 1;
 }
 
-// copy the first `channels` channels of every row (all planes); 16-byte chunks
+// copy the first `channels` channels of every row (all planes); 16-byte chunks: channels x elem_bytes is a multiple of 16
+// (the plan's Concat slot alignment, common.h)
 __global__ void __launch_bounds__(256) copy_channels_kernel(CopyArgs a) {
     const int chunks = a.channels * a.elem_bytes / 16;
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -133,9 +175,10 @@ __global__ void __launch_bounds__(256) act_to_nchw_kernel(const void* act, int p
     const long long m = ((long long)n * g.Hs + y) * g.Wp + x;
     float v = 0.f;
     if (fmt.planes == 0) v = ((const float*)act)[m * pitch + coff + ch];
+    else if (fmt.e4m3()) v = e4m3_to_float(((const uint8_t*)act)[m * pitch + coff + ch]);
     else for (int p = 0; p < fmt.planes; p++) {
         const uint16_t h = ((const uint16_t*)act)[p * plane + m * pitch + coff + ch];
-        v += fmt.f16 ? plane_to_float<true>(h) : plane_to_float<false>(h);
+        v += fmt.f16() ? plane_to_float<true>(h) : plane_to_float<false>(h);
     }
     out[idx] = v * scale;   // a power of two: exact
 }

@@ -175,7 +175,7 @@ __global__ void __launch_bounds__(256) input_im2col_kernel(PreArgs a, const floa
 #pragma unroll
         for (int j = 0; j < 8; j += 2) {
             uint16_t h0, m0, l0, h1, m1, l1;
-            if (a.fmt.f16) { split3<true>(v[j], h0, m0, l0); split3<true>(v[j + 1], h1, m1, l1); }
+            if (a.fmt.f16()) { split3<true>(v[j], h0, m0, l0); split3<true>(v[j + 1], h1, m1, l1); }
             else { split3<false>(v[j], h0, m0, l0); split3<false>(v[j + 1], h1, m1, l1); }
             pk[0][j / 2] = (uint32_t)h0 | ((uint32_t)h1 << 16);
             pk[1][j / 2] = (uint32_t)m0 | ((uint32_t)m1 << 16);
@@ -234,7 +234,7 @@ __global__ void __launch_bounds__(256) input_im2col_u8_kernel(PreArgs a) {
 static int launch_im2col_u8(const PreArgs& a, cudaStream_t st) {
     if (a.fmt.planes > 0 && a.kp >= 32) {
         const dim3 g((a.net_w + 31) / 32, (a.net_h + 7) / 8, a.nframes * a.S), b(32, 8);
-        if (a.fmt.f16) input_im2col_u8_kernel<true><<<g, b, 0, st>>>(a);
+        if (a.fmt.f16()) input_im2col_u8_kernel<true><<<g, b, 0, st>>>(a);
         else input_im2col_u8_kernel<false><<<g, b, 0, st>>>(a);
         return 1;
     }

@@ -21,6 +21,7 @@ MPI_15, COCO_18 = 0, 1
 PREC_FP32_SIMT, PREC_BF16X1, PREC_BF16X2, PREC_BF16X3 = 0, 1, 2, 3
 PREC_F16X2 = PREC_BF16X2   # the parity mode: 2 fp16 planes, chunked round-to-nearest accumulation (poseengine.h)
 PREC_F16X1 = 4             # the fast mode: the parity mode's hi plane alone, one MMA per MAC (poseengine.h)
+PREC_E4M3X1 = 5            # the FP8 mode: one e4m3 plane, one FP8 MMA per MAC; needs calibrate() (poseengine.h)
 MAX_PEOPLE = 96
 # pixel formats of forward_pixels / pixels_to_bgr (PE_PIX_*, poseengine.h)
 PIX_BGR, PIX_RGB, PIX_YUYV, PIX_NV12, PIX_I420 = 0, 1, 2, 3, 4
@@ -462,7 +463,8 @@ class PoseEngine:
         self._ck(lib().pe_calibrate(self._h, arr, len(frames)))
 
     def range_status(self):
-        """(rc, worst |stored value| / 65504, layer name); rc != 0 (PE_ERR_RANGE = 5) when a layer left the fp16 range."""
+        """(rc, worst |stored value| / the format's largest finite value (fp16 65504, e4m3 448), layer name); rc != 0
+        (PE_ERR_RANGE = 5) when a layer left the format's range."""
         worst = C.c_float()
         name = C.create_string_buffer(64)
         rc = lib().pe_range_status(self._h, C.byref(worst), name)

@@ -91,12 +91,13 @@ static void define_flags() {
     define("random_init", "", "[extension] 'he' or 'caffe': random weights instead of --caffemodel (no checkpoint offline)");
     define("model", "", "[extension] COCO or MPI when --caffeproto is not readable");
     define("precision", "2", "[extension] conv arithmetic: 0 fp32 SIMT, 1 bf16 (A/B only), 2 parity mode (two fp16 planes, 3 MMAs per MAC), "
-           "3 three bf16 planes (A/B only), 4 fast mode (one fp16 plane, 1 MMA per MAC; see --audit_every)");
+           "3 three bf16 planes (A/B only), 4 fast mode (one fp16 plane, 1 MMA per MAC; see --audit_every), "
+           "5 FP8 mode (one e4m3 plane, 1 FP8 MMA per MAC; needs --calibrate_range, see --audit_every)");
     define("batch", "0", "[extension] frames per forward per GPU: 1 = the reference's behaviour, 0 = automatic (file / synthetic sources "
            "fill two waves of 128-row tiles on the GPU, e.g. 9 frames at 656x368; results do not depend on it)");
     define("engines_per_gpu", "0", "[extension] worker handles per GPU: 1 = the reference's topology (one Net per GPU), 0 = automatic (2 when "
            "--batch is automatic: the copies and the kernel tails of one batch overlap the other; weights are shared, not duplicated)");
-    define("calibrate_range", "true", "[extension] fp16 modes (--precision 2 and 4): derive per-layer power-of-two activation scales from one synthetic frame at start-up "
+    define("calibrate_range", "true", "[extension] fp16 and e4m3 modes (--precision 2, 4 and 5): derive per-layer power-of-two activation scales from one synthetic frame at start-up "
            "(pe_calibrate), so that a model of any magnitude keeps fp32-level results", true);
     define("audit_every", "0", "[extension] N > 0: every worker also holds a parity-mode (--precision 2) handle and forwards every N-th batch "
            "through it too; each frame's peaks, person count and joints are compared with the fast handle's (within 1e-3 net px). The status "
@@ -711,7 +712,7 @@ static bool create_engines(int num_gpu, int per_gpu, int precision, std::vector<
         engines.push_back(e);
     }
     if (load_weights(engines[0], Fi("start_device"))) return false;
-    if (Fb("calibrate_range") && (precision == PE_PREC_F16X2 || precision == PE_PREC_F16X1)) {   // before the weights are replicated: the scales travel inside the packed buffer
+    if (Fb("calibrate_range") && (precision == PE_PREC_F16X2 || precision == PE_PREC_F16X1 || precision == PE_PREC_E4M3X1)) {   // before the weights are replicated: the scales travel inside the packed buffer
         std::vector<uint8_t> probe;
         synthetic_frame(0, global.disp_w, global.disp_h, probe);
         const uint8_t* ptr = probe.data();

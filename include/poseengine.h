@@ -43,6 +43,13 @@ extern "C" {
                              * roundoff 2^-11): 1.5e-3 - 2.4e-3 of the map range over the whole net against 1.7e-2 for
                              * PE_PREC_BF16X1 at the same cost, 1.9x the parity mode's frames/s (H100 80GB HBM3, 700 W; DESIGN.md
                              * sections 5, 6).  pe_compare_results measures what that does to the poses. */
+#define PE_PREC_E4M3X1 5    /* wgmma FP8 mode: one e4m3 plane (4 significant bits, largest finite 448) of activations and weights,
+                             * 1 FP8 MMA per MAC (wgmma k32 e4m3, twice the fp16 rate), weights scaled per layer by 2^k so that
+                             * max|w| lies in [128, 256), the fp32 accumulation chunked and summed with round-to-nearest as in
+                             * mode 4.  Each layer's output is rounded to e4m3 (unit roundoff 2^-4) with saturation to +-448;
+                             * conv1_1 keeps mode 4's fp16 input.  Needs pe_calibrate: an uncalibrated engine runs at scale 1,
+                             * and pe_range_status reports PE_ERR_RANGE for a layer outside e4m3's range.  DESIGN.md sections
+                             * 3-6; pe_compare_results / --audit_every measure what it does to the poses. */
 
 #define PE_MAX_PEOPLE 96   /* RENDER_MAX_PEOPLE, renderFunctions.h:6 / rtpose.cpp:88 */
 
