@@ -76,6 +76,7 @@ template <int BN>
 static int launch_bn(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap) {
     const PlaneFmt f = l.d.fmt;
     if (f.e4m3() || l.d.out_e4m3) return launch_e4m3(l, a, grid, st, bmap, BN);   // conv_fp8.cu
+    if (f.s8()) return launch_s8(l, a, grid, st, bmap, BN);                        // conv_s8.cu
     if (f.planes == 1) return f.f16() ? launch_inst<BN, 1, ELEM_F16, ELEM_F16>(l, a, grid, st, bmap)
                                       : launch_inst<BN, 1, ELEM_BF16, ELEM_BF16>(l, a, grid, st, bmap);
     if (f.planes == 2 && f.f16()) return launch_inst<BN, 2, ELEM_F16, ELEM_F16>(l, a, grid, st, bmap);
@@ -83,14 +84,15 @@ static int launch_bn(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t 
     return -1;   // no kernel for this tile width and plane format (tc_bn never picks one)
 }
 
-// box {one channel block = 128 bytes, b1, b2}; the 16-bit kinds share one 2-byte data type (TMA only moves the bytes)
+// box {one channel block = 128 bytes, b1, b2}; the 16-bit kinds share one 2-byte data type, e4m3 and s8 one 1-byte type (TMA
+// only moves the bytes)
 static int encode(EncodeTiledFn enc, CUtensorMap* map, PlaneElem elem, const void* base, cuuint64_t d0, cuuint64_t d1, cuuint64_t d2,
                   cuuint64_t s1, cuuint64_t s2, cuuint32_t b1, cuuint32_t b2, CUtensorMapL2promotion l2) {
     cuuint64_t dims[3] = {d0, d1, d2};
     cuuint64_t strides[2] = {s1, s2};
     cuuint32_t box[3] = {(cuuint32_t)tc_block_ch(elem), b1, b2};
     cuuint32_t es[3] = {1, 1, 1};
-    return (int)enc(map, elem == ELEM_E4M3 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, (void*)base, dims,
+    return (int)enc(map, elem == ELEM_E4M3 || elem == ELEM_S8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, (void*)base, dims,
                     strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, l2, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
@@ -99,7 +101,7 @@ int tc_layer_create(const TcLayerDesc& d, TcLayer& out, std::string& err) {
     if (!enc) { err = "cuTensorMapEncodeTiled unavailable"; return -1; }
     const int kb = tc_block_ch(d.fmt.elem), eb = d.fmt.elem_bytes();
     if (d.in_cused % kb) { err = "input channels not a multiple of " + std::to_string(kb); return -1; }
-    if (d.fmt.planes < 1 || d.fmt.planes > 3 || (d.fmt.e4m3() && d.fmt.planes != 1)) { err = "1 to 3 planes (e4m3: 1)"; return -1; }
+    if (d.fmt.planes < 1 || d.fmt.planes > 3 || ((d.fmt.e4m3() || d.fmt.s8()) && d.fmt.planes != 1)) { err = "1 to 3 planes (e4m3, s8: 1)"; return -1; }
     if (d.ksize < 1 || d.ksize > TC_KMAX) { err = "filter size above " + std::to_string(TC_KMAX) + " (A window rows)"; return -1; }
     out.d = d;
     out.bn = tc_bn(d.cout_pad, d.fmt.planes);
@@ -140,7 +142,7 @@ int tc_layer_launch(const TcLayer& l, int nimg, cudaStream_t st, int share) {
     a.M = (long long)nimg * d.geo.Hs * d.geo.Wp;
     // hi*hi accumulation chunk with split planes and in the fp16 fast mode: one 7-tap filter row (448 K), two 3-tap rows (384 K)
     // or four 1x1 blocks (256 K); e4m3 the same K steps of 128 channels (896, 768, 512 K: DESIGN.md section 6); bf16x1 runs one
-    // chain over the whole K
+    // chain over the whole K, and so does s8, whose integer sums are exact
     const int nk = d.ksize * d.ksize * a.kblocks_per_tap;
     a.chunk_iters = (d.fmt.planes >= 2 || d.fmt.f16() || d.fmt.e4m3()) ? (d.ksize >= 7 ? 7 : (d.ksize >= 3 ? 6 : 4)) : nk;
     static int nsm = 0;

@@ -1,10 +1,11 @@
 // Kernel side of the wgmma / TMA implicit-GEMM convolution (see conv_tc.cu for the design): argument block, PTX
-// wrappers, conv_wg_kernel and its launcher.  Shared by conv_tc.cu (16-bit planes) and conv_fp8.cu (e4m3).
+// wrappers, conv_wg_kernel and its launcher.  Shared by conv_tc.cu (16-bit planes), conv_fp8.cu (e4m3) and conv_s8.cu (s8).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp8.h>
 
 #include <atomic>
+#include <type_traits>
 
 #include "common.h"
 #include "conv_tc.h"
@@ -17,7 +18,8 @@ struct TcArgs {
     void* out; int out_pitch, out_coff; long long out_plane;   // output planes of the kernel's OUT element kind (pitch in elements)
     float* planar; int planar_C, planar_coff;
     int cout, relu;
-    const float* out_scale;                   // -> 2^-k in the packed buffer: the weights of this layer carry a factor 2^k (fp16 planes)
+    const float* out_scale;                   // -> 2^-k in the packed buffer: the weights of this layer carry a factor 2^k (fp16 planes);
+                                              // s8: -> the per-channel epilogue factors f_c [cout_pad]
     int ksize, pad, kblocks_per_tap, cin_k;   // cin_k = channels per tap in the weight K ordering
     int W, H, Wp, Hs;
     long long M;
@@ -213,6 +215,40 @@ PE_WG_E4M3(64, 32, 32, 33, 34, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%1
 PE_WG_E4M3(128, 64, 64, 65, 66, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
                     "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63")
 
+// D(64 x N, s32) (+)= A(64 x 32) * B(N x 32)^T in s8, both K-major; the same register mapping and the same 32-byte K steps as
+// e4m3.  The products and their sums are exact integers: no chunking is needed while |acc| stays inside s32 (the engine
+// bounds K, conv_s8.cu).
+#define PE_WG_S8(N, NR, DA, DB, SD, REGS)                                                                                    \
+    template <> struct WgmmaS8<N> {                                                                                          \
+        __device__ __forceinline__ static void mma(int* d, uint64_t da, uint64_t db, uint32_t scale_d) {                     \
+            asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %" #SD ", 0;\n"                                                  \
+                         "wgmma.mma_async.sync.aligned.m64n" #N "k32.s32.s8.s8 {" REGS "}, %" #DA ", %" #DB ", p;\n}"          \
+                         : PE_WG_OUT##NR##_S32 : "l"(da), "l"(db), "r"(scale_d));                                           \
+        }                                                                                                                    \
+    };
+template <int N> struct WgmmaS8;
+#define PE_WG_OUT8_S32 "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7])
+#define PE_WG_OUT16_S32 PE_WG_OUT8_S32, "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+#define PE_WG_OUT24_S32 PE_WG_OUT16_S32, "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23])
+#define PE_WG_OUT32_S32 PE_WG_OUT24_S32, "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+#define PE_WG_OUT64_S32 PE_WG_OUT32_S32, "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), \
+    "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]),      \
+    "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]),      \
+    "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+PE_WG_S8(16, 8, 8, 9, 10, "%0,%1,%2,%3,%4,%5,%6,%7")
+PE_WG_S8(32, 16, 16, 17, 18, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15")
+PE_WG_S8(48, 24, 24, 25, 26, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23")
+PE_WG_S8(64, 32, 32, 33, 34, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31")
+PE_WG_S8(128, 64, 64, 65, 66, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+                  "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63")
+
+// fp32 -> s8, round to nearest even, saturating to [-128, 127] (cvt.rni.sat.s8.f32; NaN gives 0)
+__device__ __forceinline__ uint32_t f32_to_s8(float x) {
+    int q;
+    asm("cvt.rni.sat.s8.f32 %0, %1;" : "=r"(q) : "f"(x));
+    return (uint32_t)q & 0xffu;
+}
+
 // Range tracking of the 16-bit planes: every epilogue warp folds the largest |value| it stores into one word per layer.  The
 // host reads it to calibrate per-layer power-of-two activation scales (engine.cu, pe_calibrate) and to report values that
 // left the fp16 range instead of letting inf / flushed zeros poison the following layers silently.
@@ -233,8 +269,8 @@ constexpr int TC_BK = 64;            // 16-bit elements per K block = one 128-by
 // stage inputs: 28 % fewer MACs in Mconv1), but it keeps the fp16 kernel's number of K steps - each step's mbarrier waits,
 // releases and descriptor arithmetic - while halving the tensor-core work per step, so the per-step overhead would eat the
 // gain everywhere else.  128-channel blocks keep every byte of the fp16 geometry (boxes, slots, descriptors, the 32-byte K
-// advance) and halve the steps.  The engine pads e4m3 activations to 128 channels (common.h).
-__host__ __device__ constexpr int tc_block_ch(int elem) { return elem == ELEM_E4M3 ? 128 : TC_BK; }
+// advance) and halve the steps.  The engine pads e4m3 and s8 activations to 128 channels (common.h).
+__host__ __device__ constexpr int tc_block_ch(int elem) { return elem == ELEM_E4M3 || elem == ELEM_S8 ? 128 : TC_BK; }
 constexpr int TC_WROWS = TC_BM + 8;  // rows of an A window: the tile plus the row shifts q = 1..8 of a filter row (k <= 9)
 constexpr int TC_KMAX = TC_WROWS - TC_BM + 1;
 constexpr int TC_THREADS = 384;      // warpgroup 0: TMA producer, warpgroups 1-2: consumers
@@ -274,7 +310,8 @@ template <int BN, int PLANES> struct TcShape {
 };
 
 // ELEM: element kind of the A windows and weight tiles; OUT: of the stored output planes (conv1_1 of the e4m3 mode reads
-// its fp16 im2col input and writes e4m3).
+// its fp16 im2col input and writes e4m3).  ELEM = OUT = s8: s32 accumulators over the whole K (the host sets chunk_iters to
+// it), and the per-channel epilogue t = acc * f_c + b'_c (no FMA) before cvt.rni.sat.s8.
 template <int BN, int PLANES, int ELEM, int OUT>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcArgs a) {
@@ -290,7 +327,8 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     uint8_t* const wring = smem;                          // A windows
     uint8_t* const bring = smem + WS * S::A_BYTES;        // B tiles, written by the TMA multicasts of the whole cluster
     __shared__ __align__(8) uint64_t wfull[WS], wempty[WS], bfull[BS], bempty[BS];
-    __shared__ float s_bias[BN];
+    constexpr bool S8 = ELEM == ELEM_S8;
+    __shared__ float s_bias[S8 ? 2 * BN : BN];   // s8: the biases, then the per-channel factors
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // Row tiles start at every image, so none covers only the gap rows after an image's last pixel.  A CTA past the last
@@ -311,6 +349,8 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
     }
     for (int i = threadIdx.x; i < BN; i += TC_THREADS) s_bias[i] = (n0 + i < a.cout) ? a.bias[n0 + i] : 0.f;
+    if constexpr (S8)
+        for (int i = threadIdx.x; i < BN; i += TC_THREADS) s_bias[BN + i] = (n0 + i < a.cout) ? a.out_scale[n0 + i] : 0.f;
     cluster_sync();   // every CTA's barriers are initialised before any multicast or remote arrive reaches them
     pdl_launch_dependents();
     pdl_wait();
@@ -351,7 +391,9 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
     // ===== consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile =====
     const int wg = (warp >> 2) - 1;
-    float acc_h[NACC], sum_h[NACC], acc_c[NACC];
+    using Acc = std::conditional_t<S8, int, float>;
+    Acc acc_h[NACC];
+    float sum_h[NACC], acc_c[NACC];
 #pragma unroll
     for (int j = 0; j < NACC; j++) { acc_h[j] = 0.f; sum_h[j] = 0.f; acc_c[j] = 0.f; }
     const int cs = a.chunk_iters;
@@ -376,7 +418,8 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             wg_fence();
 #pragma unroll
             for (int k = 0; k < 4; k++) {   // 32-byte K steps of the 128-byte rows: k16 in 16 bits, k32 in e4m3
-                if constexpr (ELEM == ELEM_E4M3) WgmmaE4M3<BN>::mma(acc_h, wg_desc(sa + k * 32), wg_desc(sb + k * 32), (k != 0) | h_acc);
+                if constexpr (S8) WgmmaS8<BN>::mma(acc_h, wg_desc(sa + k * 32), wg_desc(sb + k * 32), (k != 0) | h_acc);
+                else if constexpr (ELEM == ELEM_E4M3) WgmmaE4M3<BN>::mma(acc_h, wg_desc(sa + k * 32), wg_desc(sb + k * 32), (k != 0) | h_acc);
                 else Wgmma<BN>::template mma<ELEM == ELEM_F16>(acc_h, wg_desc(sa + k * 32), wg_desc(sb + k * 32), (k != 0) | h_acc);
                 if constexpr (PLANES > 1) {
 #pragma unroll
@@ -399,8 +442,10 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
         wg_wait_all();
         tc_release(bempty, wempty, prev_b, prev_w, lane);
+        if constexpr (!S8) {
 #pragma unroll
-        for (int j = 0; j < NACC; j++) sum_h[j] = __fadd_rn(sum_h[j], acc_h[j]);
+            for (int j = 0; j < NACC; j++) sum_h[j] = __fadd_rn(sum_h[j], acc_h[j]);
+        }
     }
 
     // ===== epilogue: sum, bias, ReLU, re-split into planes, store =====
@@ -422,8 +467,13 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             float v[2];
 #pragma unroll
             for (int e = 0; e < 2; e++) {
-                float t = PLANES > 1 ? __fadd_rn(sum_h[j + e], acc_c[j + e]) : sum_h[j + e];
-                t = __fmaf_rn(t, out_scale, s_bias[c + e]);   // out_scale is a power of two: exact
+                float t;
+                if constexpr (S8) {
+                    t = __fadd_rn(__fmul_rn(__int2float_rn(acc_h[j + e]), s_bias[BN + c + e]), s_bias[c + e]);
+                } else {
+                    t = PLANES > 1 ? __fadd_rn(sum_h[j + e], acc_c[j + e]) : sum_h[j + e];
+                    t = __fmaf_rn(t, out_scale, s_bias[c + e]);   // out_scale is a power of two: exact
+                }
                 if (a.relu) t = fmaxf(t, 0.f);
                 v[e] = t;
                 if (co + e < a.cout) range_max = fmaxf(range_max, fabsf(t));
@@ -432,6 +482,9 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
                 for (int e = 0; e < 2; e++)
                     if (co + e < a.cout) a.planar[(((size_t)n * a.planar_C + a.planar_coff + co + e) * a.H + y) * a.W + x] = v[e];
+            } else if constexpr (OUT == ELEM_S8) {
+                if (co < cout8)
+                    *(uint16_t*)((int8_t*)a.out + (size_t)m * a.out_pitch + a.out_coff + co) = (uint16_t)(f32_to_s8(v[0]) | f32_to_s8(v[1]) << 8);
             } else if (OUT == ELEM_E4M3) {
                 // round to nearest, saturating to +-448 as the range check expects (a larger |t| is PE_ERR_RANGE)
                 if (co < cout8)
@@ -474,5 +527,7 @@ static int launch_inst(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_
 
 // The e4m3 instances (conv_fp8.cu): layers of fmt e4m3, and fp16-input layers with out_e4m3; bn = the grid's tile width.
 int launch_e4m3(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap, int bn);
+// The s8 instances (conv_s8.cu): layers of fmt s8.
+int launch_s8(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap, int bn);
 
 }  // namespace pe

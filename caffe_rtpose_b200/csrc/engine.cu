@@ -17,6 +17,7 @@
 #include "kernels.h"
 #include "conv_tc.h"
 #include "e4m3.h"
+#include "s8.h"
 #include "jpeg_coefs.h"
 #include "jpeg_entropy.cuh"
 #include "pixels.cuh"
@@ -52,6 +53,7 @@ struct pe_engine {
     // biases / weight-scale inverses the packed epilogue fields derive from, and the kernels' running max |stored value| per conv
     std::vector<float> conv_scale, wsi;   // per conv: scale of its stored output; inverse of the power of two folded into its weights
     std::vector<std::vector<float>> bias_true;
+    std::vector<std::vector<float>> wsig;   // S8X1: per conv, the per-output-channel weight step sigma_c of pack_conv_weights (s8.h)
     unsigned* d_range = nullptr;
     bool calibrated = false, check_range = false;
     std::vector<size_t> w_off, b_off;
@@ -118,10 +120,17 @@ static PlaneFmt act_fmt(const pe_engine* e, int i) {
     return e->fmt.e4m3() && i == e->plan.input_act ? PlaneFmt{1, ELEM_F16} : e->fmt;
 }
 static PlaneFmt conv_wfmt(const pe_engine* e, int i) { return act_fmt(e, e->plan.convs[i].in_act); }
-// channel granularity of the activations (common.h): 16 (fp32 SIMT), 64 (16-bit planes), 128 (e4m3: one K block, conv_tc_kernel.cuh)
-static int act_cpad(int precision) { return precision == PE_PREC_FP32_SIMT ? 16 : precision == PE_PREC_E4M3X1 ? 128 : 64; }
-// Concat slot granularity (common.h, build_plan_from_net): 16 bytes of e4m3, 8 channels otherwise
-static int slot_align(int precision) { return precision == PE_PREC_E4M3X1 ? 16 : 8; }
+// channel granularity of the activations (common.h): 16 (fp32 SIMT), 64 (16-bit planes), 128 (e4m3, s8: one K block, conv_tc_kernel.cuh)
+static bool one_byte(int precision) { return precision == PE_PREC_E4M3X1 || precision == PE_PREC_S8X1; }
+static int act_cpad(int precision) { return precision == PE_PREC_FP32_SIMT ? 16 : one_byte(precision) ? 128 : 64; }
+// Concat slot granularity (common.h, build_plan_from_net): 16 bytes of e4m3 / s8, 8 channels otherwise
+static int slot_align(int precision) { return one_byte(precision) ? 16 : 8; }
+// channel pitch of the im2col'ed net input: 32 fp32 (SIMT), 64 fp16 / bf16 (e4m3 keeps fp16), 128 s8 (one K block)
+static int kp_input(int precision) { return precision == PE_PREC_FP32_SIMT ? 32 : precision == PE_PREC_S8X1 ? 128 : 64; }
+// S8X1: |acc| <= 128 * 127 * K must stay inside s32, so K = taps x padded input channels is at most 132104 (conv_s8.cu)
+static const long long S8_MAX_K = 132104;
+// floats of conv i's epilogue fields in the packed buffer: bias[cout_pad], then the layer's factor (S8X1: a factor per channel)
+static size_t epi_floats(const pe_engine* e, int i) { return (size_t)e->cout_pad[i] + (e->fmt.s8() ? e->cout_pad[i] : 1); }
 static size_t fmt_bytes(PlaneFmt f) { return (size_t)f.elem_bytes() * (f.planes ? f.planes : 1); }   // bytes per element, all planes
 
 static int fail(pe_engine* e, int code, const char* fmt, ...) {
@@ -312,7 +321,7 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
     if (prototxt_path) {
         std::string perr;
         if (parse_prototxt_file(prototxt_path, netdef, perr)) return fail(nullptr, PE_ERR_IO, "%s: %s", prototxt_path, perr.c_str());
-        if (build_plan_from_net(netdef, cfg->precision ? 64 : 32, act_cpad(cfg->precision), proto_plan, perr, slot_align(cfg->precision)))
+        if (build_plan_from_net(netdef, kp_input(cfg->precision), act_cpad(cfg->precision), proto_plan, perr, slot_align(cfg->precision)))
             return fail(nullptr, PE_ERR_INVALID, "%s: %s", prototxt_path, perr.c_str());
         if (cfg->model >= 0 && cfg->model != proto_plan.model)
             return fail(nullptr, PE_ERR_INVALID, "%s describes the %s model (nms num_parts %d), the configuration asks for model %d", prototxt_path,
@@ -326,7 +335,7 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
     if (cfg->max_batch < 1 || cfg->max_batch > 64) return fail(nullptr, PE_ERR_INVALID, "max_batch %d out of [1,64]", cfg->max_batch);
     if (check_resize_scales(nullptr, (float)cfg->start_scale, (float)cfg->scale_gap, cfg->num_scales)) return PE_ERR_INVALID;
     if (cfg->disp_w <= 0 || cfg->disp_h <= 0) return fail(nullptr, PE_ERR_INVALID, "bad display resolution");
-    if (cfg->precision < 0 || cfg->precision > PE_PREC_E4M3X1) return fail(nullptr, PE_ERR_INVALID, "unknown precision %d", cfg->precision);
+    if (cfg->precision < 0 || cfg->precision > PE_PREC_S8X1) return fail(nullptr, PE_ERR_INVALID, "unknown precision %d", cfg->precision);
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
         return fail(nullptr, PE_ERR_CUDA, "no CUDA device visible: the pose engine has no CPU fallback");
@@ -356,7 +365,16 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
     for (int i = 0; i < 16; i++) CKC(cudaEventCreate(&e->ev[i]));
 
     // the plan first: each level's gap is the largest pad of its convolutions (common.h)
-    e->plan = prototxt_path ? proto_plan : build_plan(cfg->model, e->fmt.planes ? 64 : 32, act_cpad(cfg->precision), slot_align(cfg->precision));
+    e->plan = prototxt_path ? proto_plan : build_plan(cfg->model, kp_input(cfg->precision), act_cpad(cfg->precision), slot_align(cfg->precision));
+    if (e->fmt.s8())
+        for (const ConvSpec& c : e->plan.convs) {
+            const long long K = (long long)(c.im2col_input ? 1 : c.k * c.k) * c.in_cused;
+            if (K > S8_MAX_K) {
+                fail(e, PE_ERR_INVALID, "layer %s: K = %lld (%dx%d taps x %d padded input channels) exceeds %lld, the largest K whose s8 sums "
+                     "stay inside s32 (|acc| <= 128 x 127 x K): PE_PREC_S8X1 cannot run it", c.name.c_str(), K, c.k, c.k, c.in_cused, S8_MAX_K);
+                return bail(PE_ERR_INVALID);
+            }
+        }
     const int N = cfg->max_batch * cfg->num_scales;
     int w = cfg->net_w, h = cfg->net_h;
     for (int l = 0; l < 4; l++) {
@@ -567,7 +585,7 @@ static size_t packed_layout(pe_engine* e) {
         e->w_off[i] = total;
         total = align256(total + K * e->cout_pad[i] * fmt_bytes(conv_wfmt(e, (int)i)));
         e->b_off[i] = total;
-        total = align256(total + (size_t)(e->cout_pad[i] + 1) * 4);   // bias[cout_pad] + the layer's epilogue scale
+        total = align256(total + epi_floats(e, (int)i) * 4);   // bias[cout_pad] + the layer's epilogue scale (S8X1: one per channel)
     }
     return total;
 }
@@ -577,21 +595,28 @@ static size_t packed_layout(pe_engine* e) {
 // next to the previous stage's L1 / L2 outputs) folds the ratios into its weights: packed w[ci] = w[ci] * s_ref / s(ci) * 2^k, so that
 //   acc = 2^k * s_ref * sum_ci w[ci] * a[ci]     and     stored = acc * out_scale + bias,  out_scale = s_out / (2^k * s_ref),
 // bias = true bias * s_out - all factors powers of two, hence exact, and ReLU commutes with them: range scaling is free at run time.
+// S8X1 replaces 2^k by a step per output channel (sigma_c, s8.h): acc * sigma_c ~ s_ref * sum w a, and the factor of channel c
+// is f_c = sigma_c * s_out / s_ref.  Its net input is stored as (p - 128) = (p/256 - 0.5) * 2^8: scale 256.
+static float net_input_scale(const pe_engine* e) { return e->fmt.s8() ? 256.f : 1.f; }
 static float input_ref_scale(const pe_engine* e, const ConvSpec& c) {
     for (int pc : c.cin_prod) if (pc >= 0) return e->conv_scale[pc];
-    return 1.f;   // the net input
+    return net_input_scale(e);   // the net input
 }
 static void fill_epilogue_fields(const pe_engine* e, int i, float* B) {
     const ConvSpec& c = e->plan.convs[i];
     const float s_ref = input_ref_scale(e, c);
     const float s_out = c.out_act >= 0 ? e->conv_scale[i] : 1.f;   // the planar stride-8 maps are true values
     for (int co = 0; co < c.cout; co++) B[co] = e->bias_true[i][co] * s_out;
+    if (e->fmt.s8()) {
+        for (int co = 0; co < c.cout; co++) B[e->cout_pad[i] + co] = e->wsig[i][co] * (s_out / s_ref);
+        return;
+    }
     B[e->cout_pad[i]] = e->wsi[i] * s_out / s_ref;
 }
 
 // Weights of conv i into `dst` (the layer's region of the packed buffer, host copy): fp32 [K][cout_pad] for the SIMT mode, else
 // P 16-bit planes [P][cout_pad][K] (K-major rows: the wgmma B operand) of w * 2^k, the per-channel range ratios folded in.
-// Sets e->wsi[i] = 2^-k.
+// Sets e->wsi[i] = 2^-k.  S8X1: one s8 plane [cout_pad][K], each output channel quantised on its own (s8.h); sets e->wsig[i].
 static void pack_conv_weights(pe_engine* e, int i, uint8_t* dst) {
     const ConvSpec& c = e->plan.convs[i];
     const HostWeights& hw = e->hw[i];
@@ -615,7 +640,14 @@ static void pack_conv_weights(pe_engine* e, int i, uint8_t* dst) {
     const PlaneFmt wf = conv_wfmt(e, i);
     memset(dst, 0, K * cop * fmt_bytes(wf));
     float wscale_inv = 1.f;
-    if (wf.planes == 0) {  // fp32 [K][cout_pad]
+    if (wf.s8()) {
+        std::vector<float> wc(K);
+        e->wsig[i].assign(cop, 0.f);
+        for (int co = 0; co < c.cout; co++) {
+            for (size_t kk = 0; kk < K; kk++) wc[kk] = src(co, (int)kk);
+            e->wsig[i][co] = s8_quantize_channel(wc.data(), K, (int8_t*)dst + (size_t)co * K);
+        }
+    } else if (wf.planes == 0) {  // fp32 [K][cout_pad]
         float* W = (float*)dst;
         for (size_t kk = 0; kk < K; kk++)
             for (int co = 0; co < c.cout; co++) W[kk * cop + co] = src(co, (int)kk);
@@ -701,6 +733,7 @@ extern "C" int pe_commit_weights(pe_engine* e) {
     e->bias_true.assign(nc, std::vector<float>());
     e->calibrated = false;
     e->wsi.assign(nc, 1.f);
+    e->wsig.assign(nc, std::vector<float>());
     e->conv_scale.assign(nc, 1.f);
     std::vector<uint8_t> host(total, 0);
     for (size_t i = 0; i < nc; i++) {
@@ -805,6 +838,9 @@ extern "C" int pe_broadcast_weights(pe_engine* const* engines, int n) {
     for (int i = 0; i < n; i++) { cudaSetDevice(devs[i]); cudaStreamSynchronize(engines[i]->stream); }
     for (int i = 0; i < n; i++) destroy(comms[i]);
     if (rc || rc2) return fail(root, PE_ERR_CUDA, "ncclBroadcast: %s", errstr ? errstr(rc ? rc : rc2) : "error");
+    // the range scales travel inside the packed buffer; the replicas also take the host copy that pe_fetch_blob divides out and
+    // the calibration state that an S8X1 forward requires
+    for (int i = 1; i < n; i++) { engines[i]->conv_scale = root->conv_scale; engines[i]->calibrated = root->calibrated; }
     return PE_OK;
 }
 
@@ -976,6 +1012,9 @@ static int setup_lanes(pe_engine* e) {
 
 static int run_net(pe_engine* e, int n) {
     if (!e->committed) return fail(e, PE_ERR_STATE, "pe_commit_weights has not been called");
+    // at scale 1 almost every activation of a typical net quantises to 0
+    if (e->fmt.s8() && !e->calibrated)
+        return fail(e, PE_ERR_STATE, "PE_PREC_S8X1 runs on calibrated range scales: call pe_calibrate (on the handle that owns the weights) before the first forward");
     if (!e->use_graphs) return run_net_eager(e, n);
     pe_engine::GraphEntry& g = e->graphs[n];
     if (g.exec) {
@@ -1398,7 +1437,7 @@ extern "C" int pe_jpeg_decode_scans(pe_engine* e, const void* const* scans, int 
 // layer that left the range (PE_ERR_RANGE), and with PE_CHECK_RANGE=1 every pe_fetch does.
 // ---------------------------------------------------------------------------------------------
 static int upload_fields(pe_engine* e, int i) {
-    std::vector<float> B((size_t)e->cout_pad[i] + 1, 0.f);
+    std::vector<float> B(epi_floats(e, i), 0.f);
     fill_epilogue_fields(e, i, B.data());
     CK(e, cudaMemcpyAsync((char*)e->d_packed + e->b_off[i], B.data(), B.size() * sizeof(float), cudaMemcpyHostToDevice, e->stream));
     return PE_OK;
@@ -1453,7 +1492,8 @@ extern "C" int pe_calibrate(pe_engine* e, const uint8_t* const* frames, int n) {
             CK(e, cudaStreamSynchronize(e->stream));
             float m; memcpy(&m, &bits, 4);
             // m * s in [32, 64) for fp16 (1000x headroom to 65504); in [64, 128) for e4m3 (3.5-7x headroom to 448, and values
-            // down to m * s * 2^-12 stay normal)
+            // down to m * s * 2^-12 stay normal); in [32, 64) for s8: 6 bits, and 2-4x headroom to 127 for frames busier than
+            // the calibration frame
             const int top = e->fmt.e4m3() ? 7 : 6;
             if (m > 0.f && m < 3e38f) { int ex = 0; frexpf(m, &ex); e->conv_scale[i] = ldexpf(1.f, std::max(-100, std::min(100, top - ex))); }
         }
@@ -1468,7 +1508,8 @@ extern "C" int pe_calibrate(pe_engine* e, const uint8_t* const* frames, int n) {
 // Largest |stored value| / the format's largest finite value (65504 for fp16, 448 for e4m3) over the conv layers since the last
 // call.  PE_ERR_RANGE when a layer reached that limit, or when a layer's maximum fell below a floor: fp16 2^-10 (its lo plane then
 // lives in fp16 subnormals and parity is lost); e4m3 2^-2, 16x above the smallest normal 2^-6, so that values a sixteenth of
-// the maximum - the bulk of a layer's outputs - are still normal.  *layer64 names the worst layer.
+// the maximum - the bulk of a layer's outputs - are still normal.  s8: the largest stored value rint(max |t|) / 127; PE_ERR_RANGE
+// when it reaches 127 (the layer saturates) or stays below 4 (under 3 bits).  *layer64 names the worst layer.
 extern "C" int pe_range_status(pe_engine* e, float* worst_ratio, char* layer64) {
     if (!e) return PE_ERR_INVALID;
     if (worst_ratio) *worst_ratio = 0.f;
@@ -1480,15 +1521,16 @@ extern "C" int pe_range_status(pe_engine* e, float* worst_ratio, char* layer64) 
     std::vector<unsigned> bits(nc);
     CK(e, cudaMemcpy(bits.data(), e->d_range, nc * sizeof(unsigned), cudaMemcpyDeviceToHost));
     CK(e, cudaMemset(e->d_range, 0, nc * sizeof(unsigned)));
-    const bool e4 = e->fmt.e4m3();
-    const float limit = e4 ? 448.f : 65504.f, floor_ = e4 ? 0.25f : 9.765625e-4f;
-    const char* what = e4 ? "the e4m3 planes" : "the fp16 planes";
+    const bool e4 = e->fmt.e4m3(), s8 = e->fmt.s8();
+    const float limit = e4 ? 448.f : s8 ? 127.f : 65504.f, floor_ = e4 ? 0.25f : s8 ? 4.f : 9.765625e-4f;
+    const char* what = e4 ? "the e4m3 planes" : s8 ? "the s8 planes" : "the fp16 planes";
     float worst = 0.f, smallest = 3e38f;
     int iw = -1, is = -1;
     for (size_t i = 0; i < nc; i++) {
         if (e->plan.convs[i].out_act < 0) continue;   // fp32 maps
         float m; memcpy(&m, &bits[i], 4);
         if (bits[i] == 0) continue;                   // layer did not run since the last call
+        if (s8 && m <= 3e38f) m = rintf(m);           // the kernels track |t| before the rounding: the stored value
         if (!(m <= 3e38f) || m / limit > worst) { worst = (m <= 3e38f) ? m / limit : 2.f; iw = (int)i; }
         if (m < smallest) { smallest = m; is = (int)i; }
     }
@@ -1501,7 +1543,7 @@ extern "C" int pe_range_status(pe_engine* e, float* worst_ratio, char* layer64) 
     if (is >= 0 && smallest < floor_) {
         if (layer64) snprintf(layer64, 64, "%s", e->plan.convs[is].name.c_str());
         return fail(e, PE_ERR_RANGE, "layer %s: largest stored value %.3g is below %s, %s lose precision: run pe_calibrate",
-                    e->plan.convs[is].name.c_str(), smallest, e4 ? "2^-2" : "2^-10", what);
+                    e->plan.convs[is].name.c_str(), smallest, e4 ? "2^-2" : s8 ? "4" : "2^-10", what);
     }
     if (layer64 && iw >= 0) snprintf(layer64, 64, "%s", e->plan.convs[iw].name.c_str());
     return PE_OK;
@@ -1663,6 +1705,23 @@ extern "C" int pe_fetch_maps(pe_engine* e, float* maps8, int n) {
     memcpy(maps8, e->h_maps, cnt * sizeof(float));
     return PE_OK;
 }
+static float blob_scale(const pe_engine* e, const BlobRef& b) {
+    if (b.prod >= 0 && b.prod < (int)e->conv_scale.size()) return e->conv_scale[b.prod];
+    return b.act == e->plan.input_act ? net_input_scale(e) : 1.f;
+}
+extern "C" int pe_blob_log2_scale(pe_engine* e, const char* blob_name, int* k) {
+    if (!e || !blob_name || !k) return PE_ERR_INVALID;
+    if (!e->fmt.ranged()) return fail(e, PE_ERR_INVALID, "this precision has no range scales");
+    for (const BlobRef& b : e->plan.blobs) {
+        if (b.name != blob_name) continue;
+        int ex = 0;
+        const float f = frexpf(blob_scale(e, b), &ex);   // a power of two: f = 0.5
+        if (f != 0.5f) return fail(e, PE_ERR_STATE, "blob %s: scale is not a power of two", blob_name);
+        *k = ex - 1;
+        return PE_OK;
+    }
+    return fail(e, PE_ERR_INVALID, "unknown blob %s", blob_name);
+}
 extern "C" int pe_fetch_blob(pe_engine* e, const char* blob_name, float* out, size_t cap, int* c, int* h, int* w) {
     if (!e || !blob_name) return PE_ERR_INVALID;
     CK(e, cudaSetDevice(e->cfg.device));
@@ -1681,8 +1740,9 @@ extern "C" int pe_fetch_blob(pe_engine* e, const char* blob_name, float* out, si
         if (cnt > cap) return fail(e, PE_ERR_INVALID, "blob %s needs %zu floats", blob_name, cnt);
         float* d = nullptr;
         CK(e, cudaMalloc(&d, cnt * sizeof(float)));
-        // stored value = true value * conv_scale[producer] (pools pass their producer's scale through; the net input has none)
-        const float inv = (b.prod >= 0 && b.prod < (int)e->conv_scale.size()) ? 1.f / e->conv_scale[b.prod] : 1.f;
+        // stored value = true value * conv_scale[producer] (pools pass their producer's scale through; the net input has
+        // net_input_scale); s8: q * 2^-k, exact in fp32
+        const float inv = 1.f / blob_scale(e, b);
         e->launches += launch_act_to_nchw(e->acts[b.act], e->plan.acts[b.act].C, b.coff, b.c, e->act_plane[b.act], act_fmt(e, b.act), g, inv, d,
                                           e->stream);
         CK(e, cudaMemcpyAsync(out, d, cnt * sizeof(float), cudaMemcpyDeviceToHost, e->stream));

@@ -2,7 +2,7 @@
 //
 // Pooling semantics: src/caffe/layers/pooling_layer.cpp:90-93 (ceil), :128-187 (max over the window clipped
 // to the image).  Activations are either fp32 [M][C], 16-bit "planes" whose SUM is the value (split
-// precision for the wgmma conv, see conv_tc.cu), or one e4m3 plane; the max is taken on the reconstructed
+// precision for the wgmma conv, see conv_tc.cu), or one e4m3 or s8 plane; the max is taken on the reconstructed
 // value and the winner's planes are copied, which keeps the split exact.
 #include "common.h"
 #include "kernels.h"
@@ -84,9 +84,11 @@ __global__ void __launch_bounds__(256) pool_planes_kernel(PoolArgs a) {
         *((uint4*)((__nv_bfloat16*)a.out + (size_t)p * a.out_plane + mo * a.C) + g) = o[p];
 }
 
-// e4m3 (one byte per channel): 16 channels per thread.  Rounding is monotone, so the max of the stored values is the stored
+// e4m3 / s8 (one byte per channel): 16 channels per thread.  Rounding is monotone, so the max of the stored values is the stored
 // max: the winner's byte is copied.
-__global__ void __launch_bounds__(256) pool_e4m3_kernel(PoolArgs a) {
+template <bool S8> __device__ __forceinline__ float byte_value(uint8_t b) { return S8 ? (float)(int8_t)b : e4m3_to_float(b); }
+template <bool S8>
+__global__ void __launch_bounds__(256) pool_bytes_kernel(PoolArgs a) {
     const unsigned cv = a.C / 16;
     const int n = blockIdx.y;
     const unsigned per_img = (unsigned)a.Hso * (unsigned)a.Wpo;
@@ -110,11 +112,11 @@ __global__ void __launch_bounds__(256) pool_e4m3_kernel(PoolArgs a) {
 #pragma unroll
     for (int j = 0; j < 16; j++) {
         uint8_t b = ((const uint8_t*)&v[0])[j];
-        float best = e4m3_to_float(b);
+        float best = byte_value<S8>(b);
 #pragma unroll
         for (int w = 1; w < 4; w++) {
             const uint8_t c = ((const uint8_t*)&v[w])[j];
-            const float f = e4m3_to_float(c);
+            const float f = byte_value<S8>(c);
             if (ok[w] && f > best) { best = f; b = c; }
         }
         ((uint8_t*)&o)[j] = b;
@@ -128,9 +130,10 @@ int launch_pool(const PoolArgs& a, cudaStream_t st) {
     if (f.planes == 0) {
         const long long total = rows_out * (a.C / 4);
         pool_f32_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(a);
-    } else if (f.e4m3()) {
+    } else if (f.e4m3() || f.s8()) {
         const unsigned per = (unsigned)a.Hso * a.Wpo * (a.C / 16);
-        pool_e4m3_kernel<<<dim3((per + 255) / 256, a.N), 256, 0, st>>>(a);
+        if (f.s8()) pool_bytes_kernel<true><<<dim3((per + 255) / 256, a.N), 256, 0, st>>>(a);
+        else pool_bytes_kernel<false><<<dim3((per + 255) / 256, a.N), 256, 0, st>>>(a);
     } else {
         const unsigned per = (unsigned)a.Hso * a.Wpo * (a.C / 8);
         const dim3 grid((per + 255) / 256, a.N);
@@ -176,6 +179,7 @@ __global__ void __launch_bounds__(256) act_to_nchw_kernel(const void* act, int p
     float v = 0.f;
     if (fmt.planes == 0) v = ((const float*)act)[m * pitch + coff + ch];
     else if (fmt.e4m3()) v = e4m3_to_float(((const uint8_t*)act)[m * pitch + coff + ch]);
+    else if (fmt.s8()) v = (float)((const int8_t*)act)[m * pitch + coff + ch];
     else for (int p = 0; p < fmt.planes; p++) {
         const uint16_t h = ((const uint16_t*)act)[p * plane + m * pitch + coff + ch];
         v += fmt.f16() ? plane_to_float<true>(h) : plane_to_float<false>(h);

@@ -117,6 +117,46 @@ int launch_warp_affine(const WarpArgs& a, int nframes, cudaStream_t st) {
     return 1;
 }
 
+// S8X1: one s8 plane of 128 channels per pixel, the 27 patch values at scale 2^8 - p - 128 from the uint8 path (exact), and
+// sat(rint(x * 256)) from a planar fp32 input - in the first 32 bytes (channels 27..31 written as 0); the rest stays zero from
+// init.  SRC as in input_im2col_kernel.  One thread = one pixel.
+template <int SRC>
+__global__ void __launch_bounds__(256) input_im2col_s8_kernel(PreArgs a, const float* planar, int nimages) {
+    const int n = blockIdx.y;
+    const unsigned per_img = (unsigned)a.net_h * (unsigned)a.net_w;
+    const unsigned idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= per_img) return;
+    const int y = (int)(idx / (unsigned)a.net_w), x = (int)(idx % (unsigned)a.net_w);
+    const AreaTab& t = a.tab[SRC == 0 ? n % a.S : 0];
+    const uint8_t* img = a.resized + (size_t)n * a.net_h * a.net_w * 3;
+    uint32_t pk[8] = {};
+#pragma unroll
+    for (int k = 0; k < 27; k++) {
+        const int tap = k / 3, c = k % 3;
+        const int yy = y + tap / 3 - 1, xx = x + tap % 3 - 1;
+        int q = 0;
+        if (yy >= 0 && yy < a.net_h && xx >= 0 && xx < a.net_w) {
+            if (SRC == 0) {
+                const int oy = yy - t.padh, ox = xx - t.padw;
+                if (oy >= 0 && oy < t.th && ox >= 0 && ox < t.tw) q = (int)img[((size_t)oy * t.tw + ox) * 3 + c] - 128;
+            } else {
+                q = __float2int_rn(fminf(fmaxf(__fmul_rn(planar[((size_t)n * 3 + c) * a.net_h * a.net_w + (size_t)yy * a.net_w + xx], 256.f),
+                                               -128.f), 127.f));
+            }
+        }
+        pk[k / 4] |= ((uint32_t)q & 0xffu) << (8 * (k % 4));
+    }
+    const long long m = ((long long)n * a.Hs + y) * a.Wp + x;
+    uint4* o = (uint4*)((int8_t*)a.out + (size_t)m * a.kp);
+    o[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+    o[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
+}
+static void launch_im2col_s8(const PreArgs& a, const float* planar, int nimages, cudaStream_t st) {
+    const unsigned per = (unsigned)a.net_h * a.net_w;
+    if (planar) input_im2col_s8_kernel<1><<<dim3((per + 255) / 256, nimages), 256, 0, st>>>(a, planar, nimages);
+    else input_im2col_s8_kernel<0><<<dim3((per + 255) / 256, nimages), 256, 0, st>>>(a, nullptr, nimages);
+}
+
 template <bool F16> __device__ __forceinline__ void split3(float x, uint16_t& h, uint16_t& m, uint16_t& l) {
     h = float_to_plane<F16>(x);
     const float r = __fsub_rn(x, plane_to_float<F16>(h));
@@ -232,6 +272,7 @@ __global__ void __launch_bounds__(256) input_im2col_u8_kernel(PreArgs a) {
 }
 
 static int launch_im2col_u8(const PreArgs& a, cudaStream_t st) {
+    if (a.fmt.s8()) { launch_im2col_s8(a, nullptr, a.nframes * a.S, st); return 1; }
     if (a.fmt.planes > 0 && a.kp >= 32) {
         const dim3 g((a.net_w + 31) / 32, (a.net_h + 7) / 8, a.nframes * a.S), b(32, 8);
         if (a.fmt.f16()) input_im2col_u8_kernel<true><<<g, b, 0, st>>>(a);
@@ -249,6 +290,7 @@ int launch_preprocess(const PreArgs& a, cudaStream_t st) {
 }
 
 int launch_input_from_planar(const float* planar, const PreArgs& a, int nimages, cudaStream_t st) {
+    if (a.fmt.s8()) { launch_im2col_s8(a, planar, nimages, st); return 1; }
     const unsigned work = (unsigned)a.Hs * a.Wp * (a.kp / 8);
     input_im2col_kernel<1><<<dim3((work + 255) / 256, nimages), 256, 0, st>>>(a, planar, nimages);
     return 1;

@@ -1,0 +1,25 @@
+// Host quantisation of one output channel's weights for PE_PREC_S8X1 (engine.cu packs every channel with it, after the range
+// ratios of its input channels are folded in):
+//   sigma = max|w| / 127 in fp32,   q = clamp(rint(w / sigma), -127, 127) in fp32 (rint: ties to even),
+// and an all-zero channel has sigma = 0 and q = 0.  The epilogue multiplies the s32 sum by sigma (times the range scales).
+// Plain C++ without CUDA, so that a CPU test compiles it on its own.
+#pragma once
+#include <math.h>
+#include <stddef.h>
+#include <stdint.h>
+
+namespace pe {
+
+inline float s8_quantize_channel(const float* w, size_t n, int8_t* q) {
+    float m = 0.f;
+    for (size_t i = 0; i < n; i++) m = fmaxf(m, fabsf(w[i]));
+    const float sigma = m / 127.f;
+    for (size_t i = 0; i < n; i++) {
+        float r = sigma > 0.f ? rintf(w[i] / sigma) : 0.f;
+        r = fminf(fmaxf(r, -127.f), 127.f);
+        q[i] = (int8_t)r;
+    }
+    return sigma;
+}
+
+}  // namespace pe

@@ -22,6 +22,7 @@ PREC_FP32_SIMT, PREC_BF16X1, PREC_BF16X2, PREC_BF16X3 = 0, 1, 2, 3
 PREC_F16X2 = PREC_BF16X2   # the parity mode: 2 fp16 planes, chunked round-to-nearest accumulation (poseengine.h)
 PREC_F16X1 = 4             # the fast mode: the parity mode's hi plane alone, one MMA per MAC (poseengine.h)
 PREC_E4M3X1 = 5            # the FP8 mode: one e4m3 plane, one FP8 MMA per MAC; needs calibrate() (poseengine.h)
+PREC_S8X1 = 6              # the INT8 mode: one s8 plane, one s8 MMA per MAC, exact s32 sums; forward needs calibrate() first
 MAX_PEOPLE = 96
 # pixel formats of forward_pixels / pixels_to_bgr (PE_PIX_*, poseengine.h)
 PIX_BGR, PIX_RGB, PIX_YUYV, PIX_NV12, PIX_I420 = 0, 1, 2, 3, 4
@@ -66,7 +67,7 @@ ABI_SYMBOLS = [
     "pe_camera_open", "pe_camera_close", "pe_camera_info", "pe_camera_grab", "pe_camera_last_error", "pe_yuyv_to_bgr",
     "pe_compare_results", "pe_jpeg_read_coefs", "pe_jpeg_coefs_to_bgr", "pe_forward_jpeg_coefs", "pe_video_read_coefs",
     "pe_jpeg_read_scan", "pe_jpeg_scan_to_coefs_host", "pe_forward_jpeg_scans", "pe_jpeg_decode_scans", "pe_video_read_scan",
-    "pe_forward_pixels", "pe_stream_wait", "pe_pixels_to_bgr",
+    "pe_forward_pixels", "pe_stream_wait", "pe_pixels_to_bgr", "pe_blob_log2_scale",
 ]
 
 
@@ -117,6 +118,7 @@ def lib():
     L.pe_fetch.argtypes = [C.c_void_p, C.c_int, _f32p, C.POINTER(C.c_int), C.c_void_p]
     L.pe_fetch_maps.argtypes = [C.c_void_p, _f32p, C.c_int]
     L.pe_fetch_blob.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_size_t] + [C.POINTER(C.c_int)] * 3
+    L.pe_blob_log2_scale.argtypes = [C.c_void_p, C.c_char_p, C.POINTER(C.c_int)]
     L.pe_sync.argtypes = [C.c_void_p]
     L.pe_host_alloc.argtypes = [C.c_size_t]
     L.pe_host_alloc.restype = C.c_void_p
@@ -463,7 +465,7 @@ class PoseEngine:
         self._ck(lib().pe_calibrate(self._h, arr, len(frames)))
 
     def range_status(self):
-        """(rc, worst |stored value| / the format's largest finite value (fp16 65504, e4m3 448), layer name); rc != 0
+        """(rc, worst |stored value| / the format's largest finite value (fp16 65504, e4m3 448, s8 127), layer name); rc != 0
         (PE_ERR_RANGE = 5) when a layer left the format's range."""
         worst = C.c_float()
         name = C.create_string_buffer(64)
@@ -496,6 +498,13 @@ class PoseEngine:
         self._ck(lib().pe_fetch_blob(self._h, name.encode(), out.ctypes.data_as(C.c_void_p), out.size, C.byref(c),
                                      C.byref(h), C.byref(w)))
         return out
+
+    def blob_log2_scale(self, name):
+        """k such that the blob's stored values are fetch_blob(name) * 2^k (pe_blob_log2_scale): the range scale of its producer,
+        8 for the net input in PREC_S8X1.  In PREC_S8X1, fetch_blob(name) * 2^k are the integers a layer read."""
+        k = C.c_int()
+        self._ck(lib().pe_blob_log2_scale(self._h, name.encode(), C.byref(k)))
+        return k.value
 
     def json(self, joints, frame_scale=1.0):
         return write_json(joints, self.num_parts, frame_scale)

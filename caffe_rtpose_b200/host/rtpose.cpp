@@ -92,13 +92,15 @@ static void define_flags() {
     define("model", "", "[extension] COCO or MPI when --caffeproto is not readable");
     define("precision", "2", "[extension] conv arithmetic: 0 fp32 SIMT, 1 bf16 (A/B only), 2 parity mode (two fp16 planes, 3 MMAs per MAC), "
            "3 three bf16 planes (A/B only), 4 fast mode (one fp16 plane, 1 MMA per MAC; see --audit_every), "
-           "5 FP8 mode (one e4m3 plane, 1 FP8 MMA per MAC; needs --calibrate_range, see --audit_every)");
+           "5 FP8 mode (one e4m3 plane, 1 FP8 MMA per MAC; needs --calibrate_range, see --audit_every), "
+           "6 INT8 mode (one s8 plane, 1 s8 MMA per MAC, exact integer sums, per-channel weight scales; requires --calibrate_range, "
+           "see --audit_every)");
     define("batch", "0", "[extension] frames per forward per GPU: 1 = the reference's behaviour, 0 = automatic (file / synthetic sources "
            "fill two waves of 128-row tiles on the GPU, e.g. 9 frames at 656x368; results do not depend on it)");
     define("engines_per_gpu", "0", "[extension] worker handles per GPU: 1 = the reference's topology (one Net per GPU), 0 = automatic (2 when "
            "--batch is automatic: the copies and the kernel tails of one batch overlap the other; weights are shared, not duplicated)");
-    define("calibrate_range", "true", "[extension] fp16 and e4m3 modes (--precision 2, 4 and 5): derive per-layer power-of-two activation scales from one synthetic frame at start-up "
-           "(pe_calibrate), so that a model of any magnitude keeps fp32-level results", true);
+    define("calibrate_range", "true", "[extension] fp16, e4m3 and s8 modes (--precision 2, 4, 5 and 6): derive per-layer power-of-two activation scales from one synthetic frame at start-up "
+           "(pe_calibrate), so that a model of any magnitude keeps fp32-level results; --precision 6 cannot run without them", true);
     define("audit_every", "0", "[extension] N > 0: every worker also holds a parity-mode (--precision 2) handle and forwards every N-th batch "
            "through it too; each frame's peaks, person count and joints are compared with the fast handle's (within 1e-3 net px). The status "
            "line reports how many frames agree, and a summary is printed at exit. Output stays the --precision handle's. 0 = off");
@@ -712,12 +714,17 @@ static bool create_engines(int num_gpu, int per_gpu, int precision, std::vector<
         engines.push_back(e);
     }
     if (load_weights(engines[0], Fi("start_device"))) return false;
-    if (Fb("calibrate_range") && (precision == PE_PREC_F16X2 || precision == PE_PREC_F16X1 || precision == PE_PREC_E4M3X1)) {   // before the weights are replicated: the scales travel inside the packed buffer
+    const bool calibrate = Fb("calibrate_range") && (precision == PE_PREC_F16X2 || precision == PE_PREC_F16X1 || precision == PE_PREC_E4M3X1 ||
+                                                     precision == PE_PREC_S8X1);
+    auto calibrate_engine = [&](pe_engine* e, int dev) {
         std::vector<uint8_t> probe;
         synthetic_frame(0, global.disp_w, global.disp_h, probe);
         const uint8_t* ptr = probe.data();
-        if (pe_calibrate(engines[0], &ptr, 1)) { LOG_ERROR("GPU %d: range calibration failed: %s", Fi("start_device"), pe_last_error(engines[0])); return false; }
-    }
+        if (pe_calibrate(e, &ptr, 1)) { LOG_ERROR("GPU %d: range calibration failed: %s", dev, pe_last_error(e)); return false; }
+        return true;
+    };
+    // before the weights are replicated: the scales travel inside the packed buffer
+    if (calibrate && !calibrate_engine(engines[0], Fi("start_device"))) return false;
     if (num_gpu > 1) {
         std::vector<pe_engine*> firsts;
         for (int g = 0; g < num_gpu; g++) firsts.push_back(engines[g * per_gpu]);
@@ -726,8 +733,10 @@ static bool create_engines(int num_gpu, int per_gpu, int precision, std::vector<
                      pe_packed_weights_bytes(engines[0]) / 1e6);
         } else {
             LOG_ERROR("weight broadcast unavailable (%s); every GPU loads the model itself", pe_last_error(engines[0]));
-            for (int g = 1; g < num_gpu; g++)
+            for (int g = 1; g < num_gpu; g++) {
                 if (load_weights(engines[g * per_gpu], Fi("start_device") + g)) return false;
+                if (calibrate && precision == PE_PREC_S8X1 && !calibrate_engine(engines[g * per_gpu], Fi("start_device") + g)) return false;
+            }
         }
     }
     for (int g = 0; g < num_gpu; g++)
@@ -1108,6 +1117,10 @@ int main(int argc, char** argv) {
     }
     if (F("frame_format") != "jpg" && F("frame_format") != "bmp") { LOG_ERROR("--frame_format must be jpg or bmp"); return 1; }
     if (Fi("audit_every") < 0) { LOG_ERROR("--audit_every must be 0 (off) or a positive number of batches"); return 1; }
+    if (Fi("precision") == PE_PREC_S8X1 && !Fb("calibrate_range")) {
+        LOG_ERROR("--precision 6 (INT8) runs on calibrated per-layer range scales: at scale 1 almost every activation quantises to 0; drop --nocalibrate_range");
+        return 1;
+    }
     if (Fi("audit_every") > 0 && Fi("precision") == PE_PREC_F16X2) {
         LOG_ERROR("--audit_every compares a faster precision with the parity mode; with --precision 2 there is nothing to compare");
         return 1;

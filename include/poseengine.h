@@ -22,7 +22,7 @@ extern "C" {
 #define PE_ERR_CUDA 2      /* CUDA runtime / driver failure (message in pe_last_error) */
 #define PE_ERR_STATE 3     /* call out of order (e.g. forward before weights) */
 #define PE_ERR_IO 4        /* file could not be read / parsed */
-#define PE_ERR_RANGE 5     /* fp16 modes: a layer's values left the range of the fp16 planes (see pe_calibrate) */
+#define PE_ERR_RANGE 5     /* fp16 / e4m3 / s8 modes: a layer's values left the range of its planes (see pe_calibrate) */
 
 #define PE_MODEL_MPI_15 0  /* ModelDescriptorFactory::Type::MPI_15  (modelDescriptorFactory.h:16-19) */
 #define PE_MODEL_COCO_18 1 /* ModelDescriptorFactory::Type::COCO_18 */
@@ -50,6 +50,18 @@ extern "C" {
                              * conv1_1 keeps mode 4's fp16 input.  Needs pe_calibrate: an uncalibrated engine runs at scale 1,
                              * and pe_range_status reports PE_ERR_RANGE for a layer outside e4m3's range.  DESIGN.md sections
                              * 3-6; pe_compare_results / --audit_every measure what it does to the poses. */
+#define PE_PREC_S8X1 6      /* wgmma INT8 mode: one s8 plane of activations and weights, 1 s8 MMA per MAC (wgmma k32 s8 -> s32, the
+                             * FP8 rate), exact integer accumulation over the whole K.  Activations are q = sat(rint(x * 2^k)) in
+                             * [-128, 127] with a power-of-two scale 2^k per conv output (the net input at k = 8: q = p - 128);
+                             * zero padding is the integer 0.  Weights are quantised per output channel after the range ratios
+                             * are folded in: sigma_c = max|w| / 127, q = clamp(rint(w / sigma_c), -127, 127).  Epilogue per
+                             * channel, in fp32 without FMA: t = acc * f_c + b'_c with f_c = sigma_c * 2^(k_out - k_in),
+                             * b'_c = b_c * 2^k_out, ReLU, then cvt.rni.sat.s8 (the fp32 maps: k_out = 0, t stored).  So every
+                             * layer is a deterministic function of integers and a few fp32 operations.  A layer whose K = k*k*Cin
+                             * (padded) exceeds 132104 could overflow s32 and is refused (PE_ERR_INVALID).  Needs pe_calibrate
+                             * (it puts each layer's largest stored value in [32, 64)): a forward before it is PE_ERR_STATE.
+                             * pe_range_status reports the largest stored value / 127 and PE_ERR_RANGE when a layer reaches 127
+                             * (saturates) or stays below 4.  DESIGN.md section 6. */
 
 #define PE_MAX_PEOPLE 96   /* RENDER_MAX_PEOPLE, renderFunctions.h:6 / rtpose.cpp:88 */
 
@@ -104,7 +116,9 @@ int pe_caffemodel_blob(const pe_caffemodel* m, int layer, int blob, const float*
 const char* pe_caffemodel_last_error(void);
 /* pack + upload; must be called once after the weights are set and before any forward */
 int pe_commit_weights(pe_engine* e);
-/* Range management of the fp16 modes (PE_PREC_F16X2, PE_PREC_F16X1; a no-op in the others).  Their activation planes are fp16 x
+/* Range management of the fp16 modes (PE_PREC_F16X2, PE_PREC_F16X1), and of the e4m3 and s8 modes (PE_PREC_E4M3X1,
+ * PE_PREC_S8X1: stored maxima in [64, 128) and [32, 64), largest values 448 and 127; PE_PREC_S8X1 refuses to forward before
+ * pe_calibrate); a no-op in the others.  Their activation planes are fp16 x
  * power-of-two scale per layer; the default
  * scale 1 suits the trained pose models.  pe_calibrate runs one forward on the given HOST frames layer by layer, measures every
  * layer's largest |output| in fp32 and sets the scales so that the stored maxima sit in [32, 64) - after that a net of any
@@ -195,6 +209,8 @@ int pe_pixels_to_bgr(const pe_pixel_format* fmt, const void* frame, uint8_t* bgr
 /* HOST net input as the reference uploads it: n x num_scales x 3 x net_h x net_w fp32 planar
  * (frame.data, rtpose.cpp:1131-1133) */
 int pe_forward_net_input(pe_engine* e, const float* net_input, int n);
+/* (PE_PREC_S8X1 quantises this input like any activation, at scale 2^8: q = sat(rint(x * 256)) in [-128, 127], so values that
+ * are not multiples of 1/256 inside [-0.5, 0.496] - the frame path's p/256 - 0.5 - are rounded or saturated.) */
 /* test hook at the concat_stage7 boundary: HOST stride-8 maps n x num_scales x C x net_h/8 x net_w/8;
  * runs resize + NMS + connectLimbs* only (SURVEY.md section 8d "map injection") */
 int pe_forward_maps(pe_engine* e, const float* maps8, int n);
@@ -210,6 +226,10 @@ int pe_fetch_maps(pe_engine* e, float* maps8, int n);
  * nets: conv5_5_CPM_L1/_L2, Mconv7_stage2_* and Mconv7_stage3_*) are overwritten by every forward: PE_ERR_STATE, and
  * pe_last_error names the layer that reuses the buffer. */
 int pe_fetch_blob(pe_engine* e, const char* blob_name, float* out, size_t cap, int* c, int* h, int* w);
+/* test hook: *k such that the blob's stored values are its true values (pe_fetch_blob) times 2^k - the range scale of its
+ * producer, 8 for the net input of PE_PREC_S8X1.  So pe_fetch_blob x 2^k rebuilds the integers an s8 layer read.  Any mode with
+ * range scales (PE_PREC_F16X2, F16X1, E4M3X1, S8X1) answers it; the others give PE_ERR_INVALID, as does an unknown blob. */
+int pe_blob_log2_scale(pe_engine* e, const char* blob_name, int* k);
 /* block until the engine's stream is idle */
 int pe_sync(pe_engine* e);
 

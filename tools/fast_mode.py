@@ -1,9 +1,10 @@
 #!/usr/bin/env python3
-"""Speed and accuracy of the fast modes (PE_PREC_F16X1, PE_PREC_E4M3X1) against the parity mode (F16X2) and bf16x1, in one run
+"""Speed and accuracy of the fast modes (PE_PREC_F16X1, PE_PREC_E4M3X1, PE_PREC_S8X1) against the parity mode (F16X2) and bf16x1, in one run
 on one GPU.
 
 Workload C2 of bench.py: COCO 656x368, one scale, 9 frames per forward, the bench's seeded 720p frames (synth.make_frame(i)),
-W-he weights (E4M3X1 calibrated with pe_calibrate on frame 0: e4m3 has no room for an uncalibrated net).  Per mode, alternating the modes over FM_ROUNDS rounds:
+W-he weights (E4M3X1 and S8X1 calibrated with pe_calibrate on frame 0: e4m3 has no room for an uncalibrated net, and s8
+refuses to run one).  Per mode, alternating the modes over FM_ROUNDS rounds:
   * resident: frames/s of FM_STEPS forwards from device memory over two handles (CUDA events, as bench.py);
   * e2e: frames/s through forward_frames + fetch of every frame (host clock, as bench.py);
   * conv ms per layer class of one 9-frame step (pe_profile_layers, classes of tools/layer_times.py, median of 5).
@@ -29,10 +30,11 @@ from caffe_rtpose_b200 import engine, synth  # noqa: E402
 from layer_times import klass  # noqa: E402
 
 MODEL, NET_W, NET_H, DISP_W, DISP_H, B = engine.COCO_18, 656, 368, 1280, 720, 9
-MODES = {"f16x2": engine.PREC_F16X2, "f16x1": engine.PREC_F16X1, "e4m3x1": engine.PREC_E4M3X1, "bf16x1": engine.PREC_BF16X1}
+MODES = {"f16x2": engine.PREC_F16X2, "f16x1": engine.PREC_F16X1, "e4m3x1": engine.PREC_E4M3X1, "s8x1": engine.PREC_S8X1,
+         "bf16x1": engine.PREC_BF16X1}
 # FM_MODES: a comma-separated subset; the parity mode always runs, since every other mode is compared with it
 MODES = {m: p for m, p in MODES.items() if m == "f16x2" or m in os.environ.get("FM_MODES", ",".join(MODES)).split(",")}
-CALIBRATED = ("e4m3x1",)
+CALIBRATED = ("e4m3x1", "s8x1")
 TOL_PX = 1e-3 * max(DISP_W / NET_W, DISP_H / NET_H)
 
 
@@ -146,13 +148,13 @@ def main():
     Wc = synth.make_weights(MODEL, "caffe")
     batch = [host[lb * B + k] for k in range(B)]
     filler = {}
-    for m in ("f16x2", "f16x1", "e4m3x1"):
+    for m in ("f16x2", "f16x1", "e4m3x1", "s8x1"):
         if m in MODES:
             e = make_engines(MODES[m], Wc, n=1, calibrate=[host[0]])[0]
             e.forward_frames(batch)
             filler[m] = results(e)
             e.close()
-    for m in ("f16x1", "e4m3x1"):
+    for m in ("f16x1", "e4m3x1", "s8x1"):
         if m in MODES:
             out[m]["vs_parity_filler_net"] = compare(filler[m], filler["f16x2"])
     print(json.dumps({"card": info, "workload": "C2 COCO 656x368, 9 frames per forward, W-he", "steps": steps, "rounds": rounds,
