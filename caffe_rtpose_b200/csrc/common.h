@@ -24,10 +24,9 @@ namespace pe {
 // That holds only while pad <= gap: a larger pad reaches into the previous / next row or image.  So the
 // plan sets each level's gap to max(1, largest pad of a convolution at that level) (NetPlan::gap; 1, 1, 1, 3
 // for the built-in graphs, whose VGG levels run 3x3 and whose stride-8 stages run 7x7).
-// Channel pitch: every activation's channel count is padded to the conv kernel's K block - 16 channels for the fp32 SIMT
-// kernel, 64 for 16-bit planes (128 bytes), 128 for e4m3 (128 bytes; conv_tc_kernel.cuh explains the choice).  TMA needs
-// global strides that are multiples of 16 bytes, so an e4m3 pitch must be a multiple of 16 channels in any case; 128 is
-// stricter.  The im2col'ed net input stays at 64 fp16 channels in every tensor-core mode.
+// Channel pitch: every activation's channel count is padded to the conv kernel's K block, the mode's act_cpad (precision.h;
+// conv_tc_kernel.cuh explains the 128-byte block).  TMA needs global strides that are multiples of 16 bytes, which that
+// padding covers.  The im2col'ed net input has a pitch of its own, the mode's kp_input.
 // ---------------------------------------------------------------------------------------------
 struct Geo {
     int W, H, gap, Wp, Hs, N;
@@ -85,12 +84,12 @@ struct NetPlan {
 };
 struct NetDef;
 // plan from a parsed prototxt / built-in definition; -1 and a message when the graph is outside the supported family
-// slot_align: channel granularity of the Concat slots, 16 bytes of the element (8 for fp32 / 16-bit, 16 for e4m3), so that
-// the copy of the shared slot moves whole 16-byte chunks without touching the next slot
+// slot_align: channel granularity of the Concat slots, so that the copy of the shared slot moves whole 16-byte chunks without
+// touching the next slot
 int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& out, std::string& err, int slot_align);
 int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& out, std::string& err);   // slot_align 8
-// kp_input: channel pitch of the im2col'ed network input (27 -> 32 for SIMT, 64 for the tensor cores)
-// cpad: channel granularity of every activation (16 SIMT / 64 tensor cores)
+// kp_input: channel pitch of the im2col'ed network input; cpad: channel granularity of every activation.  The engine passes
+// the mode's kp_input, act_cpad and slot_align (precision.h).
 NetPlan build_plan(int model, int kp_input, int cpad, int slot_align = 8);
 
 // ---------------------------------------------------------------------------------------------

@@ -7,24 +7,9 @@
 
 namespace pe {
 
-template <int BN>
-static int launch_e4m3_bn(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap) {
-    const PlaneFmt f = l.d.fmt;
-    if (f.planes != 1) return -1;
-    if (f.e4m3()) return launch_inst<BN, 1, ELEM_E4M3, ELEM_E4M3>(l, a, grid, st, bmap);
-    if (f.f16() && l.d.out_e4m3) return launch_inst<BN, 1, ELEM_F16, ELEM_E4M3>(l, a, grid, st, bmap);
-    return -1;
-}
-
 int launch_e4m3(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap, int bn) {
-    switch (bn) {
-        case 128: return launch_e4m3_bn<128>(l, a, grid, st, bmap);
-        case 64: return launch_e4m3_bn<64>(l, a, grid, st, bmap);
-        case 48: return launch_e4m3_bn<48>(l, a, grid, st, bmap);
-        case 32: return launch_e4m3_bn<32>(l, a, grid, st, bmap);
-        case 16: return launch_e4m3_bn<16>(l, a, grid, st, bmap);
-        default: return -1;
-    }
+    return l.d.fmt.f16() ? launch_widths<1, ELEM_F16, ELEM_E4M3>(l, a, grid, st, bmap, bn)
+                         : launch_widths<1, ELEM_E4M3, ELEM_E4M3>(l, a, grid, st, bmap, bn);
 }
 
 }  // namespace pe

@@ -4,27 +4,13 @@
 // sums are exact, so nothing is chunked), and the per-channel epilogue
 //   t = __fadd_rn(__fmul_rn(__int2float_rn(acc), f_c), b'_c),  ReLU,  cvt.rni.sat.s8.f32
 // (the fp32 maps store t).  Every layer, conv1_1 included, reads s8: the im2col'ed net input is p - 128 at scale 2^8.
-// |acc| <= 128 * 127 * K, which the engine keeps inside s32 by refusing K > 132104 (engine.cu, S8_MAX_K).
+// |acc| <= 128 * 127 * K, which the engine keeps inside s32 by refusing a K above Precision::max_k (precision.h).
 #include "conv_tc_kernel.cuh"
 
 namespace pe {
 
-template <int BN>
-static int launch_s8_bn(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap) {
-    const PlaneFmt f = l.d.fmt;
-    if (f.planes != 1 || !f.s8()) return -1;
-    return launch_inst<BN, 1, ELEM_S8, ELEM_S8>(l, a, grid, st, bmap);
-}
-
 int launch_s8(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap, int bn) {
-    switch (bn) {
-        case 128: return launch_s8_bn<128>(l, a, grid, st, bmap);
-        case 64: return launch_s8_bn<64>(l, a, grid, st, bmap);
-        case 48: return launch_s8_bn<48>(l, a, grid, st, bmap);
-        case 32: return launch_s8_bn<32>(l, a, grid, st, bmap);
-        case 16: return launch_s8_bn<16>(l, a, grid, st, bmap);
-        default: return -1;
-    }
+    return launch_widths<1, ELEM_S8, ELEM_S8>(l, a, grid, st, bmap, bn);
 }
 
 }  // namespace pe

@@ -19,12 +19,11 @@
 //   * Two consumer warpgroups (64 rows each) issue wgmma.mma_async m64nBNk16 from shared-memory descriptors,
 //     accumulators in registers, fp32, with one wgmma group of K steps in flight behind the one being issued.
 //   * Split precision: activations and weights are stored as P 16-bit "planes" whose sum is the fp32 value
-//     (hi / lo); the kernel issues the cross products with pa + pb < P on the tensor core.  The format (kernels.h,
-//     PlaneFmt): P=2 fp16 = parity mode, ~1e-5 over the whole net (DESIGN.md section 3); P=1 fp16 = fast mode, the
-//     parity mode's hi plane alone (one MMA per MAC); P=1 bf16 and P=3 bf16 are kept for A/B comparisons.
-//     hi*hi goes to its own accumulator, cut into chunks of a few hundred K that are added in registers with
-//     round-to-nearest (the tensor core's fp32 accumulation truncates, so a long chain drifts); the cross terms
-//     are 2^-11 smaller and run over the whole tile in a second accumulator.  bf16x1 keeps one unchunked chain.
+//     (hi / lo); the kernel issues the cross products with pa + pb < P on the tensor core.  Each mode's format and
+//     accumulation are a row of the precision table (precision.h; DESIGN.md section 3).  In the chunked modes hi*hi goes
+//     to its own accumulator, cut into chunks of a few hundred K that are added in registers with round-to-nearest (the
+//     tensor core's fp32 accumulation truncates, so a long chain drifts); the cross terms are 2^-11 smaller and run over
+//     the whole tile in a second accumulator.
 //   * Epilogue: sum, bias, ReLU, re-split into planes and store NHWC planes (channel-slice stores implement
 //     Concat), or - for the last stage - the planar fp32 concat_stage7 blob.
 #include <cuda.h>
@@ -72,27 +71,14 @@ int tc_cout_pad(int cout) {
 // Three planes (bf16x3, kept for A/B comparisons) stay at 64.
 static int tc_bn(int cout_pad, int planes) { return std::min(cout_pad, planes == 3 ? 64 : 128); }
 
-template <int BN>
-static int launch_bn(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap) {
-    const PlaneFmt f = l.d.fmt;
-    if (f.e4m3() || l.d.out_e4m3) return launch_e4m3(l, a, grid, st, bmap, BN);   // conv_fp8.cu
-    if (f.s8()) return launch_s8(l, a, grid, st, bmap, BN);                        // conv_s8.cu
-    if (f.planes == 1) return f.f16() ? launch_inst<BN, 1, ELEM_F16, ELEM_F16>(l, a, grid, st, bmap)
-                                      : launch_inst<BN, 1, ELEM_BF16, ELEM_BF16>(l, a, grid, st, bmap);
-    if (f.planes == 2 && f.f16()) return launch_inst<BN, 2, ELEM_F16, ELEM_F16>(l, a, grid, st, bmap);
-    if constexpr (BN <= 64) { if (f.planes == 3 && !f.f16()) return launch_inst<BN, 3, ELEM_BF16, ELEM_BF16>(l, a, grid, st, bmap); }
-    return -1;   // no kernel for this tile width and plane format (tc_bn never picks one)
-}
-
-// box {one channel block = 128 bytes, b1, b2}; the 16-bit kinds share one 2-byte data type, e4m3 and s8 one 1-byte type (TMA
-// only moves the bytes)
+// box {one channel block = 128 bytes, b1, b2}; TMA only moves the bytes, so the data type is any of the element's size
 static int encode(EncodeTiledFn enc, CUtensorMap* map, PlaneElem elem, const void* base, cuuint64_t d0, cuuint64_t d1, cuuint64_t d2,
                   cuuint64_t s1, cuuint64_t s2, cuuint32_t b1, cuuint32_t b2, CUtensorMapL2promotion l2) {
     cuuint64_t dims[3] = {d0, d1, d2};
     cuuint64_t strides[2] = {s1, s2};
     cuuint32_t box[3] = {(cuuint32_t)tc_block_ch(elem), b1, b2};
     cuuint32_t es[3] = {1, 1, 1};
-    return (int)enc(map, elem == ELEM_E4M3 || elem == ELEM_S8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, (void*)base, dims,
+    return (int)enc(map, elem_size(elem) == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, (void*)base, dims,
                     strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, l2, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
@@ -140,11 +126,11 @@ int tc_layer_launch(const TcLayer& l, int nimg, cudaStream_t st, int share) {
     a.ksize = d.ksize; a.pad = d.pad; a.kblocks_per_tap = d.in_cused / tc_block_ch(d.fmt.elem); a.cin_k = d.in_cused;
     a.W = d.geo.W; a.H = d.geo.H; a.Wp = d.geo.Wp; a.Hs = d.geo.Hs;
     a.M = (long long)nimg * d.geo.Hs * d.geo.Wp;
-    // hi*hi accumulation chunk with split planes and in the fp16 fast mode: one 7-tap filter row (448 K), two 3-tap rows (384 K)
-    // or four 1x1 blocks (256 K); e4m3 the same K steps of 128 channels (896, 768, 512 K: DESIGN.md section 6); bf16x1 runs one
-    // chain over the whole K, and so does s8, whose integer sums are exact
+    // hi*hi accumulation chunk of the chunked modes: one 7-tap filter row (448 K in 16 bits), two 3-tap rows (384 K) or four 1x1
+    // blocks (256 K); e4m3 the same K steps of 128 channels (896, 768, 512 K: DESIGN.md section 6).  The others run one chain
+    // over the whole K.
     const int nk = d.ksize * d.ksize * a.kblocks_per_tap;
-    a.chunk_iters = (d.fmt.planes >= 2 || d.fmt.f16() || d.fmt.e4m3()) ? (d.ksize >= 7 ? 7 : (d.ksize >= 3 ? 6 : 4)) : nk;
+    a.chunk_iters = d.chunked ? (d.ksize >= 7 ? 7 : (d.ksize >= 3 ? 6 : 4)) : nk;
     static int nsm = 0;
     if (!nsm) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev); }
     // Tile width: the full width is the efficient shape (the A tile is re-read per N tile), but a single frame at the
@@ -162,13 +148,13 @@ int tc_layer_launch(const TcLayer& l, int nimg, cudaStream_t st, int share) {
     a.tiles_img = ((d.geo.H - 1) * d.geo.Wp + d.geo.W + TC_BM - 1) / TC_BM;
     const long long tiles = ((long long)nimg * a.tiles_img + TC_CLUSTER - 1) / TC_CLUSTER * TC_CLUSTER;
     const dim3 grid((unsigned)tiles, (unsigned)(d.cout_pad / bn), 1);
-    switch (bn) {
-        case 128: return launch_bn<128>(l, a, grid, st, bmap);
-        case 64: return launch_bn<64>(l, a, grid, st, bmap);
-        case 48: return launch_bn<48>(l, a, grid, st, bmap);
-        case 32: return launch_bn<32>(l, a, grid, st, bmap);
-        default: return launch_bn<16>(l, a, grid, st, bmap);
-    }
+    const PlaneFmt f = d.fmt;
+    if (d.out_elem == ELEM_E4M3) return launch_e4m3(l, a, grid, st, bmap, bn);   // conv_fp8.cu
+    if (d.out_elem == ELEM_S8) return launch_s8(l, a, grid, st, bmap, bn);       // conv_s8.cu
+    if (f.planes == 3) return launch_widths<3, ELEM_BF16, ELEM_BF16>(l, a, grid, st, bmap, bn);
+    if (f.planes == 2) return launch_widths<2, ELEM_F16, ELEM_F16>(l, a, grid, st, bmap, bn);
+    return f.f16() ? launch_widths<1, ELEM_F16, ELEM_F16>(l, a, grid, st, bmap, bn)
+                   : launch_widths<1, ELEM_BF16, ELEM_BF16>(l, a, grid, st, bmap, bn);
 }
 
 }  // namespace pe

@@ -12,12 +12,13 @@ struct TcLayerDesc {
     const void* w;                                                // planes [P][cout_pad][K] of fmt's element kind
     const float* bias;
     int cout, cout_pad, ksize, pad, relu;
-    PlaneFmt fmt;                                                 // plane count and element kind of in and w (kernels.h)
-    bool out_e4m3 = false;                                        // out holds e4m3 (with fmt fp16: conv1_1 of PE_PREC_E4M3X1)
+    PlaneFmt fmt;                                                 // plane count and element kind of in and w (precision.h)
+    PlaneElem out_elem;                                           // element kind of out (conv1_1 of E4M3X1: fp16 in, e4m3 out)
+    bool chunked;                                                 // the mode's hi*hi accumulation (Precision::chunked)
     const float* out_scale = nullptr;                             // device: epilogue factor 2^-k (weights packed with 2^k)
     unsigned* range = nullptr;                                    // device: running max |stored value| (float bits), or null
     Geo geo;                                                      // geo.N = max images
-    void* out; int out_pitch, out_coff; long long out_plane;      // planes (e4m3 when fmt or out_e4m3 says so), or
+    void* out; int out_pitch, out_coff; long long out_plane;      // fmt.planes planes of out_elem, or
     float* planar; int planar_C, planar_coff;                     // final fp32 maps (N, planar_C, H, W)
 };
 struct TcLayer {

@@ -115,91 +115,12 @@ __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.s
 __device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 __device__ __forceinline__ void wg_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 
-// D(64 x N, fp32 registers) (+)= A(64 x 16) * B(N x 16)^T, both K-major in shared memory; scale_d = 0 overwrites D.
-// Register j of a thread holds row 16*(warp%4) + lane/4 + 8*((j/2)%2), column 8*(j/4) + 2*(lane%4) + j%2.
-template <int N> struct Wgmma;
-template <> struct Wgmma<16> {
-    template <bool F16> __device__ __forceinline__ static void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
-        if (F16) asm volatile(
-            "{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
-            "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-            : "l"(da), "l"(db), "r"(scale_d));
-        else asm volatile(
-            "{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
-            "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-            : "l"(da), "l"(db), "r"(scale_d));
-    }
-};
-template <> struct Wgmma<32> {
-    template <bool F16> __device__ __forceinline__ static void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
-        if (F16) asm volatile(
-            "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
-            "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-            : "l"(da), "l"(db), "r"(scale_d));
-        else asm volatile(
-            "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
-            "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-            : "l"(da), "l"(db), "r"(scale_d));
-    }
-};
-template <> struct Wgmma<48> {
-    template <bool F16> __device__ __forceinline__ static void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
-        if (F16) asm volatile(
-            "{\n.reg .pred p;\nsetp.ne.b32 p, %26, 0;\n"
-            "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1, 0, 0;\n}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
-            : "l"(da), "l"(db), "r"(scale_d));
-        else asm volatile(
-            "{\n.reg .pred p;\nsetp.ne.b32 p, %26, 0;\n"
-            "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1, 0, 0;\n}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
-            : "l"(da), "l"(db), "r"(scale_d));
-    }
-};
-template <> struct Wgmma<64> {
-    template <bool F16> __device__ __forceinline__ static void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
-        if (F16) asm volatile(
-            "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
-            "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-            : "l"(da), "l"(db), "r"(scale_d));
-        else asm volatile(
-            "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
-            "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-            : "l"(da), "l"(db), "r"(scale_d));
-    }
-};
-template <> struct Wgmma<128> {
-    template <bool F16> __device__ __forceinline__ static void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
-        if (F16) asm volatile(
-            "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
-            "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-            : "l"(da), "l"(db), "r"(scale_d));
-        else asm volatile(
-            "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
-            "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-            : "l"(da), "l"(db), "r"(scale_d));
-    }
-};
-
-// D(64 x N, fp32) (+)= A(64 x 32) * B(N x 32)^T in e4m3, both K-major (the only layout FP8 wgmma takes, so no transpose
-// operands); the same register mapping.  32 e4m3 elements are 32 bytes: a K step advances the descriptors as k16 does in fp16.
-#define PE_WG_E4M3(N, NR, DA, DB, SD, REGS)                                                                                  \
-    template <> struct WgmmaE4M3<N> {                                                                                        \
-        __device__ __forceinline__ static void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {                   \
-            asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %" #SD ", 0;\n"                                                  \
-                         "wgmma.mma_async.sync.aligned.m64n" #N "k32.f32.e4m3.e4m3 {" REGS "}, %" #DA ", %" #DB ", p, 1, 1;\n}" \
-                         : PE_WG_OUT##NR : "l"(da), "l"(db), "r"(scale_d));                                                 \
-        }                                                                                                                    \
-    };
-template <int N> struct WgmmaE4M3;
+// D(64 x N) (+)= A(64 x K) * B(N x K)^T, both K-major in shared memory (the only layout the 8-bit kinds take, so no transpose
+// operands); scale_d = 0 overwrites D.  One K step is 32 bytes of the 128-byte swizzle rows: k16 in fp16 / bf16, k32 in e4m3 / s8.
+// Register j of a thread holds row 16*(warp%4) + lane/4 + 8*((j/2)%2), column 8*(j/4) + 2*(lane%4) + j%2.  s8 accumulates in
+// s32: the products and their sums are exact integers, so nothing is chunked while |acc| stays inside s32 (the engine bounds K,
+// Precision::max_k).
+template <int N, int ELEM> struct Wgmma;
 #define PE_WG_OUT8 "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
 #define PE_WG_OUT16 PE_WG_OUT8, "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
 #define PE_WG_OUT24 PE_WG_OUT16, "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
@@ -208,25 +129,6 @@ template <int N> struct WgmmaE4M3;
     "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]),  \
     "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),  \
     "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-PE_WG_E4M3(16, 8, 8, 9, 10, "%0,%1,%2,%3,%4,%5,%6,%7")
-PE_WG_E4M3(32, 16, 16, 17, 18, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15")
-PE_WG_E4M3(48, 24, 24, 25, 26, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23")
-PE_WG_E4M3(64, 32, 32, 33, 34, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31")
-PE_WG_E4M3(128, 64, 64, 65, 66, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
-                    "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63")
-
-// D(64 x N, s32) (+)= A(64 x 32) * B(N x 32)^T in s8, both K-major; the same register mapping and the same 32-byte K steps as
-// e4m3.  The products and their sums are exact integers: no chunking is needed while |acc| stays inside s32 (the engine
-// bounds K, conv_s8.cu).
-#define PE_WG_S8(N, NR, DA, DB, SD, REGS)                                                                                    \
-    template <> struct WgmmaS8<N> {                                                                                          \
-        __device__ __forceinline__ static void mma(int* d, uint64_t da, uint64_t db, uint32_t scale_d) {                     \
-            asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %" #SD ", 0;\n"                                                  \
-                         "wgmma.mma_async.sync.aligned.m64n" #N "k32.s32.s8.s8 {" REGS "}, %" #DA ", %" #DB ", p;\n}"          \
-                         : PE_WG_OUT##NR##_S32 : "l"(da), "l"(db), "r"(scale_d));                                           \
-        }                                                                                                                    \
-    };
-template <int N> struct WgmmaS8;
 #define PE_WG_OUT8_S32 "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7])
 #define PE_WG_OUT16_S32 PE_WG_OUT8_S32, "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
 #define PE_WG_OUT24_S32 PE_WG_OUT16_S32, "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23])
@@ -235,12 +137,33 @@ template <int N> struct WgmmaS8;
     "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]),      \
     "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]),      \
     "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
-PE_WG_S8(16, 8, 8, 9, 10, "%0,%1,%2,%3,%4,%5,%6,%7")
-PE_WG_S8(32, 16, 16, 17, 18, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15")
-PE_WG_S8(48, 24, 24, 25, 26, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23")
-PE_WG_S8(64, 32, 32, 33, 34, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31")
-PE_WG_S8(128, 64, 64, 65, 66, "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
-                  "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63")
+#define PE_WG_REGS8 "%0,%1,%2,%3,%4,%5,%6,%7"
+#define PE_WG_REGS16 PE_WG_REGS8 ",%8,%9,%10,%11,%12,%13,%14,%15"
+#define PE_WG_REGS24 PE_WG_REGS16 ",%16,%17,%18,%19,%20,%21,%22,%23"
+#define PE_WG_REGS32 PE_WG_REGS24 ",%24,%25,%26,%27,%28,%29,%30,%31"
+#define PE_WG_REGS64 PE_WG_REGS32 ",%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54," \
+    "%55,%56,%57,%58,%59,%60,%61,%62,%63"
+// Wgmma<N, ELEM>: NR accumulator registers, then operands %NR (A), %NR+1 (B), %NR+2 (scale_d).  K: the K step; TYPES: the
+// type suffix; ACC / OUT: the accumulator type and register list (PE_WG_OUTn##OUT); IMM: the immediates after the predicate.
+#define PE_WGMMA(N, NR, DA, DB, SD, ELEM, K, TYPES, ACC, OUT, IMM)                                                             \
+    template <> struct Wgmma<N, ELEM> {                                                                                         \
+        __device__ __forceinline__ static void mma(ACC* d, uint64_t da, uint64_t db, uint32_t scale_d) {                        \
+            asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %" #SD ", 0;\n"                                                     \
+                         "wgmma.mma_async.sync.aligned.m64n" #N "k" #K "." TYPES " {" PE_WG_REGS##NR "}, %" #DA ", %" #DB ", p" \
+                         IMM ";\n}"                                                                                             \
+                         : PE_WG_OUT##NR##OUT : "l"(da), "l"(db), "r"(scale_d));                                                \
+        }                                                                                                                       \
+    };
+#define PE_WGMMA_WIDTHS(ELEM, K, TYPES, ACC, OUT, IMM)          \
+    PE_WGMMA(16, 8, 8, 9, 10, ELEM, K, TYPES, ACC, OUT, IMM)    \
+    PE_WGMMA(32, 16, 16, 17, 18, ELEM, K, TYPES, ACC, OUT, IMM) \
+    PE_WGMMA(48, 24, 24, 25, 26, ELEM, K, TYPES, ACC, OUT, IMM) \
+    PE_WGMMA(64, 32, 32, 33, 34, ELEM, K, TYPES, ACC, OUT, IMM) \
+    PE_WGMMA(128, 64, 64, 65, 66, ELEM, K, TYPES, ACC, OUT, IMM)
+PE_WGMMA_WIDTHS(ELEM_F16, 16, "f32.f16.f16", float, , ", 1, 1, 0, 0")
+PE_WGMMA_WIDTHS(ELEM_BF16, 16, "f32.bf16.bf16", float, , ", 1, 1, 0, 0")
+PE_WGMMA_WIDTHS(ELEM_E4M3, 32, "f32.e4m3.e4m3", float, , ", 1, 1")
+PE_WGMMA_WIDTHS(ELEM_S8, 32, "s32.s8.s8", int, _S32, "")
 
 // fp32 -> s8, round to nearest even, saturating to [-128, 127] (cvt.rni.sat.s8.f32; NaN gives 0)
 __device__ __forceinline__ uint32_t f32_to_s8(float x) {
@@ -269,8 +192,8 @@ constexpr int TC_BK = 64;            // 16-bit elements per K block = one 128-by
 // stage inputs: 28 % fewer MACs in Mconv1), but it keeps the fp16 kernel's number of K steps - each step's mbarrier waits,
 // releases and descriptor arithmetic - while halving the tensor-core work per step, so the per-step overhead would eat the
 // gain everywhere else.  128-channel blocks keep every byte of the fp16 geometry (boxes, slots, descriptors, the 32-byte K
-// advance) and halve the steps.  The engine pads e4m3 and s8 activations to 128 channels (common.h).
-__host__ __device__ constexpr int tc_block_ch(int elem) { return elem == ELEM_E4M3 || elem == ELEM_S8 ? 128 : TC_BK; }
+// advance) and halve the steps.  The engine pads e4m3 and s8 activations to 128 channels (Precision::act_cpad).
+__host__ __device__ constexpr int tc_block_ch(PlaneElem elem) { return 128 / elem_size(elem); }
 constexpr int TC_WROWS = TC_BM + 8;  // rows of an A window: the tile plus the row shifts q = 1..8 of a filter row (k <= 9)
 constexpr int TC_KMAX = TC_WROWS - TC_BM + 1;
 constexpr int TC_THREADS = 384;      // warpgroup 0: TMA producer, warpgroups 1-2: consumers
@@ -338,7 +261,7 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int n0 = blockIdx.y * BN;
     const int ks = a.ksize, taps = ks * ks;
     const int num_k = taps * a.kblocks_per_tap;
-    constexpr int KB = tc_block_ch(ELEM);
+    constexpr int KB = tc_block_ch(PlaneElem(ELEM));
 
     if (threadIdx.x == 0) {
         // bempty: released by the 8 consumer warps of every CTA in the cluster, since each weight tile is written into all
@@ -418,9 +341,7 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             wg_fence();
 #pragma unroll
             for (int k = 0; k < 4; k++) {   // 32-byte K steps of the 128-byte rows: k16 in 16 bits, k32 in e4m3
-                if constexpr (S8) WgmmaS8<BN>::mma(acc_h, wg_desc(sa + k * 32), wg_desc(sb + k * 32), (k != 0) | h_acc);
-                else if constexpr (ELEM == ELEM_E4M3) WgmmaE4M3<BN>::mma(acc_h, wg_desc(sa + k * 32), wg_desc(sb + k * 32), (k != 0) | h_acc);
-                else Wgmma<BN>::template mma<ELEM == ELEM_F16>(acc_h, wg_desc(sa + k * 32), wg_desc(sb + k * 32), (k != 0) | h_acc);
+                Wgmma<BN, ELEM>::mma(acc_h, wg_desc(sa + k * 32), wg_desc(sb + k * 32), (k != 0) | h_acc);
                 if constexpr (PLANES > 1) {
 #pragma unroll
                     for (int pa = 0; pa < PLANES; pa++)
@@ -428,8 +349,8 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                         for (int pb = 0; pb < PLANES - pa; pb++) {
                             if (pa + pb == 0) continue;
                             const uint32_t first = it == 0 && k == 0 && pa + pb == 1 && pa == 0;
-                            Wgmma<BN>::template mma<ELEM == ELEM_F16>(acc_c, wg_desc(sa + pa * a_plane + k * 32),
-                                                         wg_desc(sb + pb * S::B_PLANE + k * 32), first ? 0u : 1u);
+                            Wgmma<BN, ELEM>::mma(acc_c, wg_desc(sa + pa * a_plane + k * 32), wg_desc(sb + pb * S::B_PLANE + k * 32),
+                                                 first ? 0u : 1u);
                         }
                 }
             }
@@ -525,9 +446,21 @@ static int launch_inst(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_
     return cudaLaunchKernelEx(&cfg, kern, maps[0], maps[bmap], a) == cudaSuccess ? 1 : -1;
 }
 
-// The e4m3 instances (conv_fp8.cu): layers of fmt e4m3, and fp16-input layers with out_e4m3; bn = the grid's tile width.
+// The instance <bn, PLANES, ELEM, OUT> for the grid's tile width bn.  Three planes run at BN <= 64 only (tc_bn).
+template <int PLANES, int ELEM, int OUT>
+static int launch_widths(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap, int bn) {
+    switch (bn) {
+        case 128: if constexpr (PLANES < 3) return launch_inst<128, PLANES, ELEM, OUT>(l, a, grid, st, bmap); else return -1;
+        case 64: return launch_inst<64, PLANES, ELEM, OUT>(l, a, grid, st, bmap);
+        case 48: return launch_inst<48, PLANES, ELEM, OUT>(l, a, grid, st, bmap);
+        case 32: return launch_inst<32, PLANES, ELEM, OUT>(l, a, grid, st, bmap);
+        case 16: return launch_inst<16, PLANES, ELEM, OUT>(l, a, grid, st, bmap);
+        default: return -1;
+    }
+}
+
+// Layers with e4m3 output (conv_fp8.cu) and s8 layers (conv_s8.cu): their instances live in translation units of their own.
 int launch_e4m3(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap, int bn);
-// The s8 instances (conv_s8.cu): layers of fmt s8.
 int launch_s8(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap, int bn);
 
 }  // namespace pe

@@ -16,6 +16,7 @@
 #include "common.h"
 #include "kernels.h"
 #include "conv_tc.h"
+#include "precision.h"
 #include "e4m3.h"
 #include "s8.h"
 #include "jpeg_coefs.h"
@@ -41,7 +42,7 @@ struct pe_engine {
     const ModelTables* mt = nullptr;
     ModelTables mt_own;     // model tables with the prototxt's nms max_peaks
     Geo geo[4];
-    PlaneFmt fmt = {0, ELEM_BF16};   // storage of activations and packed weights (kernels.h): 0 planes = fp32 SIMT
+    const Precision* prec = nullptr;   // the precision mode's row (precision.h)
     std::vector<void*> acts;        // device
     std::vector<long long> act_plane;  // elements per plane
     std::vector<HostWeights> hw;    // per conv
@@ -114,23 +115,15 @@ struct pe_engine {
 static void drop_graphs(pe_engine* e);
 static int setup_lanes(pe_engine* e);
 
-// Storage of activation i and of conv i's packed weights: the engine's format, except that E4M3X1 keeps the im2col'ed net input,
-// and so conv1_1's weights, in one fp16 plane (kernels.h)
+// Storage of activation i and of conv i's packed weights: the mode's format, except for the im2col'ed net input.  i = -1, the
+// planar fp32 maps, gets the mode's format, which picks the kernel instance of the last layers.
 static PlaneFmt act_fmt(const pe_engine* e, int i) {
-    return e->fmt.e4m3() && i == e->plan.input_act ? PlaneFmt{1, ELEM_F16} : e->fmt;
+    const PlaneFmt f = e->prec->fmt;
+    return i == e->plan.input_act ? PlaneFmt{f.planes, e->prec->input_elem} : f;
 }
 static PlaneFmt conv_wfmt(const pe_engine* e, int i) { return act_fmt(e, e->plan.convs[i].in_act); }
-// channel granularity of the activations (common.h): 16 (fp32 SIMT), 64 (16-bit planes), 128 (e4m3, s8: one K block, conv_tc_kernel.cuh)
-static bool one_byte(int precision) { return precision == PE_PREC_E4M3X1 || precision == PE_PREC_S8X1; }
-static int act_cpad(int precision) { return precision == PE_PREC_FP32_SIMT ? 16 : one_byte(precision) ? 128 : 64; }
-// Concat slot granularity (common.h, build_plan_from_net): 16 bytes of e4m3 / s8, 8 channels otherwise
-static int slot_align(int precision) { return one_byte(precision) ? 16 : 8; }
-// channel pitch of the im2col'ed net input: 32 fp32 (SIMT), 64 fp16 / bf16 (e4m3 keeps fp16), 128 s8 (one K block)
-static int kp_input(int precision) { return precision == PE_PREC_FP32_SIMT ? 32 : precision == PE_PREC_S8X1 ? 128 : 64; }
-// S8X1: |acc| <= 128 * 127 * K must stay inside s32, so K = taps x padded input channels is at most 132104 (conv_s8.cu)
-static const long long S8_MAX_K = 132104;
-// floats of conv i's epilogue fields in the packed buffer: bias[cout_pad], then the layer's factor (S8X1: a factor per channel)
-static size_t epi_floats(const pe_engine* e, int i) { return (size_t)e->cout_pad[i] + (e->fmt.s8() ? e->cout_pad[i] : 1); }
+// floats of conv i's epilogue fields in the packed buffer: bias[cout_pad], then the layer's factor or one factor per channel
+static size_t epi_floats(const pe_engine* e, int i) { return (size_t)e->cout_pad[i] + (e->prec->per_channel_epilogue ? e->cout_pad[i] : 1); }
 static size_t fmt_bytes(PlaneFmt f) { return (size_t)f.elem_bytes() * (f.planes ? f.planes : 1); }   // bytes per element, all planes
 
 static int fail(pe_engine* e, int code, const char* fmt, ...) {
@@ -316,12 +309,14 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
     *out = nullptr;
     pe_config cfg_copy = *cfg_in;
     pe_config* cfg = &cfg_copy;
+    if (cfg->precision < 0 || cfg->precision >= NUM_PRECISIONS) return fail(nullptr, PE_ERR_INVALID, "unknown precision %d", cfg->precision);
+    const Precision& prec = precision(cfg->precision);
     NetDef netdef;
     NetPlan proto_plan;
     if (prototxt_path) {
         std::string perr;
         if (parse_prototxt_file(prototxt_path, netdef, perr)) return fail(nullptr, PE_ERR_IO, "%s: %s", prototxt_path, perr.c_str());
-        if (build_plan_from_net(netdef, kp_input(cfg->precision), act_cpad(cfg->precision), proto_plan, perr, slot_align(cfg->precision)))
+        if (build_plan_from_net(netdef, prec.kp_input, prec.act_cpad, proto_plan, perr, prec.slot_align))
             return fail(nullptr, PE_ERR_INVALID, "%s: %s", prototxt_path, perr.c_str());
         if (cfg->model >= 0 && cfg->model != proto_plan.model)
             return fail(nullptr, PE_ERR_INVALID, "%s describes the %s model (nms num_parts %d), the configuration asks for model %d", prototxt_path,
@@ -335,7 +330,6 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
     if (cfg->max_batch < 1 || cfg->max_batch > 64) return fail(nullptr, PE_ERR_INVALID, "max_batch %d out of [1,64]", cfg->max_batch);
     if (check_resize_scales(nullptr, (float)cfg->start_scale, (float)cfg->scale_gap, cfg->num_scales)) return PE_ERR_INVALID;
     if (cfg->disp_w <= 0 || cfg->disp_h <= 0) return fail(nullptr, PE_ERR_INVALID, "bad display resolution");
-    if (cfg->precision < 0 || cfg->precision > PE_PREC_S8X1) return fail(nullptr, PE_ERR_INVALID, "unknown precision %d", cfg->precision);
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
         return fail(nullptr, PE_ERR_CUDA, "no CUDA device visible: the pose engine has no CPU fallback");
@@ -348,7 +342,7 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
     e->mt_own = model_tables(cfg->model);
     if (prototxt_path) e->mt_own.max_peaks = proto_plan.nms_max_peaks;   // nms_param.max_peaks (NmsLayer::GetMaxPeaks, rtpose.cpp:195)
     e->mt = &e->mt_own;
-    e->fmt = plane_fmt(cfg->precision);
+    e->prec = &prec;
     if (const char* g = getenv("PE_CHECK_RANGE")) e->check_range = atoi(g) != 0;
     e->start_scale_f = (float)cfg->start_scale;  // ImResizeLayer::SetStartScale(float)
     e->scale_gap_f = (float)cfg->scale_gap;
@@ -356,7 +350,7 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
 #define CKC(call) do { cudaError_t err_ = (call); if (err_ != cudaSuccess) { \
     fail(e, PE_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(err_), __FILE__, __LINE__); return bail(PE_ERR_CUDA); } } while (0)
     CKC(cudaSetDevice(cfg->device));
-    if (e->fmt.planes) {
+    if (prec.fmt.planes) {
         cudaDeviceProp prop;
         CKC(cudaGetDeviceProperties(&prop, cfg->device));
         if (prop.major != 9) { fail(e, PE_ERR_INVALID, "wgmma precision modes need sm_90 (found sm_%d%d)", prop.major, prop.minor); return bail(PE_ERR_INVALID); }
@@ -365,13 +359,13 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
     for (int i = 0; i < 16; i++) CKC(cudaEventCreate(&e->ev[i]));
 
     // the plan first: each level's gap is the largest pad of its convolutions (common.h)
-    e->plan = prototxt_path ? proto_plan : build_plan(cfg->model, kp_input(cfg->precision), act_cpad(cfg->precision), slot_align(cfg->precision));
-    if (e->fmt.s8())
+    e->plan = prototxt_path ? proto_plan : build_plan(cfg->model, prec.kp_input, prec.act_cpad, prec.slot_align);
+    if (prec.max_k)
         for (const ConvSpec& c : e->plan.convs) {
             const long long K = (long long)(c.im2col_input ? 1 : c.k * c.k) * c.in_cused;
-            if (K > S8_MAX_K) {
+            if (K > prec.max_k) {
                 fail(e, PE_ERR_INVALID, "layer %s: K = %lld (%dx%d taps x %d padded input channels) exceeds %lld, the largest K whose s8 sums "
-                     "stay inside s32 (|acc| <= 128 x 127 x K): PE_PREC_S8X1 cannot run it", c.name.c_str(), K, c.k, c.k, c.in_cused, S8_MAX_K);
+                     "stay inside s32 (|acc| <= 128 x 127 x K): PE_PREC_S8X1 cannot run it", c.name.c_str(), K, c.k, c.k, c.in_cused, prec.max_k);
                 return bail(PE_ERR_INVALID);
             }
         }
@@ -383,7 +377,7 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
     }
     if (e->geo[3].W * 8 != cfg->net_w || e->geo[3].H * 8 != cfg->net_h) { fail(e, PE_ERR_INVALID, "net size not divisible by 8 after pooling"); return bail(PE_ERR_INVALID); }
     e->hw.resize(e->plan.convs.size());
-    if (e->fmt.planes && setup_lanes(e)) return bail(PE_ERR_CUDA);
+    if (prec.fmt.planes && setup_lanes(e)) return bail(PE_ERR_CUDA);
     // FLOPs (SURVEY.md section 8d): 2*Cout*Cin*k^2*Hout*Wout per conv and image
     e->flops_per_scale = 0;
     for (auto& c : e->plan.convs) {
@@ -580,12 +574,12 @@ static size_t packed_layout(pe_engine* e) {
     for (size_t i = 0; i < nc; i++) {
         const ConvSpec& c = e->plan.convs[i];
         e->cin_pad[i] = c.in_cused;
-        e->cout_pad[i] = e->fmt.planes ? tc_cout_pad(c.cout) : (c.cout + 63) / 64 * 64;
+        e->cout_pad[i] = e->prec->fmt.planes ? tc_cout_pad(c.cout) : (c.cout + 63) / 64 * 64;
         const size_t K = (size_t)(c.im2col_input ? 1 : c.k * c.k) * e->cin_pad[i];
         e->w_off[i] = total;
         total = align256(total + K * e->cout_pad[i] * fmt_bytes(conv_wfmt(e, (int)i)));
         e->b_off[i] = total;
-        total = align256(total + epi_floats(e, (int)i) * 4);   // bias[cout_pad] + the layer's epilogue scale (S8X1: one per channel)
+        total = align256(total + epi_floats(e, (int)i) * 4);
     }
     return total;
 }
@@ -596,18 +590,17 @@ static size_t packed_layout(pe_engine* e) {
 //   acc = 2^k * s_ref * sum_ci w[ci] * a[ci]     and     stored = acc * out_scale + bias,  out_scale = s_out / (2^k * s_ref),
 // bias = true bias * s_out - all factors powers of two, hence exact, and ReLU commutes with them: range scaling is free at run time.
 // S8X1 replaces 2^k by a step per output channel (sigma_c, s8.h): acc * sigma_c ~ s_ref * sum w a, and the factor of channel c
-// is f_c = sigma_c * s_out / s_ref.  Its net input is stored as (p - 128) = (p/256 - 0.5) * 2^8: scale 256.
-static float net_input_scale(const pe_engine* e) { return e->fmt.s8() ? 256.f : 1.f; }
+// is f_c = sigma_c * s_out / s_ref.  The net input carries the mode's net_input_scale.
 static float input_ref_scale(const pe_engine* e, const ConvSpec& c) {
     for (int pc : c.cin_prod) if (pc >= 0) return e->conv_scale[pc];
-    return net_input_scale(e);   // the net input
+    return e->prec->net_input_scale;   // the net input
 }
 static void fill_epilogue_fields(const pe_engine* e, int i, float* B) {
     const ConvSpec& c = e->plan.convs[i];
     const float s_ref = input_ref_scale(e, c);
     const float s_out = c.out_act >= 0 ? e->conv_scale[i] : 1.f;   // the planar stride-8 maps are true values
     for (int co = 0; co < c.cout; co++) B[co] = e->bias_true[i][co] * s_out;
-    if (e->fmt.s8()) {
+    if (e->prec->per_channel_epilogue) {
         for (int co = 0; co < c.cout; co++) B[e->cout_pad[i] + co] = e->wsig[i][co] * (s_out / s_ref);
         return;
     }
@@ -654,16 +647,14 @@ static void pack_conv_weights(pe_engine* e, int i, uint8_t* dst) {
     } else {
         uint16_t* W = (uint16_t*)dst;
         const size_t plane = (size_t)cop * K;
-        // fp16 planes: scale the layer by 2^k so that max|w| lands in [2^13, 2^14) - small weights would otherwise
-        // put their lo plane into fp16 subnormals.  e4m3: into [128, 256), below the largest finite 448, so that
-        // weights down to max|w| * 2^-13 stay normal.  Exact (power of two); the epilogue multiplies by 2^-k.
+        // scale the layer by 2^k so that max|w| lands below 2^weight_top (precision.h).  Exact (power of two); the epilogue
+        // multiplies by 2^-k.
         float wscale = 1.f;
-        if (wf.f16() || wf.e4m3()) {
+        if (const int top = weight_top(wf.elem)) {
             float mx = 0.f;
             for (int co = 0; co < c.cout; co++)
                 for (size_t kk = 0; kk < K; kk++) mx = fmaxf(mx, fabsf(src(co, (int)kk)));
             int ex = 0;
-            const int top = wf.e4m3() ? 8 : 14;
             if (mx > 0.f && mx < 3e38f) { frexpf(mx, &ex); wscale = ldexpf(1.f, std::max(-100, std::min(100, top - ex))); }
         }
         wscale_inv = 1.f / wscale;
@@ -686,11 +677,11 @@ static void pack_conv_weights(pe_engine* e, int i, uint8_t* dst) {
 // per-layer launch state (TMA descriptors) over the packed buffer the handle currently points at
 static int bind_packed(pe_engine* e) {
     const size_t nc = e->plan.convs.size();
-    if (e->fmt.ranged() && !e->d_range) {
+    if (e->prec->ranged() && !e->d_range) {
         CK(e, cudaMalloc(&e->d_range, nc * sizeof(unsigned)));
         CK(e, cudaMemset(e->d_range, 0, nc * sizeof(unsigned)));
     }
-    if (e->fmt.planes) {
+    if (e->prec->fmt.planes) {
         for (auto& t : e->tc) tc_layer_destroy(t);
         e->tc.assign(nc, TcLayer());
         for (size_t i = 0; i < nc; i++) {
@@ -701,8 +692,8 @@ static int bind_packed(pe_engine* e) {
             d.w = (char*)e->d_packed + e->w_off[i]; d.bias = (const float*)((char*)e->d_packed + e->b_off[i]);
             d.cout = c.cout; d.cout_pad = e->cout_pad[i]; d.ksize = c.im2col_input ? 1 : c.k; d.pad = c.im2col_input ? 0 : c.pad;
             d.relu = c.relu; d.fmt = conv_wfmt(e, (int)i); d.geo = g; d.out_scale = d.bias + e->cout_pad[i];
-            d.out_e4m3 = e->fmt.e4m3();
-            d.range = (e->fmt.ranged() && e->d_range) ? e->d_range + i : nullptr;
+            d.out_elem = act_fmt(e, c.out_act).elem; d.chunked = e->prec->chunked;
+            d.range = (e->prec->ranged() && e->d_range) ? e->d_range + i : nullptr;
             if (c.out_act >= 0) {
                 d.out = e->acts[c.out_act]; d.out_pitch = e->plan.acts[c.out_act].C; d.out_coff = c.out_coff; d.out_plane = e->act_plane[c.out_act];
                 d.planar = nullptr; d.planar_C = 0; d.planar_coff = 0;
@@ -904,7 +895,7 @@ static int run_op(pe_engine* e, const OpRef& op, int nimg, cudaStream_t st = nul
         const ConvSpec& c = e->plan.convs[op.idx];
         const Geo& g = e->geo[c.level];
         const long long M = (long long)nimg * g.Hs * g.Wp;
-        if (e->fmt.planes) {
+        if (e->prec->fmt.planes) {
             const int n = tc_layer_launch(e->tc[op.idx], nimg, st, share);
             if (n < 0) return fail(e, PE_ERR_CUDA, "conv %s: tensor-core launch failed or no kernel fits the tile (%s)", c.name.c_str(), cudaGetErrorString(cudaGetLastError()));
             e->launches += n;
@@ -925,7 +916,7 @@ static int run_op(pe_engine* e, const OpRef& op, int nimg, cudaStream_t st = nul
         const Geo& gi = e->geo[p.level_in]; const Geo& go = e->geo[p.level_in + 1];
         PoolArgs a;
         a.in = e->acts[p.in_act]; a.out = e->acts[p.out_act]; a.C = e->plan.acts[p.in_act].C;
-        a.in_plane = e->act_plane[p.in_act]; a.out_plane = e->act_plane[p.out_act]; a.fmt = e->fmt;
+        a.in_plane = e->act_plane[p.in_act]; a.out_plane = e->act_plane[p.out_act]; a.fmt = e->prec->fmt;
         a.Wi = gi.W; a.Hi = gi.H; a.Wpi = gi.Wp; a.Hsi = gi.Hs; a.Wo = go.W; a.Ho = go.H; a.Wpo = go.Wp; a.Hso = go.Hs; a.N = nimg;
         e->launches += launch_pool(a, st);
     } else {
@@ -933,7 +924,7 @@ static int run_op(pe_engine* e, const OpRef& op, int nimg, cudaStream_t st = nul
         const Geo& g = e->geo[3];
         CopyArgs a;
         a.src = e->acts[c.src_act]; a.dst = e->acts[c.dst_act]; a.pitch = e->plan.acts[c.src_act].C; a.channels = c.channels;
-        a.elem_bytes = e->fmt.elem_bytes(); a.M = (long long)nimg * g.Hs * g.Wp; a.plane = e->act_plane[c.src_act]; a.fmt = e->fmt;
+        a.elem_bytes = e->prec->fmt.elem_bytes(); a.M = (long long)nimg * g.Hs * g.Wp; a.plane = e->act_plane[c.src_act]; a.fmt = e->prec->fmt;
         e->launches += launch_copy_channels(a, st);
     }
     return PE_OK;
@@ -1013,7 +1004,7 @@ static int setup_lanes(pe_engine* e) {
 static int run_net(pe_engine* e, int n) {
     if (!e->committed) return fail(e, PE_ERR_STATE, "pe_commit_weights has not been called");
     // at scale 1 almost every activation of a typical net quantises to 0
-    if (e->fmt.s8() && !e->calibrated)
+    if (e->prec->needs_calibration && !e->calibrated)
         return fail(e, PE_ERR_STATE, "PE_PREC_S8X1 runs on calibrated range scales: call pe_calibrate (on the handle that owns the weights) before the first forward");
     if (!e->use_graphs) return run_net_eager(e, n);
     pe_engine::GraphEntry& g = e->graphs[n];
@@ -1457,7 +1448,7 @@ extern "C" int pe_calibrate(pe_engine* e, const uint8_t* const* frames, int n) {
     int rc = check_n(e, n); if (rc) return rc;
     if (!frames) return fail(e, PE_ERR_INVALID, "null frames");
     if (!e->committed) return fail(e, PE_ERR_STATE, "pe_commit_weights has not been called");
-    if (!e->fmt.ranged()) return PE_OK;   // fp32 / bf16 modes have fp32's exponent range
+    if (!e->prec->ranged()) return PE_OK;   // fp32 / bf16 modes have fp32's exponent range
     const size_t nc = e->plan.convs.size();
     if (e->bias_true.size() != nc || e->bias_true[0].empty() || e->hw[0].w.empty())
         return fail(e, PE_ERR_STATE, "this handle received its weights by broadcast / sharing: calibrate the source handle before replicating");
@@ -1491,10 +1482,8 @@ extern "C" int pe_calibrate(pe_engine* e, const uint8_t* const* frames, int n) {
             CK(e, cudaMemcpyAsync(&bits, e->d_range + i, sizeof bits, cudaMemcpyDeviceToHost, e->stream));
             CK(e, cudaStreamSynchronize(e->stream));
             float m; memcpy(&m, &bits, 4);
-            // m * s in [32, 64) for fp16 (1000x headroom to 65504); in [64, 128) for e4m3 (3.5-7x headroom to 448, and values
-            // down to m * s * 2^-12 stay normal); in [32, 64) for s8: 6 bits, and 2-4x headroom to 127 for frames busier than
-            // the calibration frame
-            const int top = e->fmt.e4m3() ? 7 : 6;
+            // m * s in [2^(range_top-1), 2^range_top) (precision.h)
+            const int top = e->prec->range_top;
             if (m > 0.f && m < 3e38f) { int ex = 0; frexpf(m, &ex); e->conv_scale[i] = ldexpf(1.f, std::max(-100, std::min(100, top - ex))); }
         }
         if ((rc = upload_fields(e, i))) return rc;
@@ -1505,11 +1494,9 @@ extern "C" int pe_calibrate(pe_engine* e, const uint8_t* const* frames, int n) {
     return run_post_and_return(e, n);
 }
 
-// Largest |stored value| / the format's largest finite value (65504 for fp16, 448 for e4m3) over the conv layers since the last
-// call.  PE_ERR_RANGE when a layer reached that limit, or when a layer's maximum fell below a floor: fp16 2^-10 (its lo plane then
-// lives in fp16 subnormals and parity is lost); e4m3 2^-2, 16x above the smallest normal 2^-6, so that values a sixteenth of
-// the maximum - the bulk of a layer's outputs - are still normal.  s8: the largest stored value rint(max |t|) / 127; PE_ERR_RANGE
-// when it reaches 127 (the layer saturates) or stays below 4 (under 3 bits).  *layer64 names the worst layer.
+// Largest |stored value| / the mode's range_limit (precision.h) over the conv layers since the last call.  PE_ERR_RANGE when a
+// layer reached that limit, or when a layer's maximum fell below the mode's range_floor.  s8: the largest stored value is
+// rint(max |t|).  *layer64 names the worst layer.
 extern "C" int pe_range_status(pe_engine* e, float* worst_ratio, char* layer64) {
     if (!e) return PE_ERR_INVALID;
     if (worst_ratio) *worst_ratio = 0.f;
@@ -1521,9 +1508,8 @@ extern "C" int pe_range_status(pe_engine* e, float* worst_ratio, char* layer64) 
     std::vector<unsigned> bits(nc);
     CK(e, cudaMemcpy(bits.data(), e->d_range, nc * sizeof(unsigned), cudaMemcpyDeviceToHost));
     CK(e, cudaMemset(e->d_range, 0, nc * sizeof(unsigned)));
-    const bool e4 = e->fmt.e4m3(), s8 = e->fmt.s8();
-    const float limit = e4 ? 448.f : s8 ? 127.f : 65504.f, floor_ = e4 ? 0.25f : s8 ? 4.f : 9.765625e-4f;
-    const char* what = e4 ? "the e4m3 planes" : s8 ? "the s8 planes" : "the fp16 planes";
+    const Precision& p = *e->prec;
+    const bool s8 = p.fmt.s8();
     float worst = 0.f, smallest = 3e38f;
     int iw = -1, is = -1;
     for (size_t i = 0; i < nc; i++) {
@@ -1531,19 +1517,19 @@ extern "C" int pe_range_status(pe_engine* e, float* worst_ratio, char* layer64) 
         float m; memcpy(&m, &bits[i], 4);
         if (bits[i] == 0) continue;                   // layer did not run since the last call
         if (s8 && m <= 3e38f) m = rintf(m);           // the kernels track |t| before the rounding: the stored value
-        if (!(m <= 3e38f) || m / limit > worst) { worst = (m <= 3e38f) ? m / limit : 2.f; iw = (int)i; }
+        if (!(m <= 3e38f) || m / p.range_limit > worst) { worst = (m <= 3e38f) ? m / p.range_limit : 2.f; iw = (int)i; }
         if (m < smallest) { smallest = m; is = (int)i; }
     }
     if (worst_ratio) *worst_ratio = worst;
     if (worst >= 1.f) {
         if (layer64) snprintf(layer64, 64, "%s", e->plan.convs[iw].name.c_str());
         return fail(e, PE_ERR_RANGE, "layer %s produced values outside the range of %s (max |v| = %.3g x scale): run pe_calibrate",
-                    e->plan.convs[iw].name.c_str(), what, worst * limit);
+                    e->plan.convs[iw].name.c_str(), p.range_what, worst * p.range_limit);
     }
-    if (is >= 0 && smallest < floor_) {
+    if (is >= 0 && smallest < p.range_floor) {
         if (layer64) snprintf(layer64, 64, "%s", e->plan.convs[is].name.c_str());
         return fail(e, PE_ERR_RANGE, "layer %s: largest stored value %.3g is below %s, %s lose precision: run pe_calibrate",
-                    e->plan.convs[is].name.c_str(), smallest, e4 ? "2^-2" : s8 ? "4" : "2^-10", what);
+                    e->plan.convs[is].name.c_str(), smallest, p.range_floor_text, p.range_what);
     }
     if (layer64 && iw >= 0) snprintf(layer64, 64, "%s", e->plan.convs[iw].name.c_str());
     return PE_OK;
@@ -1560,7 +1546,7 @@ extern "C" int pe_forward_net_input(pe_engine* e, const float* net_input, int n)
     PreArgs a = e->pre;
     a.nframes = n;
     e->launches += launch_input_from_planar(e->d_planar, a, n * e->cfg.num_scales, e->stream);
-    e->input_lo_dirty = e->fmt.planes > 0;
+    e->input_lo_dirty = e->prec->fmt.planes > 0;
     e->last_frames = nullptr;
     return run_net(e, n);
 }
@@ -1707,11 +1693,11 @@ extern "C" int pe_fetch_maps(pe_engine* e, float* maps8, int n) {
 }
 static float blob_scale(const pe_engine* e, const BlobRef& b) {
     if (b.prod >= 0 && b.prod < (int)e->conv_scale.size()) return e->conv_scale[b.prod];
-    return b.act == e->plan.input_act ? net_input_scale(e) : 1.f;
+    return b.act == e->plan.input_act ? e->prec->net_input_scale : 1.f;
 }
 extern "C" int pe_blob_log2_scale(pe_engine* e, const char* blob_name, int* k) {
     if (!e || !blob_name || !k) return PE_ERR_INVALID;
-    if (!e->fmt.ranged()) return fail(e, PE_ERR_INVALID, "this precision has no range scales");
+    if (!e->prec->ranged()) return fail(e, PE_ERR_INVALID, "this precision has no range scales");
     for (const BlobRef& b : e->plan.blobs) {
         if (b.name != blob_name) continue;
         int ex = 0;
@@ -1741,7 +1727,7 @@ extern "C" int pe_fetch_blob(pe_engine* e, const char* blob_name, float* out, si
         float* d = nullptr;
         CK(e, cudaMalloc(&d, cnt * sizeof(float)));
         // stored value = true value * conv_scale[producer] (pools pass their producer's scale through; the net input has
-        // net_input_scale); s8: q * 2^-k, exact in fp32
+        // the mode's net_input_scale); s8: q * 2^-k, exact in fp32
         const float inv = 1.f / blob_scale(e, b);
         e->launches += launch_act_to_nchw(e->acts[b.act], e->plan.acts[b.act].C, b.coff, b.c, e->act_plane[b.act], act_fmt(e, b.act), g, inv, d,
                                           e->stream);

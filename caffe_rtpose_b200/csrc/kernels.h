@@ -3,39 +3,10 @@
 #include <cuda_fp8.h>
 
 #include "common.h"
+#include "precision.h"   // PlaneFmt: the storage format of the conv stack's activations and packed weights
 
 namespace pe {
 
-// Storage format of the conv stack's activations and packed weights: `planes` planes whose sum is the value (0: fp32), each of
-// element kind `elem`: IEEE fp16, bf16, or e4m3 (1 byte; a single plane).  The parity mode (2 planes) stores fp16 planes: 11 + 11
-// significant bits, so hi*hi + hi*lo + lo*hi carries ~2^-22 (bf16 planes: 8 + 8 bits, ~2^-17 - measured 2.2e-5 over the net with
-// exact accumulation vs 3e-6 for fp16).  The fast mode (F16X1) is the parity mode's hi plane alone.  E4M3X1 stores one e4m3 plane
-// (4 significant bits, largest finite 448), except the im2col'ed network input, which stays one fp16 plane (the values p/256 - 0.5
-// are exact in fp16, not in e4m3): conv1_1 reads fp16 and writes e4m3.  fp16's range (65504) and e4m3's need the per-layer
-// power-of-two range scales of pe_calibrate for nets outside O(1e-2 .. 1e3) (e4m3: O(1e-1 .. 1e2)); the bf16 modes (BF16X1,
-// BF16X3) have fp32's range.  S8X1 stores one s8 plane: integers q = sat(rint(x * 2^k)) with a per-layer power-of-two scale 2^k
-// (the im2col'ed network input included, at k = 8: p - 128), multiplied by per-output-channel s8 weights and summed exactly into
-// s32; it needs pe_calibrate (engine.cu, conv_s8.cu).
-enum PlaneElem { ELEM_BF16 = 0, ELEM_F16 = 1, ELEM_E4M3 = 2, ELEM_S8 = 3 };
-struct PlaneFmt {
-    int planes; PlaneElem elem;
-    __host__ __device__ bool f16() const { return elem == ELEM_F16; }
-    __host__ __device__ bool e4m3() const { return elem == ELEM_E4M3; }
-    __host__ __device__ bool s8() const { return elem == ELEM_S8; }
-    __host__ __device__ int elem_bytes() const { return planes == 0 ? 4 : (elem == ELEM_E4M3 || elem == ELEM_S8 ? 1 : 2); }
-    __host__ __device__ bool ranged() const { return planes > 0 && elem != ELEM_BF16; }   // range scales and range tracking
-};
-inline PlaneFmt plane_fmt(int precision) {   // PE_PREC_* -> format
-    switch (precision) {
-        case PE_PREC_BF16X1: return {1, ELEM_BF16};
-        case PE_PREC_F16X2: return {2, ELEM_F16};
-        case PE_PREC_BF16X3: return {3, ELEM_BF16};
-        case PE_PREC_F16X1: return {1, ELEM_F16};
-        case PE_PREC_E4M3X1: return {1, ELEM_E4M3};
-        case PE_PREC_S8X1: return {1, ELEM_S8};
-        default: return {0, ELEM_BF16};   // PE_PREC_FP32_SIMT
-    }
-}
 #ifdef __CUDACC__
 __device__ __forceinline__ float e4m3_to_float(uint8_t b) {
     return __half2float(__half(__nv_cvt_fp8_to_halfraw((__nv_fp8_storage_t)b, __NV_E4M3)));

@@ -1,0 +1,71 @@
+// The precision modes (PE_PREC_*, include/poseengine.h) in one table: the storage format of each mode and every per-mode rule
+// of the host code.  Host code reads a mode's facts from its row; device code receives the storage format (PlaneFmt) and the
+// element kinds as arguments and template parameters.  DESIGN.md section 3 explains the choices.
+#pragma once
+#include <cuda_runtime.h>   // __host__ __device__: device code uses PlaneFmt too
+
+#include "../../include/poseengine.h"
+
+namespace pe {
+
+// Element kind of a storage plane.  Facts that depend on the kind alone are functions of it.
+enum PlaneElem { ELEM_BF16 = 0, ELEM_F16 = 1, ELEM_E4M3 = 2, ELEM_S8 = 3 };
+__host__ __device__ constexpr int elem_size(PlaneElem e) { return e == ELEM_E4M3 || e == ELEM_S8 ? 1 : 2; }   // bytes
+// pack_conv_weights scales a layer's weights by a power of two so that max|w| lies in [2^(top-1), 2^top): fp16 [2^13, 2^14) keeps
+// the lo plane of small weights out of the subnormals, e4m3 [128, 256) stays below the largest finite 448 and keeps weights down to
+// max|w| * 2^-13 normal.  0: no scaling (bf16 has fp32's range; s8 scales each output channel, s8.h).  A fact of the element kind,
+// not of the mode: E4M3X1 packs conv1_1's weights in fp16.
+constexpr int weight_top(PlaneElem e) { return e == ELEM_F16 ? 14 : e == ELEM_E4M3 ? 8 : 0; }
+
+// Storage of activations and packed weights: `planes` planes of kind `elem` whose sum is the value; 0 planes: fp32.
+struct PlaneFmt {
+    int planes; PlaneElem elem;
+    __host__ __device__ bool f16() const { return elem == ELEM_F16; }
+    __host__ __device__ bool e4m3() const { return elem == ELEM_E4M3; }
+    __host__ __device__ bool s8() const { return elem == ELEM_S8; }
+    __host__ __device__ int elem_bytes() const { return planes == 0 ? 4 : elem_size(elem); }
+};
+
+struct Precision {
+    PlaneFmt fmt;                  // activations and packed weights
+    PlaneElem input_elem;          // the im2col'ed net input, one plane, and so conv1_1's packed weights
+    int act_cpad;                  // channel granularity of every activation: one K block of the conv kernel (common.h)
+    int kp_input;                  // channel pitch of the im2col'ed net input (27 values)
+    int slot_align;                // Concat slots start at multiples of this many channels: 16 bytes of the element (plan.cpp)
+    bool chunked;                  // hi*hi accumulates in chunks summed with round-to-nearest (conv_tc.cu); else one chain over K
+    int range_top;                 // pe_calibrate puts every stored maximum into [2^(range_top-1), 2^range_top); 0: no range scales
+    float range_limit;             // pe_range_status: PE_ERR_RANGE when a layer's largest stored value reaches this ...
+    float range_floor;             // ... or stays below this
+    const char* range_floor_text;  // the floor and the planes as pe_range_status's messages name them
+    const char* range_what;
+    float net_input_scale;         // stored net input = true value x this
+    bool needs_calibration;        // a forward before pe_calibrate is PE_ERR_STATE
+    long long max_k;               // largest K = taps x padded input channels of a layer; 0: no bound
+    bool per_channel_epilogue;     // one epilogue factor per output channel after the biases in the packed buffer; else one per layer
+    bool ranged() const { return range_top != 0; }   // range scales and range tracking
+};
+
+// Row i describes PE_PREC_* = i.
+//   E4M3X1 keeps the net input in fp16: p/256 - 0.5 is exact there, not in e4m3.
+//   S8X1 stores the net input as p - 128 = (p/256 - 0.5) x 2^8.  Its sums are exact, so nothing is chunked, and
+//   |acc| <= 128 x 127 x K stays inside s32 up to K = 132104.
+//   Calibration targets: fp16 [32, 64), 1000x below 65504; e4m3 [64, 128), 3.5-7x below 448 with values down to max x 2^-12
+//   still normal; s8 [32, 64): 6 bits and 2-4x headroom for frames busier than the calibration frame.
+//   Range floors: fp16 2^-10 (below it the lo plane lives in subnormals); e4m3 2^-2, 16x above the smallest normal, so that
+//   values a sixteenth of the maximum stay normal; s8 4 (under 3 bits).
+inline constexpr Precision PRECISIONS[] = {
+    // fmt, input_elem, act_cpad, kp_input, slot_align, chunked, range_top, range_limit, range_floor, range_floor_text, range_what,
+    // net_input_scale, needs_calibration, max_k, per_channel_epilogue
+    {{0, ELEM_BF16}, ELEM_BF16, 16, 32, 8, false, 0, 0.f, 0.f, nullptr, nullptr, 1.f, false, 0, false},                              // FP32_SIMT
+    {{1, ELEM_BF16}, ELEM_BF16, 64, 64, 8, false, 0, 0.f, 0.f, nullptr, nullptr, 1.f, false, 0, false},                              // BF16X1
+    {{2, ELEM_F16}, ELEM_F16, 64, 64, 8, true, 6, 65504.f, 9.765625e-4f, "2^-10", "the fp16 planes", 1.f, false, 0, false},          // F16X2
+    {{3, ELEM_BF16}, ELEM_BF16, 64, 64, 8, true, 0, 0.f, 0.f, nullptr, nullptr, 1.f, false, 0, false},                               // BF16X3
+    {{1, ELEM_F16}, ELEM_F16, 64, 64, 8, true, 6, 65504.f, 9.765625e-4f, "2^-10", "the fp16 planes", 1.f, false, 0, false},          // F16X1
+    {{1, ELEM_E4M3}, ELEM_F16, 128, 64, 16, true, 7, 448.f, 0.25f, "2^-2", "the e4m3 planes", 1.f, false, 0, false},                 // E4M3X1
+    {{1, ELEM_S8}, ELEM_S8, 128, 128, 16, false, 6, 127.f, 4.f, "4", "the s8 planes", 256.f, true, 132104, true},                    // S8X1
+};
+constexpr int NUM_PRECISIONS = sizeof PRECISIONS / sizeof PRECISIONS[0];
+static_assert(NUM_PRECISIONS == PE_PREC_S8X1 + 1, "one row per PE_PREC_* mode");
+inline const Precision& precision(int pe_prec) { return PRECISIONS[pe_prec]; }   // pe_prec in [0, NUM_PRECISIONS)
+
+}  // namespace pe

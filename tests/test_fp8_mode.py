@@ -16,11 +16,10 @@ import numpy as np
 import pytest
 import torch
 
-from test_conv_build import per_kernel
+from test_conv_build import check_no_spills_and_no_serialised_wgmma, check_one_wgmma_group_in_flight, tu_build
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "caffe_rtpose_b200", "csrc")
-NVCC = shutil.which("nvcc") or ("/usr/local/cuda/bin/nvcc" if os.path.exists("/usr/local/cuda/bin/nvcc") else None)
 # <BN, 1, e4m3, e4m3> and <BN, 1, fp16, e4m3> (conv1_1) at BN = 16, 32, 48, 64, 128
 INSTANCES = 10
 
@@ -93,42 +92,17 @@ def test_host_e4m3_saturates_beyond_448(to_e4m3):
     assert to_e4m3(np.array([np.nan], np.float32))[0] & 0x7F == 0x7F
 
 
-@pytest.fixture(scope="module")
-def build(tmp_path_factory):
-    if NVCC is None:
-        pytest.skip("nvcc not found")
-    obj = str(tmp_path_factory.mktemp("fp8_build") / "conv_fp8.o")
-    r = subprocess.run([NVCC, "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC",
-                        "--expt-relaxed-constexpr", "-Xptxas", "-v", "-x", "cu", "-c", os.path.join(CSRC, "conv_fp8.cu"), "-o", obj],
-                       capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-4000:]
-    cuobjdump = os.path.join(os.path.dirname(os.path.realpath(NVCC)), "cuobjdump")
-    sass = subprocess.run([cuobjdump if os.path.exists(cuobjdump) else "cuobjdump", "-sass", obj],
-                          capture_output=True, text=True, check=True).stdout
-    return r.stderr, sass
+build = tu_build("conv_fp8.cu")
 
 
 def test_fp8_instances_no_spills_and_no_serialised_wgmma(build):
-    log, _ = build
-    kernels = per_kernel(log, r"(?:Compiling entry function|Function properties for) '?(\w+)")
-    assert len(kernels) == INSTANCES, sorted(kernels)
-    for name, lines in kernels.items():
-        text = "\n".join(lines)
-        spill = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", text)
-        assert spill and spill.groups() == ("0", "0"), (name, text)
-    assert not re.search(r"wgmma.*serializ", log, re.I), [l for l in log.splitlines() if re.search("serializ", l, re.I)]
+    check_no_spills_and_no_serialised_wgmma(build[0], INSTANCES)
 
 
 def test_fp8_instances_keep_one_wgmma_group_in_flight(build):
-    _, sass = build
-    kernels = per_kernel(sass, r"Function : (\w+)")
-    assert len(kernels) == INSTANCES, sorted(kernels)
+    kernels = check_one_wgmma_group_in_flight(build[1], INSTANCES)
     n_e4m3 = 0
-    for name, lines in kernels.items():
-        waits = [l for l in lines if "WARPGROUP.DEPBAR.LE" in l]
-        assert any("gsb0, 0x1" in l for l in waits), (name, waits)
-        assert any("gsb0, 0x0" in l for l in waits), (name, waits)
-        text = "\n".join(lines)
+    for name, text in kernels.items():
         assert "F2FP.SATFINITE.E4M3" in text, name     # the epilogue's cvt.rn.satfinite.e4m3x2.f32
         n_e4m3 += bool(re.search(r"QGMMA\.64x\d+x32\.F32\.E4M3\.E4M3", text))
     assert n_e4m3 == INSTANCES // 2, n_e4m3            # the fp16-input conv1_1 instances run fp16 MMAs

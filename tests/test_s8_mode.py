@@ -4,7 +4,7 @@
   the rule of poseengine.h - sigma = max|w| / 127, q = clamp(rint(w / sigma), -127, 127) - bit for bit: sigma's bits and every
   q, on random channels of several magnitudes, on channels whose values are exact .5 multiples of sigma (ties go to even), on
   all-zero channels (sigma = 0, q = 0) and on a channel with a single non-zero weight.
-* The accumulator bound: 132104 is the largest K for which 128 x 127 x K fits in s32.
+* The accumulator bound: the engine's largest K (precision.h) is the largest for which 128 x 127 x K fits in s32.
 * conv_s8.cu, the s8 instances of conv_wg_kernel, built with -Xptxas -v: the checks of test_conv_build.py (no spills, no
   serialised wgmma, one wgmma group in flight) for every instance, the s8 MMA and the saturating s8 conversion in the SASS.
 * rtpose.bin: --help lists --precision 6, and --precision 6 without range calibration is refused at start-up.
@@ -17,14 +17,13 @@ import subprocess
 import numpy as np
 import pytest
 
-from test_conv_build import per_kernel
+from test_conv_build import check_no_spills_and_no_serialised_wgmma, check_one_wgmma_group_in_flight, tu_build
+from test_precision_table import read_table
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "caffe_rtpose_b200", "csrc")
 BIN = os.path.join(ROOT, "caffe_rtpose_b200", "rtpose.bin")
-NVCC = shutil.which("nvcc") or ("/usr/local/cuda/bin/nvcc" if os.path.exists("/usr/local/cuda/bin/nvcc") else None)
 INSTANCES = 5   # <BN, 1, s8, s8> at BN = 16, 32, 48, 64, 128
-S8_MAX_K = 132104
 
 HARNESS = r"""
 #include <stdio.h>
@@ -114,48 +113,25 @@ def test_host_quantisation_equals_numpy(quantize):
     assert got[-1][1][17] == -127 and np.count_nonzero(got[-1][1]) == 1
 
 
-def test_accumulator_bound():
-    """|acc| <= 128 x 127 x K: K = 132104 stays inside s32, K = 132105 does not."""
-    assert 128 * 127 * S8_MAX_K <= 2 ** 31 - 1 < 128 * 127 * (S8_MAX_K + 1)
-    assert 49 * 2816 > S8_MAX_K   # a 7x7 on 2700 channels (padded to 2816) is over it; the shipped nets' largest K is 49 x 256
+def test_accumulator_bound(tmp_path):
+    """|acc| <= 128 x 127 x K: the engine's bound K = 132104 stays inside s32, K = 132105 does not."""
+    max_k = read_table(tmp_path)["S8X1"]["max_k"]
+    assert max_k == 132104
+    assert 128 * 127 * max_k <= 2 ** 31 - 1 < 128 * 127 * (max_k + 1)
+    assert 49 * 2816 > max_k   # a 7x7 on 2700 channels (padded to 2816) is over it; the shipped nets' largest K is 49 x 256
 
 
-@pytest.fixture(scope="module")
-def build(tmp_path_factory):
-    if NVCC is None:
-        pytest.skip("nvcc not found")
-    obj = str(tmp_path_factory.mktemp("s8_build") / "conv_s8.o")
-    r = subprocess.run([NVCC, "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC",
-                        "--expt-relaxed-constexpr", "-Xptxas", "-v", "-x", "cu", "-c", os.path.join(CSRC, "conv_s8.cu"), "-o", obj],
-                       capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-4000:]
-    cuobjdump = os.path.join(os.path.dirname(os.path.realpath(NVCC)), "cuobjdump")
-    sass = subprocess.run([cuobjdump if os.path.exists(cuobjdump) else "cuobjdump", "-sass", obj],
-                          capture_output=True, text=True, check=True).stdout
-    return r.stderr, sass
+build = tu_build("conv_s8.cu")
 
 
 def test_s8_instances_no_spills_and_no_serialised_wgmma(build):
-    log, _ = build
-    kernels = per_kernel(log, r"(?:Compiling entry function|Function properties for) '?(\w+)")
-    assert len(kernels) == INSTANCES, sorted(kernels)
-    for name, lines in kernels.items():
-        text = "\n".join(lines)
-        spill = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", text)
-        assert spill and spill.groups() == ("0", "0"), (name, text)
-    assert not re.search(r"wgmma.*serializ", log, re.I), [l for l in log.splitlines() if re.search("serializ", l, re.I)]
+    check_no_spills_and_no_serialised_wgmma(build[0], INSTANCES)
 
 
 def test_s8_instances_keep_one_wgmma_group_in_flight(build):
-    _, sass = build
-    kernels = per_kernel(sass, r"Function : (\w+)")
-    assert len(kernels) == INSTANCES, sorted(kernels)
+    kernels = check_one_wgmma_group_in_flight(build[1], INSTANCES)
     widths = set()
-    for name, lines in kernels.items():
-        waits = [l for l in lines if "WARPGROUP.DEPBAR.LE" in l]
-        assert any("gsb0, 0x1" in l for l in waits), (name, waits)
-        assert any("gsb0, 0x0" in l for l in waits), (name, waits)
-        text = "\n".join(lines)
+    for name, text in kernels.items():
         m = re.findall(r"IGMMA\.64x(\d+)x32\.S8\.S8", text)
         assert m, name                                   # wgmma m64nNk32.s32.s8.s8
         widths |= {int(x) for x in m}
