@@ -59,10 +59,11 @@ struct ConvSpec {
     std::vector<int> cin_prod; // engine input channel -> index of the conv that produced it (-1: zero pad / the net input)
     int im2col_input;          // conv1_1: the input activation already holds the 3x3x3 patch (K=27)
     double flops_per_image;
+    int elem;                  // element kind (PlaneElem) of its arithmetic: of its input activation and packed weights
 };
 struct PoolSpec { std::string name; int in_act, out_act, level_in; };
 struct CopySpec { int src_act, dst_act, channels; };  // duplicate F into the second concat buffer
-struct ActSpec { int level, C; std::string blob; int blob_c; };  // blob: prototxt top living at channel 0
+struct ActSpec { int level, C; std::string blob; int blob_c; int elem; };  // blob: prototxt top living at channel 0; elem: PlaneElem
 struct OpRef { int type, idx; };                      // 0 conv, 1 pool, 2 copy
 // A fetchable blob: where it lives, which conv produced it (its stored values carry that conv's range scale; -1: the net
 // input), and the first later op of the forward that overwrites its channels (empty: none; the ping-pong concat buffers).
@@ -83,14 +84,20 @@ struct NetPlan {
     int gap[4] = {1, 1, 1, 1};   // per level: max(1, largest conv pad at that level), see Geo
 };
 struct NetDef;
-// plan from a parsed prototxt / built-in definition; -1 and a message when the graph is outside the supported family
-// slot_align: channel granularity of the Concat slots, so that the copy of the shared slot moves whole 16-byte chunks without
-// touching the next slot
-int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& out, std::string& err, int slot_align);
-int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& out, std::string& err);   // slot_align 8
-// kp_input: channel pitch of the im2col'ed network input; cpad: channel granularity of every activation.  The engine passes
-// the mode's kp_input, act_cpad and slot_align (precision.h).
-NetPlan build_plan(int model, int kp_input, int cpad, int slot_align = 8);
+// Element kinds of a plan (plan.cpp, DESIGN.md section 3): a conv layer listed in f16 computes in fp16, the others in
+// base_elem (conv1_1: input_elem).  "narrow" in f16 stands for every conv layer that reads fewer than 128 channels.
+// layout[k]: channel pad, net input pitch and Concat slot alignment of an activation of element kind k (PlaneElem).
+struct ActLayout { int cpad, kp_input, slot_align; };
+struct PlanFormats {
+    int base_elem = 0, input_elem = 0;
+    std::vector<std::string> f16;
+    ActLayout layout[4] = {};
+};
+// plan from a parsed prototxt / built-in definition; -1 and a message when the graph is outside the supported family or the
+// fp16 list breaks the format rules
+int build_plan_from_net(const NetDef& net, const PlanFormats& f, NetPlan& out, std::string& err);
+// One element kind throughout, Concat slots 8-aligned
+int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& out, std::string& err);
 
 // ---------------------------------------------------------------------------------------------
 // kernel argument blocks

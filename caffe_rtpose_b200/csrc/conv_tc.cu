@@ -149,6 +149,7 @@ int tc_layer_launch(const TcLayer& l, int nimg, cudaStream_t st, int share) {
     const long long tiles = ((long long)nimg * a.tiles_img + TC_CLUSTER - 1) / TC_CLUSTER * TC_CLUSTER;
     const dim3 grid((unsigned)tiles, (unsigned)(d.cout_pad / bn), 1);
     const PlaneFmt f = d.fmt;
+    if (f.elem != d.out_elem && d.out_elem != ELEM_E4M3) return launch_mixed(l, a, grid, st, bmap, bn);   // conv_mixed.cu
     if (d.out_elem == ELEM_E4M3) return launch_e4m3(l, a, grid, st, bmap, bn);   // conv_fp8.cu
     if (d.out_elem == ELEM_S8) return launch_s8(l, a, grid, st, bmap, bn);       // conv_s8.cu
     if (f.planes == 3) return launch_widths<3, ELEM_BF16, ELEM_BF16>(l, a, grid, st, bmap, bn);

@@ -459,8 +459,10 @@ static int launch_widths(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStrea
     }
 }
 
-// Layers with e4m3 output (conv_fp8.cu) and s8 layers (conv_s8.cu): their instances live in translation units of their own.
+// Layers with e4m3 output (conv_fp8.cu), s8 layers (conv_s8.cu) and the format boundaries of mixed engines (conv_mixed.cu):
+// their instances live in translation units of their own.
 int launch_e4m3(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap, int bn);
 int launch_s8(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap, int bn);
+int launch_mixed(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap, int bn);
 
 }  // namespace pe

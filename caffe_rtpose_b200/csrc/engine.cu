@@ -115,15 +115,21 @@ struct pe_engine {
 static void drop_graphs(pe_engine* e);
 static int setup_lanes(pe_engine* e);
 
-// Storage of activation i and of conv i's packed weights: the mode's format, except for the im2col'ed net input.  i = -1, the
-// planar fp32 maps, gets the mode's format, which picks the kernel instance of the last layers.
-static PlaneFmt act_fmt(const pe_engine* e, int i) {
-    const PlaneFmt f = e->prec->fmt;
-    return i == e->plan.input_act ? PlaneFmt{f.planes, e->prec->input_elem} : f;
+// Storage of activation i: the mode's plane count in the element kind the plan gave it (plan.cpp: the kind of the conv layers
+// that read it).  conv i's packed weights have the kind of its arithmetic, which is that of its input.
+static PlaneFmt act_fmt(const pe_engine* e, int i) { return PlaneFmt{e->prec->fmt.planes, (PlaneElem)e->plan.acts[i].elem}; }
+static PlaneFmt conv_wfmt(const pe_engine* e, int i) { return PlaneFmt{e->prec->fmt.planes, (PlaneElem)e->plan.convs[i].elem}; }
+// Element kind conv i stores: its output activation's, or for the planar fp32 maps its own, which picks the kernel instance
+static PlaneElem conv_out_elem(const pe_engine* e, int i) {
+    const ConvSpec& c = e->plan.convs[i];
+    return (PlaneElem)(c.out_act >= 0 ? e->plan.acts[c.out_act].elem : c.elem);
 }
-static PlaneFmt conv_wfmt(const pe_engine* e, int i) { return act_fmt(e, e->plan.convs[i].in_act); }
+// Per-layer facts (precision.h, elem_row): those of the arithmetic from the row of conv i's kind, the range facts from the row
+// of the kind it stores
+static const Precision& conv_row(const pe_engine* e, int i) { return elem_row(*e->prec, (PlaneElem)e->plan.convs[i].elem); }
+static const Precision& out_row(const pe_engine* e, int i) { return elem_row(*e->prec, conv_out_elem(e, i)); }
 // floats of conv i's epilogue fields in the packed buffer: bias[cout_pad], then the layer's factor or one factor per channel
-static size_t epi_floats(const pe_engine* e, int i) { return (size_t)e->cout_pad[i] + (e->prec->per_channel_epilogue ? e->cout_pad[i] : 1); }
+static size_t epi_floats(const pe_engine* e, int i) { return (size_t)e->cout_pad[i] + (conv_row(e, i).per_channel_epilogue ? e->cout_pad[i] : 1); }
 static size_t fmt_bytes(PlaneFmt f) { return (size_t)f.elem_bytes() * (f.planes ? f.planes : 1); }   // bytes per element, all planes
 
 static int fail(pe_engine* e, int code, const char* fmt, ...) {
@@ -295,16 +301,84 @@ extern "C" int pe_plan_describe(int model, const char* prototxt_path, char* buf,
     return (int)s.size();
 }
 
-static int create_impl(const pe_config* cfg, const char* prototxt_path, pe_engine** out);
-extern "C" int pe_create(const pe_config* cfg, pe_engine** out) { return create_impl(cfg, nullptr, out); }
+static const char* elem_name(PlaneFmt f) {
+    static const char* names[] = {"bf16", "f16", "e4m3", "s8"};
+    return f.planes == 0 ? "f32" : names[f.elem];
+}
+
+// The plan of `net` in mode `prec` with the conv layers of `f16_layers` (comma-separated names and "narrow"; NULL or empty: none)
+// in fp16.  Each element kind lays out its activations by its own row (elem_row); plan.cpp applies the format rules.  Mixing is
+// for the one-byte modes E4M3X1 and S8X1 only: the other modes' plane counts or element kinds differ from F16X1's.
+static int plan_for(const NetDef& net, int prec, const char* f16_layers, NetPlan& p, std::string& err) {
+    const Precision& base = precision(prec);
+    PlanFormats f;
+    f.base_elem = base.fmt.elem; f.input_elem = base.input_elem;
+    for (int k = 0; k < 4; k++) {
+        const Precision& r = elem_row(base, (PlaneElem)k);
+        f.layout[k] = {r.act_cpad, r.kp_input, r.slot_align};
+    }
+    for (const char* s = f16_layers; s && *s;) {
+        const char* end = strchr(s, ',');
+        std::string name(s, end ? end - s : strlen(s));
+        name.erase(0, name.find_first_not_of(" \t"));
+        name.erase(name.find_last_not_of(" \t") + 1);
+        if (!name.empty()) f.f16.push_back(name);
+        s = end ? end + 1 : s + strlen(s);
+    }
+    if (!f.f16.empty() && prec != PE_PREC_E4M3X1 && prec != PE_PREC_S8X1) {
+        err = "fp16 layers mix only with PE_PREC_E4M3X1 (5) and PE_PREC_S8X1 (6), not with precision " + std::to_string(prec);
+        return -1;
+    }
+    return build_plan_from_net(net, f, p, err);
+}
+
+// Host-only view of the element kinds of a plan (DESIGN.md section 3): "act <index> <kind> <channel pitch> <blob or ->" per
+// activation, then "conv <name> <compute kind> <stored kind> <in_act> <out_act>" per conv layer; f32: the planar maps or the
+// FP32_SIMT mode.
+extern "C" int pe_plan_formats(int model, const char* prototxt_path, int prec, const char* f16_layers, char* buf, int cap) {
+    NetDef net;
+    std::string err;
+    if (prec < 0 || prec >= NUM_PRECISIONS) return -fail(nullptr, PE_ERR_INVALID, "unknown precision %d", prec);
+    if (prototxt_path) {
+        if (parse_prototxt_file(prototxt_path, net, err)) return -fail(nullptr, PE_ERR_IO, "%s: %s", prototxt_path, err.c_str());
+    } else {
+        if (model != PE_MODEL_MPI_15 && model != PE_MODEL_COCO_18) return -fail(nullptr, PE_ERR_INVALID, "unknown model %d", model);
+        net = builtin_netdef(model, 6);
+    }
+    NetPlan p;
+    if (plan_for(net, prec, f16_layers, p, err)) return -fail(nullptr, PE_ERR_INVALID, "%s", err.c_str());
+    const int planes = precision(prec).fmt.planes;
+    std::string s;
+    char t[512];
+    for (size_t i = 0; i < p.acts.size(); i++) {
+        const ActSpec& a = p.acts[i];
+        snprintf(t, sizeof t, "act %zu %s %d %s\n", i, elem_name({planes, (PlaneElem)a.elem}), a.C, a.blob.empty() ? "-" : a.blob.c_str());
+        s += t;
+    }
+    for (const ConvSpec& c : p.convs) {
+        const PlaneFmt out = c.out_act >= 0 ? PlaneFmt{planes, (PlaneElem)p.acts[c.out_act].elem} : PlaneFmt{0, ELEM_BF16};
+        snprintf(t, sizeof t, "conv %s %s %s %d %d\n", c.name.c_str(), elem_name({planes, (PlaneElem)c.elem}), elem_name(out), c.in_act, c.out_act);
+        s += t;
+    }
+    if (buf && (int)s.size() < cap) memcpy(buf, s.c_str(), s.size() + 1);
+    return (int)s.size();
+}
+
+static int create_impl(const pe_config* cfg, const char* prototxt_path, const char* f16_layers, pe_engine** out);
+extern "C" int pe_create(const pe_config* cfg, pe_engine** out) { return create_impl(cfg, nullptr, nullptr, out); }
 // new caffe::Net(proto, TEST): the graph comes from the deploy prototxt (rtpose.cpp:183, net.cpp:30-50); cfg->model may be
 // -1, the model then follows the Nms layer's num_parts as in rtpose.cpp:212-229.
 extern "C" int pe_create_from_prototxt(const pe_config* cfg, const char* prototxt_path, pe_engine** out) {
     if (!prototxt_path) return fail(nullptr, PE_ERR_INVALID, "null prototxt path");
-    return create_impl(cfg, prototxt_path, out);
+    return create_impl(cfg, prototxt_path, nullptr, out);
+}
+extern "C" int pe_create_mixed(const pe_config* cfg, const char* prototxt_path, const char* f16_layers, pe_engine** out) {
+    if (cfg && cfg->precision != PE_PREC_E4M3X1 && cfg->precision != PE_PREC_S8X1)
+        return fail(nullptr, PE_ERR_INVALID, "pe_create_mixed: the base precision must be PE_PREC_E4M3X1 (5) or PE_PREC_S8X1 (6), not %d", cfg->precision);
+    return create_impl(cfg, prototxt_path, f16_layers, out);
 }
 
-static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_engine** out) {
+static int create_impl(const pe_config* cfg_in, const char* prototxt_path, const char* f16_layers, pe_engine** out) {
     if (!cfg_in || !out) return fail(nullptr, PE_ERR_INVALID, "null argument");
     *out = nullptr;
     pe_config cfg_copy = *cfg_in;
@@ -312,18 +386,22 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
     if (cfg->precision < 0 || cfg->precision >= NUM_PRECISIONS) return fail(nullptr, PE_ERR_INVALID, "unknown precision %d", cfg->precision);
     const Precision& prec = precision(cfg->precision);
     NetDef netdef;
-    NetPlan proto_plan;
+    NetPlan plan;
     if (prototxt_path) {
         std::string perr;
         if (parse_prototxt_file(prototxt_path, netdef, perr)) return fail(nullptr, PE_ERR_IO, "%s: %s", prototxt_path, perr.c_str());
-        if (build_plan_from_net(netdef, prec.kp_input, prec.act_cpad, proto_plan, perr, prec.slot_align))
+        if (plan_for(netdef, cfg->precision, f16_layers, plan, perr))
             return fail(nullptr, PE_ERR_INVALID, "%s: %s", prototxt_path, perr.c_str());
-        if (cfg->model >= 0 && cfg->model != proto_plan.model)
+        if (cfg->model >= 0 && cfg->model != plan.model)
             return fail(nullptr, PE_ERR_INVALID, "%s describes the %s model (nms num_parts %d), the configuration asks for model %d", prototxt_path,
-                        proto_plan.model == PE_MODEL_MPI_15 ? "MPI" : "COCO", proto_plan.nms_num_parts, cfg->model);
-        cfg->model = proto_plan.model;
+                        plan.model == PE_MODEL_MPI_15 ? "MPI" : "COCO", plan.nms_num_parts, cfg->model);
+        cfg->model = plan.model;
     }
     if (cfg->model != PE_MODEL_MPI_15 && cfg->model != PE_MODEL_COCO_18) return fail(nullptr, PE_ERR_INVALID, "unknown model %d", cfg->model);
+    if (!prototxt_path) {
+        std::string perr;
+        if (plan_for(builtin_netdef(cfg->model, 6), cfg->precision, f16_layers, plan, perr)) return fail(nullptr, PE_ERR_INVALID, "%s", perr.c_str());
+    }
     if (cfg->net_w <= 0 || cfg->net_h <= 0 || cfg->net_w % 8 || cfg->net_h % 8)
         return fail(nullptr, PE_ERR_INVALID, "net resolution %dx%d must be positive multiples of 8", cfg->net_w, cfg->net_h);
     if (cfg->num_scales < 1 || cfg->num_scales > PE_MAX_SCALES) return fail(nullptr, PE_ERR_INVALID, "num_scales %d out of [1,%d]", cfg->num_scales, PE_MAX_SCALES);
@@ -340,7 +418,7 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
     memset(&e->pre, 0, sizeof e->pre);
     e->cfg = *cfg;
     e->mt_own = model_tables(cfg->model);
-    if (prototxt_path) e->mt_own.max_peaks = proto_plan.nms_max_peaks;   // nms_param.max_peaks (NmsLayer::GetMaxPeaks, rtpose.cpp:195)
+    if (prototxt_path) e->mt_own.max_peaks = plan.nms_max_peaks;   // nms_param.max_peaks (NmsLayer::GetMaxPeaks, rtpose.cpp:195)
     e->mt = &e->mt_own;
     e->prec = &prec;
     if (const char* g = getenv("PE_CHECK_RANGE")) e->check_range = atoi(g) != 0;
@@ -359,13 +437,13 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, pe_en
     for (int i = 0; i < 16; i++) CKC(cudaEventCreate(&e->ev[i]));
 
     // the plan first: each level's gap is the largest pad of its convolutions (common.h)
-    e->plan = prototxt_path ? proto_plan : build_plan(cfg->model, prec.kp_input, prec.act_cpad, prec.slot_align);
-    if (prec.max_k)
-        for (const ConvSpec& c : e->plan.convs) {
+    e->plan = plan;
+    for (const ConvSpec& c : e->plan.convs)   // the s8 bound of the layers that compute in s8
+        if (const long long max_k = elem_row(prec, (PlaneElem)c.elem).max_k) {
             const long long K = (long long)(c.im2col_input ? 1 : c.k * c.k) * c.in_cused;
-            if (K > prec.max_k) {
+            if (K > max_k) {
                 fail(e, PE_ERR_INVALID, "layer %s: K = %lld (%dx%d taps x %d padded input channels) exceeds %lld, the largest K whose s8 sums "
-                     "stay inside s32 (|acc| <= 128 x 127 x K): PE_PREC_S8X1 cannot run it", c.name.c_str(), K, c.k, c.k, c.in_cused, prec.max_k);
+                     "stay inside s32 (|acc| <= 128 x 127 x K): PE_PREC_S8X1 cannot run it", c.name.c_str(), K, c.k, c.k, c.in_cused, max_k);
                 return bail(PE_ERR_INVALID);
             }
         }
@@ -593,14 +671,14 @@ static size_t packed_layout(pe_engine* e) {
 // is f_c = sigma_c * s_out / s_ref.  The net input carries the mode's net_input_scale.
 static float input_ref_scale(const pe_engine* e, const ConvSpec& c) {
     for (int pc : c.cin_prod) if (pc >= 0) return e->conv_scale[pc];
-    return e->prec->net_input_scale;   // the net input
+    return elem_row(*e->prec, (PlaneElem)e->plan.acts[c.in_act].elem).net_input_scale;   // the net input
 }
 static void fill_epilogue_fields(const pe_engine* e, int i, float* B) {
     const ConvSpec& c = e->plan.convs[i];
     const float s_ref = input_ref_scale(e, c);
     const float s_out = c.out_act >= 0 ? e->conv_scale[i] : 1.f;   // the planar stride-8 maps are true values
     for (int co = 0; co < c.cout; co++) B[co] = e->bias_true[i][co] * s_out;
-    if (e->prec->per_channel_epilogue) {
+    if (conv_row(e, i).per_channel_epilogue) {
         for (int co = 0; co < c.cout; co++) B[e->cout_pad[i] + co] = e->wsig[i][co] * (s_out / s_ref);
         return;
     }
@@ -692,7 +770,7 @@ static int bind_packed(pe_engine* e) {
             d.w = (char*)e->d_packed + e->w_off[i]; d.bias = (const float*)((char*)e->d_packed + e->b_off[i]);
             d.cout = c.cout; d.cout_pad = e->cout_pad[i]; d.ksize = c.im2col_input ? 1 : c.k; d.pad = c.im2col_input ? 0 : c.pad;
             d.relu = c.relu; d.fmt = conv_wfmt(e, (int)i); d.geo = g; d.out_scale = d.bias + e->cout_pad[i];
-            d.out_elem = act_fmt(e, c.out_act).elem; d.chunked = e->prec->chunked;
+            d.out_elem = conv_out_elem(e, (int)i); d.chunked = conv_row(e, (int)i).chunked;
             d.range = (e->prec->ranged() && e->d_range) ? e->d_range + i : nullptr;
             if (c.out_act >= 0) {
                 d.out = e->acts[c.out_act]; d.out_pitch = e->plan.acts[c.out_act].C; d.out_coff = c.out_coff; d.out_plane = e->act_plane[c.out_act];
@@ -756,6 +834,7 @@ extern "C" int pe_share_weights(pe_engine* from, pe_engine* to) {
     for (size_t i = 0; i < to->plan.convs.size(); i++) {
         const ConvSpec &a = from->plan.convs[i], &b = to->plan.convs[i];
         if (a.name != b.name || a.cout != b.cout || a.cin != b.cin || a.k != b.k) return fail(from, PE_ERR_INVALID, "layer %s differs between the handles", a.name.c_str());
+        if (a.elem != b.elem) return fail(from, PE_ERR_INVALID, "layer %s runs in fp16 in one handle only: the fp16 layers differ", a.name.c_str());
     }
     CK(to, cudaSetDevice(to->cfg.device));
     CK(to, cudaStreamSynchronize(to->stream));
@@ -786,6 +865,9 @@ extern "C" int pe_broadcast_weights(pe_engine* const* engines, int n) {
         if (!e || e->cfg.model != root->cfg.model || e->cfg.precision != root->cfg.precision || e->cfg.net_w != root->cfg.net_w ||
             e->cfg.net_h != root->cfg.net_h)
             return fail(root, PE_ERR_INVALID, "engine %d is not a replica of engine 0 (model / precision / net size differ)", i);
+        bool same = e->plan.convs.size() == root->plan.convs.size();
+        for (size_t l = 0; same && l < e->plan.convs.size(); l++) same = e->plan.convs[l].elem == root->plan.convs[l].elem;
+        if (!same) return fail(root, PE_ERR_INVALID, "engine %d is not a replica of engine 0 (the fp16 layers differ)", i);
         if (!e->committed) {   // allocate the packed buffer + TMA maps with the same layout (values arrive by broadcast)
             for (size_t l = 0; l < e->plan.convs.size(); l++) {
                 const ConvSpec& c = e->plan.convs[l];
@@ -916,7 +998,7 @@ static int run_op(pe_engine* e, const OpRef& op, int nimg, cudaStream_t st = nul
         const Geo& gi = e->geo[p.level_in]; const Geo& go = e->geo[p.level_in + 1];
         PoolArgs a;
         a.in = e->acts[p.in_act]; a.out = e->acts[p.out_act]; a.C = e->plan.acts[p.in_act].C;
-        a.in_plane = e->act_plane[p.in_act]; a.out_plane = e->act_plane[p.out_act]; a.fmt = e->prec->fmt;
+        a.in_plane = e->act_plane[p.in_act]; a.out_plane = e->act_plane[p.out_act]; a.fmt = act_fmt(e, p.in_act);
         a.Wi = gi.W; a.Hi = gi.H; a.Wpi = gi.Wp; a.Hsi = gi.Hs; a.Wo = go.W; a.Ho = go.H; a.Wpo = go.Wp; a.Hso = go.Hs; a.N = nimg;
         e->launches += launch_pool(a, st);
     } else {
@@ -924,7 +1006,7 @@ static int run_op(pe_engine* e, const OpRef& op, int nimg, cudaStream_t st = nul
         const Geo& g = e->geo[3];
         CopyArgs a;
         a.src = e->acts[c.src_act]; a.dst = e->acts[c.dst_act]; a.pitch = e->plan.acts[c.src_act].C; a.channels = c.channels;
-        a.elem_bytes = e->prec->fmt.elem_bytes(); a.M = (long long)nimg * g.Hs * g.Wp; a.plane = e->act_plane[c.src_act]; a.fmt = e->prec->fmt;
+        a.fmt = act_fmt(e, c.src_act); a.elem_bytes = a.fmt.elem_bytes(); a.M = (long long)nimg * g.Hs * g.Wp; a.plane = e->act_plane[c.src_act];
         e->launches += launch_copy_channels(a, st);
     }
     return PE_OK;
@@ -1482,8 +1564,8 @@ extern "C" int pe_calibrate(pe_engine* e, const uint8_t* const* frames, int n) {
             CK(e, cudaMemcpyAsync(&bits, e->d_range + i, sizeof bits, cudaMemcpyDeviceToHost, e->stream));
             CK(e, cudaStreamSynchronize(e->stream));
             float m; memcpy(&m, &bits, 4);
-            // m * s in [2^(range_top-1), 2^range_top) (precision.h)
-            const int top = e->prec->range_top;
+            // m * s in [2^(range_top-1), 2^range_top) of the stored kind's row (precision.h)
+            const int top = out_row(e, i).range_top;
             if (m > 0.f && m < 3e38f) { int ex = 0; frexpf(m, &ex); e->conv_scale[i] = ldexpf(1.f, std::max(-100, std::min(100, top - ex))); }
         }
         if ((rc = upload_fields(e, i))) return rc;
@@ -1494,9 +1576,9 @@ extern "C" int pe_calibrate(pe_engine* e, const uint8_t* const* frames, int n) {
     return run_post_and_return(e, n);
 }
 
-// Largest |stored value| / the mode's range_limit (precision.h) over the conv layers since the last call.  PE_ERR_RANGE when a
-// layer reached that limit, or when a layer's maximum fell below the mode's range_floor.  s8: the largest stored value is
-// rint(max |t|).  *layer64 names the worst layer.
+// Largest |stored value| / range_limit (precision.h) over the conv layers since the last call.  PE_ERR_RANGE when a layer
+// reached that limit, or when a layer's maximum fell below range_floor; both from the row of the kind the layer stores (out_row).
+// s8: the largest stored value is rint(max |t|).  *layer64 names the worst layer.
 extern "C" int pe_range_status(pe_engine* e, float* worst_ratio, char* layer64) {
     if (!e) return PE_ERR_INVALID;
     if (worst_ratio) *worst_ratio = 0.f;
@@ -1508,25 +1590,26 @@ extern "C" int pe_range_status(pe_engine* e, float* worst_ratio, char* layer64) 
     std::vector<unsigned> bits(nc);
     CK(e, cudaMemcpy(bits.data(), e->d_range, nc * sizeof(unsigned), cudaMemcpyDeviceToHost));
     CK(e, cudaMemset(e->d_range, 0, nc * sizeof(unsigned)));
-    const Precision& p = *e->prec;
-    const bool s8 = p.fmt.s8();
-    float worst = 0.f, smallest = 3e38f;
+    float worst = 0.f, smallest = 3e38f, lowest = 3e38f;   // lowest: the smallest maximum relative to its layer's floor
     int iw = -1, is = -1;
     for (size_t i = 0; i < nc; i++) {
         if (e->plan.convs[i].out_act < 0) continue;   // fp32 maps
+        const Precision& p = out_row(e, (int)i);
         float m; memcpy(&m, &bits[i], 4);
         if (bits[i] == 0) continue;                   // layer did not run since the last call
-        if (s8 && m <= 3e38f) m = rintf(m);           // the kernels track |t| before the rounding: the stored value
+        if (p.fmt.s8() && m <= 3e38f) m = rintf(m);   // the kernels track |t| before the rounding: the stored value
         if (!(m <= 3e38f) || m / p.range_limit > worst) { worst = (m <= 3e38f) ? m / p.range_limit : 2.f; iw = (int)i; }
-        if (m < smallest) { smallest = m; is = (int)i; }
+        if (m / p.range_floor < lowest) { lowest = m / p.range_floor; smallest = m; is = (int)i; }
     }
     if (worst_ratio) *worst_ratio = worst;
     if (worst >= 1.f) {
+        const Precision& p = out_row(e, iw);
         if (layer64) snprintf(layer64, 64, "%s", e->plan.convs[iw].name.c_str());
         return fail(e, PE_ERR_RANGE, "layer %s produced values outside the range of %s (max |v| = %.3g x scale): run pe_calibrate",
                     e->plan.convs[iw].name.c_str(), p.range_what, worst * p.range_limit);
     }
-    if (is >= 0 && smallest < p.range_floor) {
+    if (is >= 0 && lowest < 1.f) {
+        const Precision& p = out_row(e, is);
         if (layer64) snprintf(layer64, 64, "%s", e->plan.convs[is].name.c_str());
         return fail(e, PE_ERR_RANGE, "layer %s: largest stored value %.3g is below %s, %s lose precision: run pe_calibrate",
                     e->plan.convs[is].name.c_str(), smallest, p.range_floor_text, p.range_what);
@@ -1693,7 +1776,7 @@ extern "C" int pe_fetch_maps(pe_engine* e, float* maps8, int n) {
 }
 static float blob_scale(const pe_engine* e, const BlobRef& b) {
     if (b.prod >= 0 && b.prod < (int)e->conv_scale.size()) return e->conv_scale[b.prod];
-    return b.act == e->plan.input_act ? e->prec->net_input_scale : 1.f;
+    return b.act == e->plan.input_act ? elem_row(*e->prec, act_fmt(e, b.act).elem).net_input_scale : 1.f;
 }
 extern "C" int pe_blob_log2_scale(pe_engine* e, const char* blob_name, int* k) {
     if (!e || !blob_name || !k) return PE_ERR_INVALID;

@@ -11,6 +11,7 @@
 #include <map>
 
 #include "common.h"
+#include "precision.h"
 #include "prototxt.h"
 
 namespace pe {
@@ -65,7 +66,7 @@ static const int kMaxChannels = 16384;   // a user's prototxt is untrusted input
 // "same"-padded convolutions, in-place ReLU, 2x2/2 MAX pooling, channel Concat, ImResize(factor 8), Nms, any number
 // of stages.  Anything else is reported as an error (the reference would run it through generic Caffe layers).
 // ---------------------------------------------------------------------------------------------
-int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, std::string& err, int slot_align) {
+int build_plan_from_net(const NetDef& net, const PlanFormats& fm, NetPlan& p, std::string& err) {
     p = NetPlan();
     const int NL = (int)net.layers.size();
     auto fail = [&](const std::string& m) { err = m; return -1; };
@@ -89,7 +90,7 @@ int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, s
     if (nms.nms_max_peaks < 1 || nms.nms_max_peaks > PE_MAX_PEAKS) return fail("nms max_peaks out of range");
     if (nms.bottoms.size() != 1 || rsz.tops.size() != 1 || nms.bottoms[0] != rsz.tops[0]) return fail("Nms must consume the ImResize output");
     const ModelTables& mt = model_tables(p.model);
-    p.c_l1 = 2 * mt.num_limbs; p.c_l2 = mt.num_parts + 1; p.kp_input = kp_input;
+    p.c_l1 = 2 * mt.num_limbs; p.c_l2 = mt.num_parts + 1;
     p.nms_threshold = nms.nms_threshold; p.nms_max_peaks = nms.nms_max_peaks; p.nms_num_parts = nms.nms_num_parts;
     p.resize_start_scale = rsz.resize_start_scale; p.resize_scale_gap = rsz.resize_scale_gap;
 
@@ -159,6 +160,60 @@ int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, s
     // ---- concat buffers: slice layout shared by all non-final concats, two physical buffers
     std::vector<int> concats;
     for (int i = 0; i < NL; i++) if (net.layers[i].type == "Concat" && i != final_concat) concats.push_back(i);
+
+    // ---- element kinds (DESIGN.md section 3).  A conv layer computes in fp16 when it is listed, else in the mode's kind (conv1_1
+    // in the net input's).  Blobs that live in one buffer form a group: a pool's input and output (the pool passes the format
+    // through), and every non-final Concat with its bottoms - the two ping-pong buffers and the shared conv4_4_CPM, which the copy
+    // moves without converting.  A group takes the kind of the conv layers that read it, so those must agree.
+    std::map<std::string, std::string> up;   // union-find over blob names
+    auto root = [&](std::string b) { while (up.count(b) && up[b] != b) b = up[b]; return b; };
+    auto unite = [&](const std::string& a, const std::string& b) { const std::string ra = root(a), rb = root(b); if (ra != rb) up[ra] = rb; };
+    for (int i = 0; i < NL; i++) {
+        const ProtoLayer& l = net.layers[i];
+        if (l.type == "Pooling") unite(l.bottoms[0], l.tops[0]);
+        if (l.type == "Concat" && i != final_concat) {
+            for (const std::string& b : l.bottoms) unite(b, l.tops[0]);
+            unite(l.tops[0], net.layers[concats[0]].tops[0]);
+        }
+    }
+    std::map<std::string, int> conv_layer;                // conv name -> layer index
+    std::map<std::string, std::vector<int>> readers;      // group -> conv layers reading it, in net order
+    for (int i = 0; i < NL; i++)
+        if (net.layers[i].type == "Convolution") { conv_layer[net.layers[i].name] = i; readers[root(net.layers[i].bottoms[0])].push_back(i); }
+    std::map<std::string, bool> listed;
+    bool narrow = false;
+    for (const std::string& n : fm.f16) {
+        if (n == "narrow") narrow = true;
+        else if (!conv_layer.count(n)) return fail("unknown conv layer " + n + " in the fp16 layer list");
+        else listed[n] = true;
+    }
+    if (narrow)   // every reader of the group reads fewer than 128 channels: its e4m3 / s8 K block is partly padding
+        for (const auto& g : readers) {
+            bool all = true;
+            for (int i : g.second) all = all && channels[net.layers[i].bottoms[0]] < 128;
+            if (all) for (int i : g.second) listed[net.layers[i].name] = true;
+        }
+    auto conv_elem = [&](int i) {
+        const ProtoLayer& l = net.layers[i];
+        return listed.count(l.name) ? (int)ELEM_F16 : l.bottoms[0] == input_blob ? fm.input_elem : fm.base_elem;
+    };
+    std::map<std::string, int> group_elem;
+    for (const auto& g : readers) {
+        for (int i : g.second)
+            if (conv_elem(i) != conv_elem(g.second[0])) {
+                std::string names;
+                for (int j : g.second) names += (names.empty() ? "" : ", ") + net.layers[j].name;
+                return fail("layers " + names + " read one buffer and must run in one format: list all of them as fp16 layers or none");
+            }
+        group_elem[g.first] = conv_elem(g.second[0]);
+    }
+    auto elem_of = [&](const std::string& blob) {
+        auto it = group_elem.find(root(blob));
+        return it == group_elem.end() ? fm.base_elem : it->second;
+    };
+    const int cc_elem = concats.empty() ? fm.base_elem : elem_of(net.layers[concats[0]].tops[0]);
+    const int cpad = fm.layout[cc_elem].cpad, slot_align = fm.layout[cc_elem].slot_align;   // of the concat buffers
+
     std::map<std::string, int> n_in_concats;
     for (int ci : concats) for (const std::string& b : net.layers[ci].bottoms) n_in_concats[b]++;
     struct Slot { int caffe_off, eng_off, c; bool shared; };
@@ -202,8 +257,8 @@ int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, s
                 return fail("the stages overlap in a way the two-buffer concat scheme cannot hold");
     }
 
-    auto new_act = [&](int lv, int c, const std::string& blob, int blob_c) {
-        ActSpec a; a.level = lv; a.C = round_up(c, cpad); a.blob = blob; a.blob_c = blob_c;
+    auto new_act = [&](int lv, int c, const std::string& blob, int blob_c, int elem) {
+        ActSpec a; a.level = lv; a.C = round_up(c, fm.layout[elem].cpad); a.blob = blob; a.blob_c = blob_c; a.elem = elem;
         p.acts.push_back(a);
         if (!blob.empty()) p.blobs.push_back({blob, (int)p.acts.size() - 1, 0, blob_c});
         return (int)p.acts.size() - 1;
@@ -218,7 +273,9 @@ int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, s
     std::map<std::string, int> conv_index;   // blob -> index in p.convs of its producer
 
     // network input, im2col'ed 3x3x3 patches: engine channel (r*3+s)*3+c  <-  original weight index (c, r, s)
-    p.input_act = new_act(0, kp_input, "", 0);
+    const int input_elem = elem_of(input_blob), kp_input = fm.layout[input_elem].kp_input;
+    p.kp_input = kp_input;
+    p.input_act = new_act(0, kp_input, "", 0, input_elem);
     p.acts[p.input_act].C = kp_input;
     p.blobs.push_back({input_blob, p.input_act, 12, 3});  // centre tap (r=1,s=1) of the patch = the net input itself
     int cc[2] = {-1, -1};
@@ -235,7 +292,7 @@ int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, s
             c.name = l.name; c.cout = l.num_output; c.k = l.kernel; c.pad = l.pad; c.level = level[top];
             c.relu = 0;
             for (int u : consumers[top]) if (net.layers[u].type == "ReLU") c.relu = 1;
-            c.planar_coff = 0; c.out_coff = 0; c.flops_per_image = 0; c.im2col_input = 0;
+            c.planar_coff = 0; c.out_coff = 0; c.flops_per_image = 0; c.im2col_input = 0; c.elem = conv_elem(i);
             // input
             if (l.bottoms[0] == input_blob) {
                 if (l.kernel != 3) return fail("layer " + l.name + ": the first convolution must be 3x3 (it consumes the im2col'ed input)");
@@ -252,7 +309,7 @@ int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, s
                 c.out_act = -1; c.planar_coff = final_off[top];
             } else if (concat_slot.count(top)) {
                 if (cc[0] < 0) {   // the two ping-pong concat buffers [shared | stage outputs]
-                    for (int b = 0; b < nbuf; b++) { cc[b] = new_act(3, cc_c, "", 0); p.acts[cc[b]].C = cc_c; }
+                    for (int b = 0; b < nbuf; b++) { cc[b] = new_act(3, cc_c, "", 0, cc_elem); p.acts[cc[b]].C = cc_c; }
                 }
                 const int j = concat_slot[top].first, k = concat_slot[top].second;
                 const Slot& sdef = slots[j][k];
@@ -267,7 +324,7 @@ int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, s
                     loc[top] = o;
                 }
             } else {
-                c.out_act = new_act(c.level, c.cout, top, c.cout);
+                c.out_act = new_act(c.level, c.cout, top, c.cout, elem_of(top));
                 p.blobs.back().prod = (int)p.convs.size(); p.blobs.back().pos = (int)p.order.size();
                 Loc o; o.act = c.out_act; o.coff = 0; o.cused = p.acts[c.out_act].C; o.cmap = ident(c.cout, o.cused);
                 o.prod.assign(o.cused, -1);
@@ -284,7 +341,7 @@ int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, s
         } else if (l.type == "Pooling") {
             const Loc& in = loc[l.bottoms[0]];
             if (in.act < 0 || in.coff != 0 || p.acts[in.act].level != level[l.bottoms[0]]) return fail("layer " + l.name + ": unsupported pooling input");
-            const int out = new_act(level[top], channels[top], top, channels[top]);
+            const int out = new_act(level[top], channels[top], top, channels[top], elem_of(top));
             p.blobs.back().prod = in.prod.empty() ? -1 : in.prod[0]; p.blobs.back().pos = (int)p.order.size();
             if (p.acts[out].C != p.acts[in.act].C) return fail("layer " + l.name + ": channel pitch mismatch");
             p.pools.push_back({l.name, in.act, out, level[l.bottoms[0]]});
@@ -330,14 +387,9 @@ int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, s
 }
 
 int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, std::string& err) {
-    return build_plan_from_net(net, kp_input, cpad, p, err, 8);
-}
-
-NetPlan build_plan(int model, int kp_input, int cpad, int slot_align) {
-    NetPlan p;
-    std::string err;
-    if (build_plan_from_net(builtin_netdef(model, 6), kp_input, cpad, p, err, slot_align)) fprintf(stderr, "poseengine: built-in plan: %s\n", err.c_str());
-    return p;
+    PlanFormats f;
+    for (ActLayout& l : f.layout) l = {cpad, kp_input, 8};
+    return build_plan_from_net(net, f, p, err);
 }
 
 }  // namespace pe

@@ -68,4 +68,12 @@ constexpr int NUM_PRECISIONS = sizeof PRECISIONS / sizeof PRECISIONS[0];
 static_assert(NUM_PRECISIONS == PE_PREC_S8X1 + 1, "one row per PE_PREC_* mode");
 inline const Precision& precision(int pe_prec) { return PRECISIONS[pe_prec]; }   // pe_prec in [0, NUM_PRECISIONS)
 
+// The row of a layer or activation of element kind k in an engine of mode `base`.  The one-plane 16-bit and 8-bit modes give
+// each kind one row - fp16: F16X1, e4m3: E4M3X1, s8: S8X1 - so that a layer of another kind than the mode's (E4M3X1's fp16 net
+// input, the fp16 layers of pe_create_mixed) follows its own kind's arithmetic, pads and range.  Other modes: their own row.
+inline const Precision& elem_row(const Precision& base, PlaneElem k) {
+    if (base.fmt.planes != 1 || k == ELEM_BF16) return base;
+    return precision(k == ELEM_F16 ? PE_PREC_F16X1 : k == ELEM_E4M3 ? PE_PREC_E4M3X1 : PE_PREC_S8X1);
+}
+
 }  // namespace pe

@@ -67,7 +67,7 @@ ABI_SYMBOLS = [
     "pe_camera_open", "pe_camera_close", "pe_camera_info", "pe_camera_grab", "pe_camera_last_error", "pe_yuyv_to_bgr",
     "pe_compare_results", "pe_jpeg_read_coefs", "pe_jpeg_coefs_to_bgr", "pe_forward_jpeg_coefs", "pe_video_read_coefs",
     "pe_jpeg_read_scan", "pe_jpeg_scan_to_coefs_host", "pe_forward_jpeg_scans", "pe_jpeg_decode_scans", "pe_video_read_scan",
-    "pe_forward_pixels", "pe_stream_wait", "pe_pixels_to_bgr", "pe_blob_log2_scale",
+    "pe_forward_pixels", "pe_stream_wait", "pe_pixels_to_bgr", "pe_blob_log2_scale", "pe_create_mixed", "pe_plan_formats",
 ]
 
 
@@ -83,6 +83,8 @@ def lib():
     L.pe_create.argtypes = [C.POINTER(_Config), C.POINTER(C.c_void_p)]
     L.pe_create_from_prototxt.argtypes = [C.POINTER(_Config), C.c_char_p, C.POINTER(C.c_void_p)]
     L.pe_plan_describe.argtypes = [C.c_int, C.c_char_p, C.c_char_p, C.c_int]
+    L.pe_create_mixed.argtypes = [C.POINTER(_Config), C.c_char_p, C.c_char_p, C.POINTER(C.c_void_p)]
+    L.pe_plan_formats.argtypes = [C.c_int, C.c_char_p, C.c_int, C.c_char_p, C.c_char_p, C.c_int]
     L.pe_destroy.argtypes = [C.c_void_p]
     L.pe_last_error.restype = C.c_char_p
     L.pe_last_error.argtypes = [C.c_void_p]
@@ -275,14 +277,19 @@ class PoseEngine:
     """One GPU worker (the reference's NetCopy + warmup(), rtpose.cpp:133-142, 173-237)."""
 
     def __init__(self, model=COCO_18, net_w=656, net_h=368, disp_w=1280, disp_h=720, num_scales=1, start_scale=1.0,
-                 scale_gap=0.3, device=0, max_batch=1, precision=PREC_BF16X2, prototxt=None):
+                 scale_gap=0.3, device=0, max_batch=1, precision=PREC_BF16X2, prototxt=None, f16_layers=None):
         """prototxt: path of a deploy prototxt (`new caffe::Net(proto, TEST)`, rtpose.cpp:183); model may then be None
-        and follows the Nms layer's num_parts (rtpose.cpp:212-229).  Without it the built-in graph of `model` is used."""
+        and follows the Nms layer's num_parts (rtpose.cpp:212-229).  Without it the built-in graph of `model` is used.
+        f16_layers: conv layer names (a list or a comma-separated string, "narrow" included) that run with PREC_F16X1's
+        arithmetic inside a PREC_E4M3X1 or PREC_S8X1 engine (pe_create_mixed); see plan_formats."""
         L = lib()
         cfg = _Config(device, -1 if model is None else model, net_w, net_h, disp_w, disp_h, num_scales, start_scale, scale_gap,
                       max_batch, precision)
         h = C.c_void_p()
-        if prototxt is not None:
+        if f16_layers is not None:
+            path = os.fsencode(prototxt) if prototxt is not None else None
+            rc = L.pe_create_mixed(C.byref(cfg), path, _layer_list(f16_layers), C.byref(h))
+        elif prototxt is not None:
             rc = L.pe_create_from_prototxt(C.byref(cfg), os.fsencode(prototxt), C.byref(h))
         else:
             rc = L.pe_create(C.byref(cfg), C.byref(h))
@@ -549,6 +556,32 @@ def plan_describe(model=None, prototxt=None):
     buf = C.create_string_buffer(n + 1)
     L.pe_plan_describe(-1 if model is None else model, path, buf, n + 1)
     return buf.value.decode()
+
+
+def _layer_list(layers):
+    return (layers if isinstance(layers, str) else ",".join(layers)).encode()
+
+
+def plan_formats(model=None, precision=PREC_E4M3X1, f16_layers=None, prototxt=None):
+    """Element kinds of the plan pe_create_mixed builds (host only, no GPU): {"acts": [(kind, channel pitch, blob or None)],
+    "convs": {name: (compute kind, stored kind, in_act, out_act)}}.  f16_layers None or empty: the plain plan of `precision`."""
+    L = lib()
+    path = os.fsencode(prototxt) if prototxt is not None else None
+    layers = _layer_list(f16_layers) if f16_layers is not None else None
+    m = -1 if model is None else model
+    n = L.pe_plan_formats(m, path, precision, layers, None, 0)
+    if n < 0:
+        raise PoseEngineError("pe_plan_formats failed (%d): %s" % (-n, L.pe_last_error(None).decode()))
+    buf = C.create_string_buffer(n + 1)
+    L.pe_plan_formats(m, path, precision, layers, buf, n + 1)
+    acts, convs = [], {}
+    for line in buf.value.decode().splitlines():
+        f = line.split()
+        if f[0] == "act":
+            acts.append((f[2], int(f[3]), None if f[4] == "-" else f[4]))
+        else:
+            convs[f[1]] = (f[2], f[3], int(f[4]), int(f[5]))
+    return {"acts": acts, "convs": convs}
 
 
 def write_json(joints, num_parts, frame_scale=1.0):

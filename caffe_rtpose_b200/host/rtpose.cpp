@@ -95,6 +95,9 @@ static void define_flags() {
            "5 FP8 mode (one e4m3 plane, 1 FP8 MMA per MAC; needs --calibrate_range, see --audit_every), "
            "6 INT8 mode (one s8 plane, 1 s8 MMA per MAC, exact integer sums, per-channel weight scales; requires --calibrate_range, "
            "see --audit_every)");
+    define("f16_layers", "", "[extension] with --precision 5 or 6: comma-separated conv layers that run in fp16 with --precision 4's arithmetic "
+           "while the others keep the FP8 / INT8 format; 'narrow' = the layers that read fewer than 128 channels (conv1_1, conv1_2, conv2_1). "
+           "Layers that read one buffer go together (pe_create_mixed); empty = none");
     define("batch", "0", "[extension] frames per forward per GPU: 1 = the reference's behaviour, 0 = automatic (file / synthetic sources "
            "fill two waves of 128-row tiles on the GPU, e.g. 9 frames at 656x368; results do not depend on it)");
     define("engines_per_gpu", "0", "[extension] worker handles per GPU: 1 = the reference's topology (one Net per GPU), 0 = automatic (2 when "
@@ -700,7 +703,7 @@ static int load_weights(pe_engine* e, int device) {   // CopyTrainedLayersFrom (
 // packs it and the replicas receive the packed buffer by one ncclBroadcast (the path's only collective).
 // engines[g * per_gpu + k] = handle k of GPU g.  Handle 0 of GPU 0 loads the model; handle 0 of the other GPUs receives the packed
 // weights by broadcast; handles k > 0 share their GPU's buffer (Net::ShareTrainedLayersWith).
-static bool create_engines(int num_gpu, int per_gpu, int precision, std::vector<pe_engine*>& engines) {
+static bool create_engines(int num_gpu, int per_gpu, int precision, const std::string& f16_layers, std::vector<pe_engine*>& engines) {
     const int batch = global.batch;
     for (int tid = 0; tid < num_gpu * per_gpu; tid++) {
         pe_config c;
@@ -709,7 +712,9 @@ static bool create_engines(int num_gpu, int per_gpu, int precision, std::vector<
         c.disp_w = global.disp_w; c.disp_h = global.disp_h; c.num_scales = Fi("num_scales");
         c.start_scale = Fd("start_scale"); c.scale_gap = Fd("scale_gap"); c.max_batch = batch; c.precision = precision;
         pe_engine* e = nullptr;
-        const int rc = global.proto_readable ? pe_create_from_prototxt(&c, F("caffeproto").c_str(), &e) : pe_create(&c, &e);
+        const std::string proto = F("caffeproto");
+        const int rc = !f16_layers.empty() ? pe_create_mixed(&c, global.proto_readable ? proto.c_str() : nullptr, f16_layers.c_str(), &e)
+                       : global.proto_readable ? pe_create_from_prototxt(&c, proto.c_str(), &e) : pe_create(&c, &e);
         if (rc) { LOG_ERROR("GPU %d: %s", c.device, pe_last_error(nullptr)); return false; }
         engines.push_back(e);
     }
@@ -1121,6 +1126,10 @@ int main(int argc, char** argv) {
         LOG_ERROR("--precision 6 (INT8) runs on calibrated per-layer range scales: at scale 1 almost every activation quantises to 0; drop --nocalibrate_range");
         return 1;
     }
+    if (!F("f16_layers").empty() && Fi("precision") != PE_PREC_E4M3X1 && Fi("precision") != PE_PREC_S8X1) {
+        LOG_ERROR("--f16_layers runs chosen layers in fp16 inside the FP8 or INT8 mode: it needs --precision 5 or 6");
+        return 1;
+    }
     if (Fi("audit_every") > 0 && Fi("precision") == PE_PREC_F16X2) {
         LOG_ERROR("--audit_every compares a faster precision with the parity mode; with --precision 2 there is nothing to compare");
         return 1;
@@ -1166,6 +1175,11 @@ int main(int argc, char** argv) {
     if (model == -2) { LOG_ERROR("Unknown number of parts! Couldn't set model"); return 1; }
     if (global.proto_readable) LOG_INFO("Net built from %s", F("caffeproto").c_str());
     global.model = model;
+    if (!F("f16_layers").empty() &&   // unknown names and lists that split a shared buffer, before any GPU call
+        pe_plan_formats(model, global.proto_readable ? F("caffeproto").c_str() : nullptr, Fi("precision"), F("f16_layers").c_str(), nullptr, 0) < 0) {
+        LOG_ERROR("--f16_layers %s: %s", F("f16_layers").c_str(), pe_last_error(nullptr));
+        return 1;
+    }
     {
         std::unique_ptr<ModelDescriptor> md;
         ModelDescriptorFactory::createModelDescriptor(model == PE_MODEL_MPI_15 ? ModelDescriptorFactory::Type::MPI_15 : ModelDescriptorFactory::Type::COCO_18, md);
@@ -1189,8 +1203,8 @@ int main(int argc, char** argv) {
     const int num_gpu = std::max(1, Fi("num_gpu"));
     std::vector<pe_engine*> engines, audit;
     const int per_gpu = global.engines_per_gpu, num_workers = num_gpu * per_gpu;
-    if (!create_engines(num_gpu, per_gpu, Fi("precision"), engines) ||
-        (Fi("audit_every") > 0 && !create_engines(num_gpu, per_gpu, PE_PREC_F16X2, audit))) {
+    if (!create_engines(num_gpu, per_gpu, Fi("precision"), F("f16_layers"), engines) ||
+        (Fi("audit_every") > 0 && !create_engines(num_gpu, per_gpu, PE_PREC_F16X2, "", audit))) {
         for (pe_engine* e : engines) pe_destroy(e);
         for (pe_engine* e : audit) pe_destroy(e);
         return 1;

@@ -90,6 +90,24 @@ int pe_create_from_prototxt(const pe_config* cfg, const char* prototxt_path, pe_
 /* host-only (no GPU): text description of the execution plan of a prototxt (or of the built-in graph of `model` when
  * prototxt_path is NULL); returns the text length (call with buf NULL to size it) or -PE_ERR_* */
 int pe_plan_describe(int model, const char* prototxt_path, char* buf, int cap);
+/* Mixed precision: an engine of base precision PE_PREC_E4M3X1 or PE_PREC_S8X1 (anything else is PE_ERR_INVALID) whose conv layers
+ * named in f16_layers run with PE_PREC_F16X1's arithmetic - one fp16 plane, weights scaled to max|w| in [2^13, 2^14), chunked
+ * round-to-nearest fp32 accumulation, stored maxima calibrated into [32, 64) - while the others keep the base mode's.
+ * f16_layers: comma-separated conv layer names, and/or "narrow" = every conv layer that reads fewer than 128 channels, whose
+ * e4m3 / s8 K block is partly padding (conv1_1, conv1_2, conv2_1 of the shipped nets); NULL or "": none, the base mode exactly.
+ * An activation is stored in the format of the layers that read it; the producing layer's epilogue converts.  Layers that read
+ * one buffer must be listed together (both branches' first layers; every stage's first layers together with the layers that
+ * read conv4_4_CPM, whose output shares the stage-input buffers): a list that splits such a group, or names an unknown layer,
+ * is PE_ERR_INVALID and pe_last_error(NULL) names the layers.  Range facts (calibration target, pe_range_status's limit and
+ * floor) follow the format a layer stores; engine-wide facts stay the base mode's (PE_PREC_S8X1 still needs pe_calibrate).
+ * pe_share_weights / pe_broadcast_weights need the same fp16 layers on both sides.  prototxt_path: NULL for the built-in graph
+ * of cfg->model, else as pe_create_from_prototxt.  DESIGN.md section 3. */
+int pe_create_mixed(const pe_config* cfg, const char* prototxt_path, const char* f16_layers, pe_engine** out);
+/* host-only: the element kinds pe_create_mixed (or, with f16_layers NULL or "", pe_create / pe_create_from_prototxt of any
+ * precision) gives the plan: "act <index> <kind> <channel pitch> <blob or ->" per activation, then "conv <name> <compute kind>
+ * <stored kind> <in_act> <out_act>" per conv layer; kinds are f32, bf16, f16, e4m3, s8 (f32: the planar maps).  Returns the
+ * text length as pe_plan_describe does, or -PE_ERR_INVALID with the reason in pe_last_error(NULL) for a list the rules refuse. */
+int pe_plan_formats(int model, const char* prototxt_path, int precision, const char* f16_layers, char* buf, int cap);
 void pe_destroy(pe_engine* e);
 /* last error text of this handle (or of the failed pe_create / pe_pixels_to_bgr when e == NULL) */
 const char* pe_last_error(const pe_engine* e);

@@ -12,7 +12,9 @@ On the resident loop's last step: the max error of the stride-8 maps relative to
 pe_compare_results against the parity mode at the north-star tolerance (1e-3 net px, in display px).  The same statistics on
 the prototxt-filler net (gaussian(0.01) weights, maps ~3e-11), calibrated with pe_calibrate on the first frame.  The He-init
 maps are noise with thousands of near-tie NMS decisions, so these pose statistics are a worst case, not what a trained
-model shows.  Prints the card, its power limit and SM clocks, then one JSON line."""
+model shows.  FM_MODES also takes mixed-precision entries "<base>+<fp16 layers>" (pe_create_mixed), e.g. e4m3x1+narrow or
+s8x1+conv1_1+conv1_2: calibrated like their base and reported like the other modes.  Prints the card, its power limit and SM
+clocks, then one JSON line."""
 import json
 import os
 import statistics
@@ -32,9 +34,18 @@ from layer_times import klass  # noqa: E402
 MODEL, NET_W, NET_H, DISP_W, DISP_H, B = engine.COCO_18, 656, 368, 1280, 720, 9
 MODES = {"f16x2": engine.PREC_F16X2, "f16x1": engine.PREC_F16X1, "e4m3x1": engine.PREC_E4M3X1, "s8x1": engine.PREC_S8X1,
          "bf16x1": engine.PREC_BF16X1}
-# FM_MODES: a comma-separated subset; the parity mode always runs, since every other mode is compared with it
-MODES = {m: p for m, p in MODES.items() if m == "f16x2" or m in os.environ.get("FM_MODES", ",".join(MODES)).split(",")}
 CALIBRATED = ("e4m3x1", "s8x1")
+
+
+def mode_spec(m):
+    """(PE_PREC_* of the base, fp16 layers or None) of an FM_MODES entry "<mode>" or "<base>+<layer>+<layer>..."."""
+    base, _, layers = m.partition("+")
+    return BASES[base], layers.replace("+", ",") or None
+
+
+# FM_MODES: a comma-separated subset; the parity mode always runs, since every other mode is compared with it
+BASES = MODES
+MODES = {m: mode_spec(m) for m in ["f16x2"] + [m for m in os.environ.get("FM_MODES", ",".join(BASES)).split(",") if m != "f16x2"]}
 TOL_PX = 1e-3 * max(DISP_W / NET_W, DISP_H / NET_H)
 
 
@@ -48,8 +59,10 @@ def card():
         return {"error": repr(ex)}
 
 
-def make_engines(prec, W, n=2, calibrate=None):
-    engs = [engine.PoseEngine(MODEL, NET_W, NET_H, DISP_W, DISP_H, max_batch=B, precision=prec) for _ in range(n)]
+def make_engines(spec, W, n=2, calibrate=None):
+    """n handles of mode spec (precision, fp16 layers) sharing one packed buffer, calibrated on `calibrate` when given."""
+    prec, layers = spec
+    engs = [engine.PoseEngine(MODEL, NET_W, NET_H, DISP_W, DISP_H, max_batch=B, precision=prec, f16_layers=layers) for _ in range(n)]
     engs[0].set_weights(W)
     if calibrate is not None:
         engs[0].calibrate(calibrate)
@@ -129,7 +142,7 @@ def main():
     dev = host_t.cuda()
     nb = n_frames // B
     W = synth.make_weights(MODEL, "he")
-    engs = {m: make_engines(p, W, calibrate=[host[0]] if m in CALIBRATED else None) for m, p in MODES.items()}
+    engs = {m: make_engines(p, W, calibrate=[host[0]] if m.partition("+")[0] in CALIBRATED else None) for m, p in MODES.items()}
     out = {m: {"resident_fps": [], "e2e_fps": []} for m in MODES}
     last = {}
     for _ in range(rounds):
@@ -148,14 +161,14 @@ def main():
     Wc = synth.make_weights(MODEL, "caffe")
     batch = [host[lb * B + k] for k in range(B)]
     filler = {}
-    for m in ("f16x2", "f16x1", "e4m3x1", "s8x1"):
-        if m in MODES:
+    for m in MODES:
+        if m.partition("+")[0] in ("f16x2", "f16x1", "e4m3x1", "s8x1"):
             e = make_engines(MODES[m], Wc, n=1, calibrate=[host[0]])[0]
             e.forward_frames(batch)
             filler[m] = results(e)
             e.close()
-    for m in ("f16x1", "e4m3x1", "s8x1"):
-        if m in MODES:
+    for m in filler:
+        if m != "f16x2":
             out[m]["vs_parity_filler_net"] = compare(filler[m], filler["f16x2"])
     print(json.dumps({"card": info, "workload": "C2 COCO 656x368, 9 frames per forward, W-he", "steps": steps, "rounds": rounds,
                       "tol_px": TOL_PX, "modes": out}), flush=True)
