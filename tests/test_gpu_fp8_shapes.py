@@ -12,14 +12,23 @@ The last stage's convolutions write the planar fp32 maps unrounded, so there d =
 the chunked FP8 accumulation.  In "three_stages" that layer is a 7x7 on 129 channels (padded to 256): 49 K steps of 128
 channels in chunks of 7 steps, 896 K each - the longest chunk the mode runs - so its error measures the chunk length.
 Max pooling is checked exact.
+
+Calibrated, three_stages: pe_calibrate gives every producer its own range scale, so the Concat readers of stages 2 and 3 fold
+power-of-two range ratios of three producers into their e4m3 weights; the reference rounds the weights with those ratios
+folded in (float_layer of tests/test_gpu_mixed_precision.py).  The width rule restated: the cases run every one-byte instance
+at every filter size (tests/test_gpu_s8_shapes.py states it without a GPU).
 """
 import numpy as np
 import pytest
+import torch
 
 from caffe_rtpose_b200 import engine
 from test_conv_shapes import CASES, FRAMES, layer_class, level_dims, spec_weights, write_prototxt
-from test_gpu_conv_layers import Blobs, conv_layers, conv_ref, plan_gaps, sample_pixels
+from test_gpu_conv_layers import Blobs, conv_layers, conv_ref, frames_for, plan_gaps, sample_pixels
 from test_gpu_fp8_mode import B_E8, e4m3_cell, packed_weights
+from test_gpu_mixed_precision import float_layer
+from test_gpu_s8_mode import IntBlobs
+from test_gpu_s8_shapes import WANT_ONE_BYTE, one_byte_widths
 
 pytestmark = pytest.mark.gpu
 E8 = engine.PREC_E4M3X1
@@ -80,3 +89,41 @@ def test_generated_convs_vs_float64_e4m3(name, tmp_path):
         over = {k: v for k, v in worst.items() if v > MEASURED_MAX[k]}
         assert not over, "accumulation error above what this kernel measured: %s" % over
 
+
+def test_generated_convs_vs_float64_e4m3_calibrated(tmp_path):
+    name = "three_stages"
+    spec, path = write_prototxt(name, tmp_path)
+    c = CASES[name]
+    net_w, net_h = c["net_w"], c["net_h"]
+    gaps = plan_gaps(prototxt=path)
+    kinds = engine.plan_formats(None, E8, None, prototxt=path)["convs"]
+    W = spec_weights(spec)
+    eng = engine.PoseEngine(None, net_w, net_h, 2 * net_w, 2 * net_h, start_scale=0.5, precision=E8, prototxt=path,
+                            max_batch=max(FRAMES))
+    eng.set_weights(W)
+    rng = np.random.default_rng(11)
+    worst, mixed = {}, set()
+    for n in FRAMES:
+        eng.calibrate(frames_for(n, 2 * net_w, 2 * net_h))
+        eng.forward_net_input((rng.integers(0, 256, (n, 3, net_h, net_w)) / 256.0 - 0.5).astype(np.float32))
+        ib = IntBlobs(eng, n, None, W, spec)
+        for layer in conv_layers(None, spec)[0]:
+            w_, h_ = level_dims(net_w, net_h, layer["level"])
+            pts = sample_pixels(n, h_, w_, gaps[layer["level"]], rng, 300)
+            compute, out = kinds[layer["name"]][:2]
+            r = float_layer(layer, eng, ib.blobs, ib.k, W, compute, out, pts)
+            key = layer_class(layer) + (" fp32" if out == "f32" else "")
+            worst[key] = max(worst.get(key, 0.0), r)
+            if len(set(ib.k(layer["bottom"]))) > 1:
+                mixed.add(layer["name"])
+    eng.close()
+    print("\n%s e4m3x1 calibrated: largest d / mag per layer class: %s; readers of mixed range scales: %s" % (
+        name, " ".join("%s %.3e" % (k, worst[k]) for k in sorted(worst)), sorted(mixed)))
+    assert {"Mconv1_stage%d_L%d" % (s, b) for s in (2, 3) for b in (1, 2)} <= mixed, mixed
+    over = {k: v for k, v in worst.items() if v > MEASURED_MAX[k]}
+    assert not over, "accumulation error above what this kernel measured: %s" % over
+
+
+def test_cases_run_every_one_byte_instance(tmp_path):
+    seen = one_byte_widths(tmp_path, torch.cuda.get_device_properties(0).multi_processor_count)
+    assert WANT_ONE_BYTE <= seen, sorted(WANT_ONE_BYTE - seen, key=str)

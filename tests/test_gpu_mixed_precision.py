@@ -139,8 +139,8 @@ def cell(got, kind, k):
     return lo * 2.0 ** -k, hi * 2.0 ** -k
 
 
-def float_layer(layer, eng, blobs, kscale, W, compute, out, pts):
-    """d / mag of an fp16 or e4m3 layer (module docstring)."""
+def float_layer(layer, eng, blobs, kscale, W, compute, out, pts, bound=None):
+    """d / mag of an fp16 or e4m3 layer (module docstring); bound: the layer's B instead of B_F16 / B_E8."""
     w, b = W[layer["name"]]
     kin = kscale(layer["bottom"])
     r = np.ldexp(1.0, kin.max() - kin).astype(np.float32)   # the power-of-two range ratios the packer folds in
@@ -153,7 +153,7 @@ def float_layer(layer, eng, blobs, kscale, W, compute, out, pts):
     else:
         lo, hi = cell(got, out, int(kscale(layer["top"])[0]))
         d = np.maximum(0.0, np.maximum(ref - hi, lo - ref))
-    B = B_F16 if compute == "f16" else B_E8
+    B = bound or (B_F16 if compute == "f16" else B_E8)
     bad = d > B * mag
     if bad.any():
         i, c = np.argwhere(bad)[0]

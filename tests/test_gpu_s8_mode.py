@@ -108,7 +108,7 @@ class IntBlobs:
 
 
 def check_layer(layer, ib, W, pts):
-    """Bit-exact check of one conv layer at sampled pixels; returns the number of compared values."""
+    """Bit-exact check of one conv layer at sampled pixels; returns (the number of compared values, the largest |acc|)."""
     w, b = W[layer["name"]]
     sigma, q = quantize(fold(w, ib.k(layer["bottom"])))
     acc = int_acc_at(ib.ints(layer["bottom"]), q, pts)
@@ -123,7 +123,7 @@ def check_layer(layer, ib, W, pts):
         i, c = np.argwhere(bad)[0]
         raise AssertionError("%s: %d of %d values differ; first at (n, y, x) = %s channel %d: got %.9g, want %.9g (k_out %d)"
                              % (layer["name"], int(bad.sum()), bad.size, tuple(pts[i]), c, got[i, c], want[i, c], k_out))
-    return bad.size
+    return bad.size, float(np.abs(acc).max())
 
 
 def make_engine(cfg, tmp_path, W=None):
@@ -162,7 +162,7 @@ def test_conv_layers_bit_exact(cfg, tmp_path):
     seen, count = set(), 0
     for layer in layers:
         w_, h_, gap = level_geo(net_w, net_h, layer["level"], gaps)
-        count += check_layer(layer, ib, W, sample_pixels(n, h_, w_, gap, rng, 300))
+        count += check_layer(layer, ib, W, sample_pixels(n, h_, w_, gap, rng, 300))[0]
         seen.add((layer_class(layer), tc_bn(W[layer["name"]][0].shape[0], n * (h_ + gap) * (w_ + gap), nsm)))
     eng.close()
     print("\n%s: %d layers, %d values bit-exact; (layer class, BN) run: %s" % (cfg, len(layers), count, sorted(seen, key=str)))
@@ -184,12 +184,13 @@ def test_configs_run_both_tile_widths():
     assert want <= seen, sorted(want - seen, key=str)
 
 
-def whole_stack(model, W, eng, nimg):
-    """The net in integers up to concat_stage7 from the engine's stored input (pe_fetch_blob of the input x 2^8): every conv
-    as in check_layer over the whole image (each at the k the engine calibrated), 2x2 max pooling (ceil mode) and Concat."""
-    convs, concat, final = conv_layers(model)
-    spec_layers = [l for l in netspec(model)["layers"] if l["type"] == "Pooling"]
-    inp = netspec(model)["input"]
+def whole_stack(spec, W, eng, nimg):
+    """The net of the layer table `spec` (netspec format) in integers up to its final Concat from the engine's stored input
+    (pe_fetch_blob of the input x 2^8): every conv as in check_layer over the whole image (each at the k the engine
+    calibrated), 2x2 max pooling (ceil mode) and Concat."""
+    convs, concat, final = conv_layers(None, spec)
+    spec_layers = [l for l in spec["layers"] if l["type"] == "Pooling"]
+    inp = spec["input"]
     k = {inp: eng.blob_log2_scale(inp)}
     val = {inp: eng.fetch_blob(inp)[:nimg].astype(np.float64) * 2.0 ** k[inp]}
     pools = {l["top"][0]: l["bottom"][0] for l in spec_layers}
@@ -237,7 +238,7 @@ def test_whole_stack_bit_exact(model):
     eng.calibrate(frames[:1])
     eng.forward_frames(frames)
     maps = eng.fetch_maps(2).astype(np.float64)
-    want = whole_stack(model, W, eng, 2)
+    want = whole_stack(netspec(model), W, eng, 2)
     eng.close()
     bad = maps != want
     assert not bad.any(), "%d of %d map values differ, max |diff| %.3g" % (int(bad.sum()), bad.size, float(np.abs(maps - want).max()))
