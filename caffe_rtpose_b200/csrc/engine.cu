@@ -24,6 +24,7 @@
 #include "pixels.cuh"
 #include <climits>
 #include "prototxt.h"
+#include "calib_table.h"
 
 // NVTX ranges (header-only nvtx3: resolved at run time, no-ops without a profiler attached) around the phases of a forward, so that
 // nsys / ncu timelines read like the reference's stage names (SURVEY.md section 5)
@@ -57,6 +58,11 @@ struct pe_engine {
     std::vector<std::vector<float>> wsig;   // S8X1: per conv, the per-output-channel weight step sigma_c of pack_conv_weights (s8.h)
     unsigned* d_range = nullptr;
     bool calibrated = false, check_range = false;
+    // pe_calibrate_begin .. _end: per conv, the largest true |output| (recorded / conv_scale) over the forwards since begin
+    bool collecting = false;
+    int collect_forwards = 0;
+    std::vector<float> collect_max;
+    uint64_t weights_hash = 0; bool weights_hash_valid = false;   // of hw (calibration tables); reset by pe_commit_weights
     std::vector<size_t> w_off, b_off;
     std::vector<int> cout_pad, cin_pad;
     std::vector<TcLayer> tc;        // wgmma per-conv launch state
@@ -790,8 +796,10 @@ static int bind_packed(pe_engine* e) {
 
 extern "C" int pe_commit_weights(pe_engine* e) {
     if (!e) return PE_ERR_INVALID;
+    if (e->collecting) return fail(e, PE_ERR_STATE, "a calibration collection is running: call pe_calibrate_end first");
     CK(e, cudaSetDevice(e->cfg.device));
     const size_t nc = e->plan.convs.size();
+    e->weights_hash_valid = false;
     for (size_t i = 0; i < nc; i++) {
         const ConvSpec& c = e->plan.convs[i];
         if (!e->hw[i].set || e->hw[i].w.size() != (size_t)c.cout * c.cin * c.k * c.k || e->hw[i].b.size() != (size_t)c.cout)
@@ -1088,6 +1096,7 @@ static int run_net(pe_engine* e, int n) {
     // at scale 1 almost every activation of a typical net quantises to 0
     if (e->prec->needs_calibration && !e->calibrated)
         return fail(e, PE_ERR_STATE, "PE_PREC_S8X1 runs on calibrated range scales: call pe_calibrate (on the handle that owns the weights) before the first forward");
+    if (e->collecting) e->collect_forwards++;   // its maxima accumulate in d_range (folded by pe_range_status and pe_calibrate_end)
     if (!e->use_graphs) return run_net_eager(e, n);
     pe_engine::GraphEntry& g = e->graphs[n];
     if (g.exec) {
@@ -1531,6 +1540,7 @@ extern "C" int pe_calibrate(pe_engine* e, const uint8_t* const* frames, int n) {
     if (!frames) return fail(e, PE_ERR_INVALID, "null frames");
     if (!e->committed) return fail(e, PE_ERR_STATE, "pe_commit_weights has not been called");
     if (!e->prec->ranged()) return PE_OK;   // fp32 / bf16 modes have fp32's exponent range
+    if (e->collecting) return fail(e, PE_ERR_STATE, "a calibration collection is running: call pe_calibrate_end first");
     const size_t nc = e->plan.convs.size();
     if (e->bias_true.size() != nc || e->bias_true[0].empty() || e->hw[0].w.empty())
         return fail(e, PE_ERR_STATE, "this handle received its weights by broadcast / sharing: calibrate the source handle before replicating");
@@ -1576,6 +1586,17 @@ extern "C" int pe_calibrate(pe_engine* e, const uint8_t* const* frames, int n) {
     return run_post_and_return(e, n);
 }
 
+// During a collection (pe_calibrate_begin): the maxima the kernels recorded since d_range was last cleared, in true units, into the
+// running maxima.  Scales are powers of two, so recorded / conv_scale is exact; NaN (a layer that produced one) is ignored.
+static void fold_range(pe_engine* e, const std::vector<unsigned>& bits) {
+    if (!e->collecting) return;
+    for (size_t i = 0; i < bits.size(); i++) {
+        if (e->plan.convs[i].out_act < 0 || bits[i] == 0) continue;
+        float m; memcpy(&m, &bits[i], 4);
+        if (m == m) e->collect_max[i] = fmaxf(e->collect_max[i], m / e->conv_scale[i]);
+    }
+}
+
 // Largest |stored value| / range_limit (precision.h) over the conv layers since the last call.  PE_ERR_RANGE when a layer
 // reached that limit, or when a layer's maximum fell below range_floor; both from the row of the kind the layer stores (out_row).
 // s8: the largest stored value is rint(max |t|).  *layer64 names the worst layer.
@@ -1590,6 +1611,7 @@ extern "C" int pe_range_status(pe_engine* e, float* worst_ratio, char* layer64) 
     std::vector<unsigned> bits(nc);
     CK(e, cudaMemcpy(bits.data(), e->d_range, nc * sizeof(unsigned), cudaMemcpyDeviceToHost));
     CK(e, cudaMemset(e->d_range, 0, nc * sizeof(unsigned)));
+    fold_range(e, bits);
     float worst = 0.f, smallest = 3e38f, lowest = 3e38f;   // lowest: the smallest maximum relative to its layer's floor
     int iw = -1, is = -1;
     for (size_t i = 0; i < nc; i++) {
@@ -1616,6 +1638,142 @@ extern "C" int pe_range_status(pe_engine* e, float* worst_ratio, char* layer64) 
     }
     if (layer64 && iw >= 0) snprintf(layer64, 64, "%s", e->plan.convs[iw].name.c_str());
     return PE_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Calibration over a set of frames (pe_calibrate_begin / _end) and calibration tables (pe_calibration_get / _set), DESIGN.md
+// section 3.  The kernels record every layer's largest |stored value| on every forward, on every input route; a collection folds
+// those maxima, divided by the layer's scale, into per-layer running maxima, and pe_calibrate_end sets the scales from them with
+// pe_calibrate's rule.  A table carries the scales to another engine with the same weights.
+// ---------------------------------------------------------------------------------------------
+static int calib_owner_check(pe_engine* e, const char* what) {
+    if (!e->committed) return fail(e, PE_ERR_STATE, "%s: pe_commit_weights has not been called", what);
+    if (!e->prec->ranged()) return fail(e, PE_ERR_INVALID, "%s: precision %d has no range scales (only 2, 4, 5 and 6 have)", what, e->cfg.precision);
+    const size_t nc = e->plan.convs.size();
+    if (e->bias_true.size() != nc || e->bias_true[0].empty() || e->hw[0].w.empty())
+        return fail(e, PE_ERR_STATE, "%s: this handle received its weights by broadcast / sharing: calibrate the handle that owns them", what);
+    if (e->packed_owner.use_count() > 1)
+        return fail(e, PE_ERR_STATE, "%s: this handle already shares its weights with another handle, which would keep the old scales: "
+                    "calibrate before pe_share_weights", what);
+    return PE_OK;
+}
+
+// The engine's table: every conv layer that stores an activation, with its stored kind and log2 scale
+static CalibTable engine_table(pe_engine* e) {
+    CalibTable t;
+    t.precision = e->cfg.precision;
+    if (!e->weights_hash_valid) {   // name, fp32 weights, fp32 biases of every conv layer in plan order
+        Fnv1a64 h;
+        for (size_t i = 0; i < e->plan.convs.size(); i++) {
+            const std::string& n = e->plan.convs[i].name;
+            h.add(n.c_str(), n.size() + 1);
+            h.add(e->hw[i].w.data(), e->hw[i].w.size() * sizeof(float));
+            h.add(e->hw[i].b.data(), e->hw[i].b.size() * sizeof(float));
+        }
+        e->weights_hash = h.h;
+        e->weights_hash_valid = true;
+    }
+    t.weights = e->weights_hash;
+    for (size_t i = 0; i < e->plan.convs.size(); i++) {
+        if (e->plan.convs[i].out_act < 0) continue;
+        int ex = 0;
+        frexpf(e->conv_scale[i], &ex);
+        t.layers.push_back({e->plan.convs[i].name, elem_name({e->prec->fmt.planes, conv_out_elem(e, (int)i)}), ex - 1});
+    }
+    return t;
+}
+
+// Sets the scales to `s`, re-packs the layers whose producers' scales changed (the Concat ratios and S8X1's per-channel quantisation
+// are folded into the weights) and every layer's epilogue fields, drops the graphs and the range state.  *changed: layers whose scale moved.
+static int apply_scales(pe_engine* e, const std::vector<float>& s, int* changed) {
+    CK(e, cudaSetDevice(e->cfg.device));
+    CK(e, cudaStreamSynchronize(e->stream));
+    drop_graphs(e);
+    const std::vector<float> old = e->conv_scale;
+    e->conv_scale = s;
+    int moved = 0;
+    for (size_t i = 0; i < s.size(); i++) moved += s[i] != old[i];
+    int rc;
+    for (size_t i = 0; i < s.size(); i++) {
+        bool repack = false;
+        for (int pc : e->plan.convs[i].cin_prod) if (pc >= 0 && s[pc] != old[pc]) repack = true;
+        if (repack && (rc = upload_weights(e, (int)i))) return rc;
+        if ((rc = upload_fields(e, (int)i))) return rc;
+    }
+    CK(e, cudaMemsetAsync(e->d_range, 0, s.size() * sizeof(unsigned), e->stream));
+    CK(e, cudaStreamSynchronize(e->stream));
+    e->calibrated = true;
+    if (changed) *changed = moved;
+    return PE_OK;
+}
+
+extern "C" int pe_calibrate_begin(pe_engine* e) {
+    if (!e) return PE_ERR_INVALID;
+    int rc = calib_owner_check(e, "pe_calibrate_begin"); if (rc) return rc;
+    if (e->collecting) return fail(e, PE_ERR_STATE, "pe_calibrate_begin: a collection is already running");
+    if (e->prec->needs_calibration && !e->calibrated)
+        return fail(e, PE_ERR_STATE, "pe_calibrate_begin: PE_PREC_S8X1 forwards only on calibrated scales: start with pe_calibrate or pe_calibration_set");
+    CK(e, cudaSetDevice(e->cfg.device));
+    CK(e, cudaStreamSynchronize(e->stream));
+    CK(e, cudaMemset(e->d_range, 0, e->plan.convs.size() * sizeof(unsigned)));   // maxima of earlier forwards do not count
+    e->collect_max.assign(e->plan.convs.size(), 0.f);
+    e->collect_forwards = 0;
+    e->collecting = true;
+    return PE_OK;
+}
+
+extern "C" int pe_calibrate_end(pe_engine* e, int* changed) {
+    if (!e) return PE_ERR_INVALID;
+    if (changed) *changed = 0;
+    int rc = calib_owner_check(e, "pe_calibrate_end"); if (rc) return rc;
+    if (!e->collecting) return fail(e, PE_ERR_STATE, "pe_calibrate_end: pe_calibrate_begin has not been called");
+    if (!e->collect_forwards) return fail(e, PE_ERR_STATE, "pe_calibrate_end: no forward since pe_calibrate_begin");
+    CK(e, cudaSetDevice(e->cfg.device));
+    CK(e, cudaStreamSynchronize(e->stream));
+    const size_t nc = e->plan.convs.size();
+    std::vector<unsigned> bits(nc);
+    CK(e, cudaMemcpy(bits.data(), e->d_range, nc * sizeof(unsigned), cudaMemcpyDeviceToHost));
+    fold_range(e, bits);
+    e->collecting = false;
+    std::vector<float> s = e->conv_scale;
+    for (size_t i = 0; i < nc; i++) {
+        if (e->plan.convs[i].out_act < 0) continue;
+        const float m = e->collect_max[i];   // pe_calibrate's rule: m * s in [2^(top-1), 2^top) of the stored kind's row; 0 keeps the scale
+        const int top = out_row(e, (int)i).range_top;
+        if (m > 0.f && m < 3e38f) { int ex = 0; frexpf(m, &ex); s[i] = ldexpf(1.f, std::max(-100, std::min(100, top - ex))); }
+    }
+    return apply_scales(e, s, changed);
+}
+
+extern "C" int pe_calibration_get(const pe_engine* ce, char* buf, int cap) {
+    if (!ce) return -PE_ERR_INVALID;
+    pe_engine* e = const_cast<pe_engine*>(ce);   // the error text and the cached weights hash
+    if (!e->committed) return -fail(e, PE_ERR_STATE, "pe_calibration_get: pe_commit_weights has not been called");
+    if (!e->prec->ranged()) return -fail(e, PE_ERR_INVALID, "pe_calibration_get: precision %d has no range scales", e->cfg.precision);
+    if (e->bias_true.size() != e->plan.convs.size() || e->bias_true[0].empty() || e->hw[0].w.empty())
+        return -fail(e, PE_ERR_STATE, "pe_calibration_get: this handle received its weights by broadcast / sharing: ask the handle that owns them");
+    for (const ConvSpec& c : e->plan.convs)
+        if (c.name.find_first_of(" \t\r\n#") != std::string::npos)
+            return -fail(e, PE_ERR_INVALID, "pe_calibration_get: layer name '%s' cannot be written into a table (white space or '#')", c.name.c_str());
+    const std::string s = write_calibration_table(engine_table(e));
+    if (buf && (int)s.size() < cap) memcpy(buf, s.c_str(), s.size() + 1);
+    return (int)s.size();
+}
+
+extern "C" int pe_calibration_set(pe_engine* e, const char* text) {
+    if (!e) return PE_ERR_INVALID;
+    int rc = calib_owner_check(e, "pe_calibration_set"); if (rc) return rc;
+    if (e->collecting) return fail(e, PE_ERR_STATE, "pe_calibration_set: a calibration collection is running: call pe_calibrate_end first");
+    if (!text) return fail(e, PE_ERR_INVALID, "pe_calibration_set: null table");
+    const CalibTable want = engine_table(e);
+    std::vector<int> k;
+    std::string err;
+    if (read_calibration_table(text, want, k, err)) return fail(e, PE_ERR_INVALID, "%s", err.c_str());
+    std::vector<float> s = e->conv_scale;
+    size_t j = 0;
+    for (size_t i = 0; i < s.size(); i++)
+        if (e->plan.convs[i].out_act >= 0) s[i] = ldexpf(1.f, k[j++]);
+    return apply_scales(e, s, nullptr);
 }
 
 extern "C" int pe_forward_net_input(pe_engine* e, const float* net_input, int n) {

@@ -54,7 +54,8 @@ _lib = None
 # every symbol include/poseengine.h declares (checked by tests/test_abi.py)
 ABI_SYMBOLS = [
     "pe_create", "pe_destroy", "pe_last_error", "pe_num_conv_layers", "pe_conv_layer_info", "pe_set_conv_weights",
-    "pe_load_weights_file", "pe_commit_weights", "pe_share_weights", "pe_calibrate", "pe_range_status", "pe_nms_get_max_peaks", "pe_nms_get_num_parts", "pe_nms_get_threshold",
+    "pe_load_weights_file", "pe_commit_weights", "pe_share_weights", "pe_calibrate", "pe_range_status", "pe_calibrate_begin", "pe_calibrate_end",
+    "pe_calibration_get", "pe_calibration_set", "pe_nms_get_max_peaks", "pe_nms_get_num_parts", "pe_nms_get_threshold",
     "pe_nms_set_threshold", "pe_resize_set_start_scale", "pe_resize_set_scale_gap", "pe_resize_get_start_scale",
     "pe_resize_get_scale_gap", "pe_set_connect_params", "pe_forward_frames", "pe_forward_frames_device",
     "pe_forward_net_input", "pe_forward_maps", "pe_fetch", "pe_fetch_maps", "pe_fetch_blob", "pe_sync", "pe_write_json",
@@ -96,6 +97,10 @@ def lib():
     L.pe_share_weights.argtypes = [C.c_void_p, C.c_void_p]
     L.pe_calibrate.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int]
     L.pe_range_status.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.c_char_p]
+    L.pe_calibrate_begin.argtypes = [C.c_void_p]
+    L.pe_calibrate_end.argtypes = [C.c_void_p, C.POINTER(C.c_int)]
+    L.pe_calibration_get.argtypes = [C.c_void_p, C.c_char_p, C.c_int]
+    L.pe_calibration_set.argtypes = [C.c_void_p, C.c_char_p]
     L.pe_load_caffemodel.argtypes = [C.c_void_p, C.c_char_p]
     L.pe_caffemodel_open.argtypes = [C.c_char_p, C.POINTER(C.c_void_p)]
     L.pe_caffemodel_close.argtypes = [C.c_void_p]
@@ -470,6 +475,53 @@ class PoseEngine:
         frames = [np.ascontiguousarray(f, np.uint8) for f in frames]
         arr = (C.c_void_p * len(frames))(*[f.ctypes.data for f in frames])
         self._ck(lib().pe_calibrate(self._h, arr, len(frames)))
+
+    def calibrate_begin(self):
+        """pe_calibrate_begin: from now on every forward adds each layer's largest true |output| to a running maximum."""
+        self._ck(lib().pe_calibrate_begin(self._h))
+
+    def calibrate_end(self):
+        """pe_calibrate_end: scales from the maxima collected since calibrate_begin(); returns how many layers' scales moved."""
+        n = C.c_int()
+        self._ck(lib().pe_calibrate_end(self._h, C.byref(n)))
+        return n.value
+
+    def calibration_table(self):
+        """The engine's calibration table as text (pe_calibration_get)."""
+        L = lib()
+        n = L.pe_calibration_get(self._h, None, 0)
+        if n < 0:
+            self._ck(-n)
+        buf = C.create_string_buffer(n + 1)
+        L.pe_calibration_get(self._h, buf, n + 1)
+        return buf.value.decode()
+
+    def set_calibration_table(self, text):
+        """Apply a table of calibration_table() (pe_calibration_set): the scales of the engine it came from, bit for bit."""
+        self._ck(lib().pe_calibration_set(self._h, text.encode()))
+
+    def calibrate_on(self, batches, max_passes=None):
+        """Passes of calibrate_begin(), a forward of every batch, calibrate_end() until a pass changes no scale; returns the number of
+        passes.  batches: lists of uint8 BGR images of one size each; display-size batches go through forward_frames, others through
+        forward_camera_frames.  max_passes defaults to the number of conv layers that store an activation, which bounds the passes
+        (DESIGN.md section 3); reaching it raises."""
+        batches = [list(b) for b in batches]
+        if not batches or any(not b for b in batches):
+            raise ValueError("calibrate_on needs at least one non-empty batch")
+        if max_passes is None:
+            max_passes = sum(1 for l in self.calibration_table().splitlines() if l.startswith("layer "))
+        disp = (self.cfg.disp_h, self.cfg.disp_w, 3)
+        for p in range(1, max_passes + 1):
+            self.calibrate_begin()
+            for b in batches:
+                if all(np.shape(f) == disp for f in b):
+                    self.forward_frames(b)
+                else:
+                    self.forward_camera_frames(b)
+            self.sync()
+            if self.calibrate_end() == 0:
+                return p
+        raise PoseEngineError("calibrate_on: the scales still moved after %d passes" % max_passes)
 
     def range_status(self):
         """(rc, worst |stored value| / the format's largest finite value (fp16 65504, e4m3 448, s8 127), layer name); rc != 0

@@ -104,6 +104,13 @@ static void define_flags() {
            "--batch is automatic: the copies and the kernel tails of one batch overlap the other; weights are shared, not duplicated)");
     define("calibrate_range", "true", "[extension] fp16, e4m3 and s8 modes (--precision 2, 4, 5 and 6): derive per-layer power-of-two activation scales from one synthetic frame at start-up "
            "(pe_calibrate), so that a model of any magnitude keeps fp32-level results; --precision 6 cannot run without them", true);
+    define("calibration_dir", "", "[extension] --precision 2, 4, 5 or 6: after the synthetic-frame calibration of --calibrate_range, calibrate GPU 0's "
+           "engine on the images of this directory (.jpg / .png / .bmp / .ppm of any size, sorted, at most --calibration_frames): passes of "
+           "one forward of every batch each (pe_calibrate_begin / pe_calibrate_end) until a pass changes no layer's scale");
+    define("calibration_frames", "64", "[extension] --calibration_dir: the largest number of images it reads");
+    define("calibration_table", "", "[extension] --precision 2, 4, 5 or 6: apply this calibration table (--save_calibration, pe_calibration_set) "
+           "to GPU 0's engine instead of calibrating; a table of other weights, another precision or other --f16_layers ends start-up");
+    define("save_calibration", "", "[extension] write GPU 0's calibration table (pe_calibration_get) to this file once calibration is done");
     define("audit_every", "0", "[extension] N > 0: every worker also holds a parity-mode (--precision 2) handle and forwards every N-th batch "
            "through it too; each frame's peaks, person count and joints are compared with the fast handle's (within 1e-3 net px). The status "
            "line reports how many frames agree, and a summary is printed at exit. Output stays the --precision handle's. 0 = off");
@@ -703,7 +710,50 @@ static int load_weights(pe_engine* e, int device) {   // CopyTrainedLayersFrom (
 // packs it and the replicas receive the packed buffer by one ncclBroadcast (the path's only collective).
 // engines[g * per_gpu + k] = handle k of GPU g.  Handle 0 of GPU 0 loads the model; handle 0 of the other GPUs receives the packed
 // weights by broadcast; handles k > 0 share their GPU's buffer (Net::ShareTrainedLayersWith).
-static bool create_engines(int num_gpu, int per_gpu, int precision, const std::string& f16_layers, std::vector<pe_engine*>& engines) {
+// --calibration_dir: the decoded images (read before any GPU call)
+struct CalibImage { int w, h; std::vector<uint8_t> bgr; };
+static std::vector<CalibImage> g_calib_images;
+
+static bool ranged_precision(int p) { return p == PE_PREC_F16X2 || p == PE_PREC_F16X1 || p == PE_PREC_E4M3X1 || p == PE_PREC_S8X1; }
+
+static std::string calibration_table_of(pe_engine* e) {
+    const int n = pe_calibration_get(e, nullptr, 0);
+    if (n < 0) return std::string();
+    std::vector<char> buf((size_t)n + 1);
+    pe_calibration_get(e, buf.data(), n + 1);
+    return std::string(buf.data(), (size_t)n);
+}
+
+// --calibration_dir: passes over the images until one changes no scale.  Consecutive images of one size form a batch of at most --batch
+// frames; display-size batches go through pe_forward_frames, the others through pe_forward_camera_frames (warped to the display size).
+static bool calibrate_on_images(pe_engine* e, int dev) {
+    const std::string table = calibration_table_of(e);
+    int max_passes = 0;   // the passes are bounded by the number of ranged layers (DESIGN.md section 3)
+    for (size_t p = table.find("\nlayer "); p != std::string::npos; p = table.find("\nlayer ", p + 1)) max_passes++;
+    if (max_passes == 0) { LOG_ERROR("GPU %d: --calibration_dir: %s", dev, pe_last_error(e)); return false; }
+    for (int pass = 1; pass <= max_passes; pass++) {
+        if (pe_calibrate_begin(e)) { LOG_ERROR("GPU %d: --calibration_dir: %s", dev, pe_last_error(e)); return false; }
+        for (size_t i = 0; i < g_calib_images.size();) {
+            std::vector<const uint8_t*> ptrs;
+            const int w = g_calib_images[i].w, h = g_calib_images[i].h;
+            while (i < g_calib_images.size() && (int)ptrs.size() < global.batch && g_calib_images[i].w == w && g_calib_images[i].h == h)
+                ptrs.push_back(g_calib_images[i++].bgr.data());
+            double scale = 1.0;
+            const int rc = (w == global.disp_w && h == global.disp_h) ? pe_forward_frames(e, ptrs.data(), (int)ptrs.size())
+                                                                     : pe_forward_camera_frames(e, ptrs.data(), (int)ptrs.size(), w, h, &scale);
+            if (rc) { LOG_ERROR("GPU %d: --calibration_dir: forward failed: %s", dev, pe_last_error(e)); return false; }
+        }
+        int changed = 0;
+        if (pe_calibrate_end(e, &changed)) { LOG_ERROR("GPU %d: --calibration_dir: %s", dev, pe_last_error(e)); return false; }
+        LOG_INFO("GPU %d: calibration pass %d over %d images: %d layers changed their scale", dev, pass, (int)g_calib_images.size(), changed);
+        if (changed == 0) return true;
+    }
+    LOG_ERROR("GPU %d: --calibration_dir: the scales still moved after %d passes", dev, max_passes);
+    return false;
+}
+
+static bool create_engines(int num_gpu, int per_gpu, int precision, const std::string& f16_layers, std::vector<pe_engine*>& engines,
+                           bool serving) {
     const int batch = global.batch;
     for (int tid = 0; tid < num_gpu * per_gpu; tid++) {
         pe_config c;
@@ -728,8 +778,31 @@ static bool create_engines(int num_gpu, int per_gpu, int precision, const std::s
         if (pe_calibrate(e, &ptr, 1)) { LOG_ERROR("GPU %d: range calibration failed: %s", dev, pe_last_error(e)); return false; }
         return true;
     };
-    // before the weights are replicated: the scales travel inside the packed buffer
-    if (calibrate && !calibrate_engine(engines[0], Fi("start_device"))) return false;
+    // before the weights are replicated: the scales travel inside the packed buffer.  --calibration_table and --calibration_dir are
+    // for the engines that serve frames; the --audit_every parity handles keep their own synthetic-frame calibration.
+    if (serving && !F("calibration_table").empty()) {
+        std::ifstream f(F("calibration_table"));
+        const std::string text((std::istreambuf_iterator<char>(f)), std::istreambuf_iterator<char>());
+        if (!f || pe_calibration_set(engines[0], text.c_str())) {
+            LOG_ERROR("--calibration_table %s: %s", F("calibration_table").c_str(), f ? pe_last_error(engines[0]) : "cannot read the file");
+            return false;
+        }
+        LOG_INFO("GPU %d: calibration table %s applied", Fi("start_device"), F("calibration_table").c_str());
+    } else if (calibrate && !calibrate_engine(engines[0], Fi("start_device"))) {
+        return false;
+    }
+    if (serving && !g_calib_images.empty() && !calibrate_on_images(engines[0], Fi("start_device"))) return false;
+    if (serving && !F("save_calibration").empty()) {
+        const std::string table = calibration_table_of(engines[0]);
+        FILE* f = table.empty() ? nullptr : fopen(F("save_calibration").c_str(), "w");
+        const bool ok = f && fwrite(table.data(), 1, table.size(), f) == table.size();
+        if (f && fclose(f)) f = nullptr;
+        if (!ok || !f) {
+            LOG_ERROR("--save_calibration %s: %s", F("save_calibration").c_str(), table.empty() ? pe_last_error(engines[0]) : "cannot write the file");
+            return false;
+        }
+        LOG_INFO("GPU %d: calibration table written to %s", Fi("start_device"), F("save_calibration").c_str());
+    }
     if (num_gpu > 1) {
         std::vector<pe_engine*> firsts;
         for (int g = 0; g < num_gpu; g++) firsts.push_back(engines[g * per_gpu]);
@@ -738,9 +811,22 @@ static bool create_engines(int num_gpu, int per_gpu, int precision, const std::s
                      pe_packed_weights_bytes(engines[0]) / 1e6);
         } else {
             LOG_ERROR("weight broadcast unavailable (%s); every GPU loads the model itself", pe_last_error(engines[0]));
+            // every GPU computes what GPU 0 computes, in every mode with range scales: scales that came from --calibration_table or
+            // --calibration_dir reach the other GPUs' first engines as engine 0's calibration table; the synthetic-frame calibration is
+            // repeated on each GPU (the same frame and weights give the same scales).  Otherwise all run at scale 1, like engine 0.
+            const bool own_table = serving && ranged_precision(precision) && (!F("calibration_table").empty() || !g_calib_images.empty());
+            const std::string table = own_table ? calibration_table_of(engines[0]) : std::string();
+            if (own_table && table.empty()) { LOG_ERROR("GPU %d: %s", Fi("start_device"), pe_last_error(engines[0])); return false; }
             for (int g = 1; g < num_gpu; g++) {
                 if (load_weights(engines[g * per_gpu], Fi("start_device") + g)) return false;
-                if (calibrate && precision == PE_PREC_S8X1 && !calibrate_engine(engines[g * per_gpu], Fi("start_device") + g)) return false;
+                if (own_table) {
+                    if (pe_calibration_set(engines[g * per_gpu], table.c_str())) {
+                        LOG_ERROR("GPU %d: calibration table of GPU %d: %s", Fi("start_device") + g, Fi("start_device"), pe_last_error(engines[g * per_gpu]));
+                        return false;
+                    }
+                } else if (calibrate && !calibrate_engine(engines[g * per_gpu], Fi("start_device") + g)) {
+                    return false;
+                }
             }
         }
     }
@@ -1126,6 +1212,38 @@ int main(int argc, char** argv) {
         LOG_ERROR("--precision 6 (INT8) runs on calibrated per-layer range scales: at scale 1 almost every activation quantises to 0; drop --nocalibrate_range");
         return 1;
     }
+    if ((!F("calibration_dir").empty() || !F("calibration_table").empty() || !F("save_calibration").empty()) && !ranged_precision(Fi("precision"))) {
+        LOG_ERROR("--calibration_dir, --calibration_table and --save_calibration are for the modes with range scales: --precision 2, 4, 5 or 6");
+        return 1;
+    }
+    if (!F("calibration_table").empty() && !F("calibration_dir").empty()) {
+        LOG_ERROR("--calibration_table applies saved scales instead of calibrating: it does not combine with --calibration_dir");
+        return 1;
+    }
+    if (!F("calibration_table").empty() && !Fb("calibrate_range")) {
+        LOG_ERROR("--calibration_table sets the range scales: it does not combine with --nocalibrate_range");
+        return 1;
+    }
+    if (!F("calibration_dir").empty()) {   // decoded before any GPU call: an empty or undecodable directory ends start-up here
+        if (Fi("calibration_frames") < 1) { LOG_ERROR("--calibration_frames must be at least 1"); return 1; }
+        DIR* d = opendir(F("calibration_dir").c_str());
+        if (!d) { LOG_ERROR("--calibration_dir: folder %s does not exist", F("calibration_dir").c_str()); return 1; }
+        std::vector<std::string> files;
+        while (dirent* ent = readdir(d)) {
+            const std::string n = ent->d_name, le = lower_ext(n);
+            if (le == ".jpg" || le == ".png" || le == ".bmp" || le == ".jpeg" || le == ".ppm") files.push_back(F("calibration_dir") + "/" + n);
+        }
+        closedir(d);
+        std::sort(files.begin(), files.end());
+        if ((int)files.size() > Fi("calibration_frames")) files.resize(Fi("calibration_frames"));
+        if (files.empty()) { LOG_ERROR("--calibration_dir %s holds no .jpg / .png / .bmp / .ppm image", F("calibration_dir").c_str()); return 1; }
+        for (const std::string& p : files) {
+            CalibImage im;
+            if (!read_image(p, im.w, im.h, im.bgr)) { LOG_ERROR("--calibration_dir: cannot decode %s (supported: .jpg, .png, 24-bit .bmp, P6 .ppm)", p.c_str()); return 1; }
+            g_calib_images.push_back(std::move(im));
+        }
+        LOG_INFO("--calibration_dir: %d images", (int)g_calib_images.size());
+    }
     if (!F("f16_layers").empty() && Fi("precision") != PE_PREC_E4M3X1 && Fi("precision") != PE_PREC_S8X1) {
         LOG_ERROR("--f16_layers runs chosen layers in fp16 inside the FP8 or INT8 mode: it needs --precision 5 or 6");
         return 1;
@@ -1203,8 +1321,8 @@ int main(int argc, char** argv) {
     const int num_gpu = std::max(1, Fi("num_gpu"));
     std::vector<pe_engine*> engines, audit;
     const int per_gpu = global.engines_per_gpu, num_workers = num_gpu * per_gpu;
-    if (!create_engines(num_gpu, per_gpu, Fi("precision"), F("f16_layers"), engines) ||
-        (Fi("audit_every") > 0 && !create_engines(num_gpu, per_gpu, PE_PREC_F16X2, "", audit))) {
+    if (!create_engines(num_gpu, per_gpu, Fi("precision"), F("f16_layers"), engines, true) ||
+        (Fi("audit_every") > 0 && !create_engines(num_gpu, per_gpu, PE_PREC_F16X2, "", audit, false))) {
         for (pe_engine* e : engines) pe_destroy(e);
         for (pe_engine* e : audit) pe_destroy(e);
         return 1;

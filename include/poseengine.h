@@ -148,6 +148,30 @@ int pe_commit_weights(pe_engine* e);
  * pe_fetch(idx 0) performs this check, so range problems are errors instead of silent inf / zeros. */
 int pe_calibrate(pe_engine* e, const uint8_t* const* frames, int n);
 int pe_range_status(pe_engine* e, float* worst_ratio, char* layer64);
+/* Calibration over a set of frames of any size, through any input route (DESIGN.md section 3).  pe_calibrate_begin starts a
+ * collection: from then on every forward of `e` adds each layer's largest true |output| to a per-layer running maximum (range
+ * maxima recorded before begin do not count; pe_range_status and PE_CHECK_RANGE keep working and lose nothing).  pe_calibrate_end
+ * sets every layer's scale from the collected maxima with pe_calibrate's rule (a layer whose maximum is 0 keeps its scale), re-packs
+ * what the new scales change, clears the range state and writes the number of layers whose scale moved to *changed.  A pass is
+ * begin, a forward of every batch of the set, end; repeat passes until *changed is 0.  The first p ranged layers are final after
+ * pass p (each layer's input depends only on the layers before it), so a set converges in at most as many passes as the net has
+ * ranged conv layers, in one or two when the starting scales were roughly right; the result is the table pe_calibrate would give on
+ * the whole set as one batch.
+ * pe_calibration_get writes the engine's calibration table as text (precision, an FNV-1a 64 hash of the conv layers' names and fp32
+ * weights and biases, then "layer <name> <stored kind> <log2 scale>" per conv layer that stores an activation) and returns its
+ * length; with buf NULL (or cap too small) it writes nothing.  -PE_ERR_* on error.  pe_calibration_set applies such a table: the
+ * engine then computes bit for bit what the engine the table came from computes; it replaces the pe_calibrate that PE_PREC_S8X1
+ * needs.  The table does not record the net size or the scale count: a table calibrated at 656x368 applies at 992x736.  It refuses
+ * (PE_ERR_INVALID, pe_last_error names the line or layer) another version or precision, other weights, a missing, repeated,
+ * reordered or unknown layer, another stored kind (another f16_layers list), an exponent outside [-100, 100] and trailing text.
+ * All four work on the handle that owns the weights, before pe_share_weights / pe_broadcast_weights: a receiving handle, or an
+ * owner whose weights are already shared, gets PE_ERR_STATE.  Modes without range scales (0, 1, 3): PE_ERR_INVALID.  Also
+ * PE_ERR_STATE: begin on a PE_PREC_S8X1 engine never calibrated, end without a forward since begin, and pe_calibrate,
+ * pe_calibration_set or pe_commit_weights during a collection.  pe_commit_weights resets the calibration. */
+int pe_calibrate_begin(pe_engine* e);
+int pe_calibrate_end(pe_engine* e, int* changed);
+int pe_calibration_get(const pe_engine* e, char* buf, int cap);
+int pe_calibration_set(pe_engine* e, const char* text);
 /* Net::ShareTrainedLayersWith (net.cpp:682-706): `to` - another handle on the SAME GPU running the same net - uses `from`'s
  * committed weights (the packed device buffer is shared, not copied, and lives until its last user is destroyed). */
 int pe_share_weights(pe_engine* from, pe_engine* to);
