@@ -51,10 +51,9 @@ struct pe_engine {
     // packed weights (one device buffer): per conv offsets (bytes)
     void* d_packed = nullptr; size_t packed_bytes = 0;
     std::shared_ptr<void> packed_owner;   // frees d_packed when the last handle using it goes (pe_share_weights)
-    // range management of the fp16 and e4m3 modes (F16X2, F16X1, E4M3X1): per-conv-output power-of-two scale s (stored value = true value * s), the true
-    // biases / weight-scale inverses the packed epilogue fields derive from, and the kernels' running max |stored value| per conv
+    // range management of the fp16 and e4m3 modes (F16X2, F16X1, E4M3X1): per-conv-output power-of-two scale s (stored value = true value * s), the
+    // weight-scale inverses the packed epilogue fields derive from (with the true biases hw[i].b), and the kernels' running max |stored value| per conv
     std::vector<float> conv_scale, wsi;   // per conv: scale of its stored output; inverse of the power of two folded into its weights
-    std::vector<std::vector<float>> bias_true;
     std::vector<std::vector<float>> wsig;   // S8X1: per conv, the per-output-channel weight step sigma_c of pack_conv_weights (s8.h)
     unsigned* d_range = nullptr;
     bool calibrated = false, check_range = false;
@@ -78,7 +77,7 @@ struct pe_engine {
     int last_lane1_conv = -1;
     cudaEvent_t ev[16] = {};
     uint8_t* d_frames = nullptr; uint8_t* d_resized = nullptr;
-    uint8_t* h_frames = nullptr;    // pinned staging
+    uint8_t* h_frames = nullptr; size_t h_frames_cap = 0;   // pinned staging for pageable frames (upload_host)
     float* d_planar = nullptr; float* h_planar = nullptr;
     std::vector<void*> d_tabs;
     PreArgs pre;
@@ -483,7 +482,6 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, const
     // io buffers
     const size_t frame_bytes = (size_t)cfg->disp_w * cfg->disp_h * 3;
     CKC(cudaMalloc(&e->d_frames, frame_bytes * cfg->max_batch));
-    CKC(cudaMallocHost(&e->h_frames, frame_bytes * cfg->max_batch));
     CKC(cudaMalloc(&e->d_resized, (size_t)N * cfg->net_w * cfg->net_h * 3));
     const size_t planar_n = (size_t)N * 3 * cfg->net_w * cfg->net_h;
     CKC(cudaMalloc(&e->d_planar, planar_n * sizeof(float)));
@@ -675,6 +673,16 @@ static size_t packed_layout(pe_engine* e) {
 // bias = true bias * s_out - all factors powers of two, hence exact, and ReLU commutes with them: range scaling is free at run time.
 // S8X1 replaces 2^k by a step per output channel (sigma_c, s8.h): acc * sigma_c ~ s_ref * sum w a, and the factor of channel c
 // is f_c = sigma_c * s_out / s_ref.  The net input carries the mode's net_input_scale.
+//
+// The one rule that picks those powers of two (range scales and the weights' 2^k): the s that puts a maximum m into
+// [2^(top-1), 2^top), exponent clamped to [-100, 100]; `otherwise` when m says nothing (0, infinite or NaN).
+static float pow2_for(float m, int top, float otherwise = 1.f) {
+    if (!(m > 0.f && m < 3e38f)) return otherwise;
+    int ex = 0;
+    frexpf(m, &ex);
+    return ldexpf(1.f, std::max(-100, std::min(100, top - ex)));
+}
+static int log2_of_scale(float s) { int ex = 0; frexpf(s, &ex); return ex - 1; }
 static float input_ref_scale(const pe_engine* e, const ConvSpec& c) {
     for (int pc : c.cin_prod) if (pc >= 0) return e->conv_scale[pc];
     return elem_row(*e->prec, (PlaneElem)e->plan.acts[c.in_act].elem).net_input_scale;   // the net input
@@ -683,7 +691,7 @@ static void fill_epilogue_fields(const pe_engine* e, int i, float* B) {
     const ConvSpec& c = e->plan.convs[i];
     const float s_ref = input_ref_scale(e, c);
     const float s_out = c.out_act >= 0 ? e->conv_scale[i] : 1.f;   // the planar stride-8 maps are true values
-    for (int co = 0; co < c.cout; co++) B[co] = e->bias_true[i][co] * s_out;
+    for (int co = 0; co < c.cout; co++) B[co] = e->hw[i].b[co] * s_out;
     if (conv_row(e, i).per_channel_epilogue) {
         for (int co = 0; co < c.cout; co++) B[e->cout_pad[i] + co] = e->wsig[i][co] * (s_out / s_ref);
         return;
@@ -738,8 +746,7 @@ static void pack_conv_weights(pe_engine* e, int i, uint8_t* dst) {
             float mx = 0.f;
             for (int co = 0; co < c.cout; co++)
                 for (size_t kk = 0; kk < K; kk++) mx = fmaxf(mx, fabsf(src(co, (int)kk)));
-            int ex = 0;
-            if (mx > 0.f && mx < 3e38f) { frexpf(mx, &ex); wscale = ldexpf(1.f, std::max(-100, std::min(100, top - ex))); }
+            wscale = pow2_for(mx, top);
         }
         wscale_inv = 1.f / wscale;
         if (wf.e4m3()) {   // one byte per weight, [cout_pad][K]
@@ -807,7 +814,6 @@ extern "C" int pe_commit_weights(pe_engine* e) {
                         e->committed ? " on this handle (a broadcast replica keeps no fp32 copy: set every layer again)" : "");
     }
     const size_t total = packed_layout(e);
-    e->bias_true.assign(nc, std::vector<float>());
     e->calibrated = false;
     e->wsi.assign(nc, 1.f);
     e->wsig.assign(nc, std::vector<float>());
@@ -815,7 +821,6 @@ extern "C" int pe_commit_weights(pe_engine* e) {
     std::vector<uint8_t> host(total, 0);
     for (size_t i = 0; i < nc; i++) {
         pack_conv_weights(e, (int)i, host.data() + e->w_off[i]);
-        e->bias_true[i] = e->hw[i].b;
         fill_epilogue_fields(e, (int)i, (float*)(host.data() + e->b_off[i]));   // travels with the packed buffer (weight broadcast)
     }
     e->packed_owner.reset();
@@ -851,7 +856,7 @@ extern "C" int pe_share_weights(pe_engine* from, pe_engine* to) {
     to->d_packed = from->d_packed;
     to->packed_bytes = from->packed_bytes;
     for (auto& h : to->hw) { std::vector<float>().swap(h.w); std::vector<float>().swap(h.b); h.set = false; }
-    to->conv_scale = from->conv_scale; to->calibrated = from->calibrated; to->bias_true.clear();
+    to->conv_scale = from->conv_scale; to->calibrated = from->calibrated;
     return bind_packed(to);
 }
 
@@ -1143,43 +1148,69 @@ static int check_n(pe_engine* e, int n) {
     return PE_OK;
 }
 
-extern "C" int pe_forward_frames_device(pe_engine* e, const void* d_frames, int n) {
-    NvtxRange r("pe_forward_frames_device");
-    int rc = check_n(e, n); if (rc) return rc;
-    CK(e, cudaSetDevice(e->cfg.device));
+// (re)allocates *p to hold at least `need` bytes; the stream is drained first because queued work may still use the old buffer
+static int grow_buffer(pe_engine* e, uint8_t** p, size_t* cap, size_t need, bool host) {
+    if (*cap >= need) return PE_OK;
+    CK(e, cudaStreamSynchronize(e->stream));
+    if (host) { cudaFreeHost(*p); *p = nullptr; CK(e, cudaMallocHost((void**)p, need)); }
+    else { cudaFree(*p); *p = nullptr; CK(e, cudaMalloc((void**)p, need)); }
+    *cap = need;
+    return PE_OK;
+}
+
+// n host buffers (bytes[i] bytes from src[i]) to dst + i * stride.  Every pointer is checked before anything is copied.  When all are
+// page-locked (pe_host_alloc) they are DMA'd directly, fully asynchronously; otherwise they go through the pinned staging buffer
+// *staging in one copy of stride * n bytes, which drains the stream first because queued work may still read that buffer.
+static int upload_host(pe_engine* e, const void* const* src, const std::vector<size_t>& bytes, int n, size_t stride, uint8_t* dst,
+                       uint8_t** staging, size_t* staging_cap, const char* what) {
+    bool pinned = true;
+    for (int i = 0; i < n; i++) {
+        if (!src[i]) return fail(e, PE_ERR_INVALID, "null %s %d", what, i);
+        cudaPointerAttributes at;
+        if (pinned && (cudaPointerGetAttributes(&at, src[i]) != cudaSuccess || at.type != cudaMemoryTypeHost)) { pinned = false; cudaGetLastError(); }
+    }
+    if (pinned) {
+        for (int i = 0; i < n; i++) CK(e, cudaMemcpyAsync(dst + i * stride, src[i], bytes[i], cudaMemcpyHostToDevice, e->stream));
+        return PE_OK;
+    }
+    CK(e, cudaStreamSynchronize(e->stream));
+    int rc = grow_buffer(e, staging, staging_cap, stride * n, true); if (rc) return rc;
+    for (int i = 0; i < n; i++) memcpy(*staging + i * stride, src[i], bytes[i]);
+    CK(e, cudaMemcpyAsync(dst, *staging, stride * n, cudaMemcpyHostToDevice, e->stream));
+    return PE_OK;
+}
+
+// n display frames in device memory -> the net input
+static int preprocess_frames(pe_engine* e, const uint8_t* d_frames, int n) {
     PreArgs a = e->pre;
-    a.frames = (const uint8_t*)d_frames; a.nframes = n;
+    a.frames = d_frames; a.nframes = n;
     if (e->input_lo_dirty) {   // the uint8 path only writes the hi plane; drop what the planar path left behind
         const size_t bytes = (size_t)e->act_plane[e->plan.input_act] * fmt_bytes(act_fmt(e, e->plan.input_act));
         CK(e, cudaMemsetAsync(e->acts[e->plan.input_act], 0, bytes, e->stream));
         e->input_lo_dirty = false;
     }
     e->launches += launch_preprocess(a, e->stream);
-    e->last_frames = (const uint8_t*)d_frames;
+    e->last_frames = d_frames;
+    return PE_OK;
+}
+extern "C" int pe_forward_frames_device(pe_engine* e, const void* d_frames, int n) {
+    NvtxRange r("pe_forward_frames_device");
+    int rc = check_n(e, n); if (rc) return rc;
+    CK(e, cudaSetDevice(e->cfg.device));
+    if ((rc = preprocess_frames(e, (const uint8_t*)d_frames, n))) return rc;
     return run_net(e, n);
+}
+// n display frames in host memory -> e->d_frames
+static int upload_frames(pe_engine* e, const uint8_t* const* frames, int n) {
+    if (!frames) return fail(e, PE_ERR_INVALID, "null frames");
+    const size_t fb = (size_t)e->cfg.disp_w * e->cfg.disp_h * 3;
+    return upload_host(e, (const void* const*)frames, std::vector<size_t>(n, fb), n, fb, e->d_frames, &e->h_frames, &e->h_frames_cap, "frame");
 }
 extern "C" int pe_forward_frames(pe_engine* e, const uint8_t* const* frames, int n) {
     NvtxRange r("pe_forward_frames (H2D)");
     int rc = check_n(e, n); if (rc) return rc;
-    if (!frames) return fail(e, PE_ERR_INVALID, "null frames");
     CK(e, cudaSetDevice(e->cfg.device));
-    const size_t fb = (size_t)e->cfg.disp_w * e->cfg.disp_h * 3;
-    // Page-locked caller buffers are DMA'd directly (fully asynchronous); pageable ones go through the
-    // engine's pinned staging buffer, which forces a stream sync because that buffer is reused.
-    bool pinned = true;
-    for (int i = 0; i < n && pinned; i++) {
-        cudaPointerAttributes at;
-        if (!frames[i]) return fail(e, PE_ERR_INVALID, "null frame %d", i);
-        if (cudaPointerGetAttributes(&at, frames[i]) != cudaSuccess || at.type != cudaMemoryTypeHost) { pinned = false; cudaGetLastError(); }
-    }
-    if (pinned) {
-        for (int i = 0; i < n; i++)
-            CK(e, cudaMemcpyAsync(e->d_frames + i * fb, frames[i], fb, cudaMemcpyHostToDevice, e->stream));
-    } else {
-        CK(e, cudaStreamSynchronize(e->stream));
-        for (int i = 0; i < n; i++) memcpy(e->h_frames + i * fb, frames[i], fb);
-        CK(e, cudaMemcpyAsync(e->d_frames, e->h_frames, fb * n, cudaMemcpyHostToDevice, e->stream));
-    }
+    if ((rc = upload_frames(e, frames, n))) return rc;
     return pe_forward_frames_device(e, e->d_frames, n);
 }
 // bicubic weight table of OpenCV's fixed-point remap (initInterTab2D(INTER_CUBIC, fixpt)): a = -0.75, 15-bit shorts,
@@ -1243,16 +1274,6 @@ static int prepare_warp(pe_engine* e, int ow, int oh) {
     CK(e, cudaMemcpy(e->d_wx0, x0.data(), dh * sizeof(int), cudaMemcpyHostToDevice));
     CK(e, cudaMemcpy(e->d_wy0, y0.data(), dh * sizeof(int), cudaMemcpyHostToDevice));
     e->warp_w = ow; e->warp_h = oh; e->warp_scale = s;
-    return PE_OK;
-}
-
-// (re)allocates *p to hold at least `need` bytes; the stream is drained first because queued work may still use the old buffer
-static int grow_buffer(pe_engine* e, uint8_t** p, size_t* cap, size_t need, bool host) {
-    if (*cap >= need) return PE_OK;
-    CK(e, cudaStreamSynchronize(e->stream));
-    if (host) { cudaFreeHost(*p); *p = nullptr; CK(e, cudaMallocHost((void**)p, need)); }
-    else { cudaFree(*p); *p = nullptr; CK(e, cudaMalloc((void**)p, need)); }
-    *cap = need;
     return PE_OK;
 }
 
@@ -1367,7 +1388,7 @@ extern "C" int pe_forward_jpeg_coefs(pe_engine* e, const void* const* coefs, int
     // the kernels index with the headers' numbers: every header must be one pe_jpeg_read_coefs writes, all frames one size
     int W = 0, H = 0;
     long long max_bytes = 0, max_blocks = 0;
-    std::vector<long long> bytes(n);
+    std::vector<size_t> bytes(n);
     for (int i = 0; i < n; i++) {
         if (!coefs[i]) return fail(e, PE_ERR_INVALID, "null coefficient image %d", i);
         pe_jpeg_coef_header hd;
@@ -1382,20 +1403,7 @@ extern "C" int pe_forward_jpeg_coefs(pe_engine* e, const void* const* coefs, int
     }
     const size_t stride = ((size_t)max_bytes + 255) & ~(size_t)255;
     rc = grow_buffer(e, &e->d_jcoef, &e->jcoef_cap, stride * n, false); if (rc) return rc;
-    // page-locked caller buffers (pe_host_alloc) are DMA'd directly; pageable ones are staged, which drains the stream
-    bool pinned = true;
-    for (int i = 0; i < n && pinned; i++) {
-        cudaPointerAttributes at;
-        if (cudaPointerGetAttributes(&at, coefs[i]) != cudaSuccess || at.type != cudaMemoryTypeHost) { pinned = false; cudaGetLastError(); }
-    }
-    if (pinned) {
-        for (int i = 0; i < n; i++) CK(e, cudaMemcpyAsync(e->d_jcoef + i * stride, coefs[i], bytes[i], cudaMemcpyHostToDevice, e->stream));
-    } else {
-        CK(e, cudaStreamSynchronize(e->stream));
-        rc = grow_buffer(e, &e->h_jcoef, &e->h_jcoef_cap, stride * n, true); if (rc) return rc;
-        for (int i = 0; i < n; i++) memcpy(e->h_jcoef + i * stride, coefs[i], bytes[i]);
-        CK(e, cudaMemcpyAsync(e->d_jcoef, e->h_jcoef, stride * n, cudaMemcpyHostToDevice, e->stream));
-    }
+    rc = upload_host(e, coefs, bytes, n, stride, e->d_jcoef, &e->h_jcoef, &e->h_jcoef_cap, "coefficient image"); if (rc) return rc;
     return reconstruct_and_forward(e, n, W, H, stride, max_blocks, scale);
 }
 
@@ -1418,7 +1426,7 @@ static int decode_scans(pe_engine* e, const void* const* scans, int n, int S, in
     if (!scans) return fail(e, PE_ERR_INVALID, "null scan images");
     if (S < 8 || S > (1 << 30)) return fail(e, PE_ERR_INVALID, "subsequence length %d bits outside [8, 2^30]", S);
     long long max_scan = 0, max_coef = 0, max_seg = 0, max_sub = 0;
-    std::vector<long long> bytes(n);
+    std::vector<size_t> bytes(n);
     for (int i = 0; i < n; i++) {
         if (!scans[i]) return fail(e, PE_ERR_INVALID, "null scan image %d", i);
         const pe_jpeg_scan_header& hd = *(const pe_jpeg_scan_header*)scans[i];
@@ -1444,19 +1452,7 @@ static int decode_scans(pe_engine* e, const void* const* scans, int n, int S, in
     rc = grow_buffer(e, &e->d_jscan, &e->jscan_cap, sstride * n, false); if (rc) return rc;
     rc = grow_buffer(e, &e->d_jwork, &e->jwork_cap, tab_b + seg_b + pub_b + flag_b + 2 * small_b, false); if (rc) return rc;
     rc = grow_buffer(e, &e->h_jstatus, &e->h_jstatus_cap, (size_t)4 * e->cfg.max_batch, true); if (rc) return rc;
-    bool pinned = true;   // page-locked caller buffers (pe_host_alloc) are DMA'd directly; pageable ones are staged, which drains the stream
-    for (int i = 0; i < n && pinned; i++) {
-        cudaPointerAttributes at;
-        if (cudaPointerGetAttributes(&at, scans[i]) != cudaSuccess || at.type != cudaMemoryTypeHost) { pinned = false; cudaGetLastError(); }
-    }
-    if (pinned) {
-        for (int i = 0; i < n; i++) CK(e, cudaMemcpyAsync(e->d_jscan + i * sstride, scans[i], bytes[i], cudaMemcpyHostToDevice, e->stream));
-    } else {
-        CK(e, cudaStreamSynchronize(e->stream));
-        rc = grow_buffer(e, &e->h_jscan, &e->h_jscan_cap, sstride * n, true); if (rc) return rc;
-        for (int i = 0; i < n; i++) memcpy(e->h_jscan + i * sstride, scans[i], bytes[i]);
-        CK(e, cudaMemcpyAsync(e->d_jscan, e->h_jscan, sstride * n, cudaMemcpyHostToDevice, e->stream));
-    }
+    rc = upload_host(e, scans, bytes, n, sstride, e->d_jscan, &e->h_jscan, &e->h_jscan_cap, "scan image"); if (rc) return rc;
     CK(e, cudaMemsetAsync(e->d_jcoef, 0, *cstride * n, e->stream));
     JpegScanArgs a;
     a.scans = e->d_jscan; a.scan_stride = (long long)sstride;
@@ -1535,53 +1531,66 @@ static int upload_weights(pe_engine* e, int i) {   // re-pack layer i with the c
     return PE_OK;
 }
 
+// Brings conv i's region of the packed buffer up to conv_scale: re-packs its weights when a producer's scale differs from
+// `packed_with`, the scales they were packed with (the bytes depend only on the ratios of those scales), then rewrites its
+// epilogue fields.
+static int refresh_layer(pe_engine* e, int i, const std::vector<float>& packed_with) {
+    for (int pc : e->plan.convs[i].cin_prod)
+        if (pc >= 0 && e->conv_scale[pc] != packed_with[pc]) {
+            const int rc = upload_weights(e, i); if (rc) return rc;
+            break;
+        }
+    return upload_fields(e, i);
+}
+
+// The handle holds the fp32 weights of every layer (pe_set_conv_weights); a share receiver and a broadcast replica do not.
+static bool owns_weights(const pe_engine* e) {
+    return std::all_of(e->hw.begin(), e->hw.end(), [](const HostWeights& h) { return h.set; });
+}
+
+// The calls that change the scales re-pack and rewrite the packed buffer from the fp32 weights, so they need those weights and a
+// buffer no other handle uses (a sharer would keep the old scales).
+static int calib_owner_check(pe_engine* e, const char* what) {
+    if (!e->committed) return fail(e, PE_ERR_STATE, "%s: pe_commit_weights has not been called", what);
+    if (!e->prec->ranged()) return fail(e, PE_ERR_INVALID, "%s: precision %d has no range scales (only 2, 4, 5 and 6 have)", what, e->cfg.precision);
+    if (!owns_weights(e))
+        return fail(e, PE_ERR_STATE, "%s: this handle received its weights by broadcast / sharing: calibrate the source handle, which owns them", what);
+    if (e->packed_owner.use_count() > 1)
+        return fail(e, PE_ERR_STATE, "%s: this handle already shares its weights with another handle, which would keep the old scales: "
+                    "calibrate before pe_share_weights", what);
+    return PE_OK;
+}
+
 extern "C" int pe_calibrate(pe_engine* e, const uint8_t* const* frames, int n) {
     int rc = check_n(e, n); if (rc) return rc;
     if (!frames) return fail(e, PE_ERR_INVALID, "null frames");
-    if (!e->committed) return fail(e, PE_ERR_STATE, "pe_commit_weights has not been called");
-    if (!e->prec->ranged()) return PE_OK;   // fp32 / bf16 modes have fp32's exponent range
+    if (e->committed && !e->prec->ranged()) return PE_OK;   // fp32 / bf16 modes have fp32's exponent range
+    if ((rc = calib_owner_check(e, "pe_calibrate"))) return rc;
     if (e->collecting) return fail(e, PE_ERR_STATE, "a calibration collection is running: call pe_calibrate_end first");
-    const size_t nc = e->plan.convs.size();
-    if (e->bias_true.size() != nc || e->bias_true[0].empty() || e->hw[0].w.empty())
-        return fail(e, PE_ERR_STATE, "this handle received its weights by broadcast / sharing: calibrate the source handle before replicating");
     CK(e, cudaSetDevice(e->cfg.device));
     drop_graphs(e);
-    // frames -> device -> net input
-    const size_t fb = (size_t)e->cfg.disp_w * e->cfg.disp_h * 3;
-    CK(e, cudaStreamSynchronize(e->stream));
-    for (int i = 0; i < n; i++) { if (!frames[i]) return fail(e, PE_ERR_INVALID, "null frame %d", i); memcpy(e->h_frames + i * fb, frames[i], fb); }
-    CK(e, cudaMemcpyAsync(e->d_frames, e->h_frames, fb * n, cudaMemcpyHostToDevice, e->stream));
-    PreArgs a = e->pre;
-    a.frames = e->d_frames; a.nframes = n;
-    e->launches += launch_preprocess(a, e->stream);
-    e->last_frames = e->d_frames;
+    if ((rc = upload_frames(e, frames, n)) || (rc = preprocess_frames(e, e->d_frames, n))) return rc;
+    const std::vector<float> packed_with = e->conv_scale;
     const int nimg = n * e->cfg.num_scales;
     for (const OpRef& op : e->plan.order) {
         if (op.type != 0) { if ((rc = run_op(e, op, nimg))) return rc; continue; }
         const int i = op.idx;
-        const ConvSpec& c = e->plan.convs[i];
-        // the producers of this layer's input are final: fold their scales into the weights if they are not all equal to what is packed
-        bool mixed = false;
-        const float s_ref = input_ref_scale(e, c);
-        for (int pc : c.cin_prod) if (pc >= 0 && e->conv_scale[pc] != s_ref) mixed = true;
-        if (mixed || e->calibrated) { if ((rc = upload_weights(e, i))) return rc; }
-        if (c.out_act >= 0) {
-            e->conv_scale[i] = 1.f;               // measure the true output range: fp32 epilogue values, before the fp16 split
-            if ((rc = upload_fields(e, i))) return rc;
+        const bool stores = e->plan.convs[i].out_act >= 0;
+        if (stores) e->conv_scale[i] = 1.f;   // measure the true output range: fp32 epilogue values, before the fp16 split
+        if ((rc = refresh_layer(e, i, packed_with))) return rc;   // its producers are final (plan order)
+        if (stores) {
             CK(e, cudaMemsetAsync(e->d_range + i, 0, sizeof(unsigned), e->stream));
             if ((rc = run_op(e, op, nimg))) return rc;
             unsigned bits = 0;
             CK(e, cudaMemcpyAsync(&bits, e->d_range + i, sizeof bits, cudaMemcpyDeviceToHost, e->stream));
             CK(e, cudaStreamSynchronize(e->stream));
             float m; memcpy(&m, &bits, 4);
-            // m * s in [2^(range_top-1), 2^range_top) of the stored kind's row (precision.h)
-            const int top = out_row(e, i).range_top;
-            if (m > 0.f && m < 3e38f) { int ex = 0; frexpf(m, &ex); e->conv_scale[i] = ldexpf(1.f, std::max(-100, std::min(100, top - ex))); }
+            e->conv_scale[i] = pow2_for(m, out_row(e, i).range_top);
+            if ((rc = upload_fields(e, i))) return rc;
         }
-        if ((rc = upload_fields(e, i))) return rc;
         if ((rc = run_op(e, op, nimg))) return rc;
     }
-    CK(e, cudaMemsetAsync(e->d_range, 0, nc * sizeof(unsigned), e->stream));
+    CK(e, cudaMemsetAsync(e->d_range, 0, e->plan.convs.size() * sizeof(unsigned), e->stream));
     e->calibrated = true;
     return run_post_and_return(e, n);
 }
@@ -1646,18 +1655,6 @@ extern "C" int pe_range_status(pe_engine* e, float* worst_ratio, char* layer64) 
 // those maxima, divided by the layer's scale, into per-layer running maxima, and pe_calibrate_end sets the scales from them with
 // pe_calibrate's rule.  A table carries the scales to another engine with the same weights.
 // ---------------------------------------------------------------------------------------------
-static int calib_owner_check(pe_engine* e, const char* what) {
-    if (!e->committed) return fail(e, PE_ERR_STATE, "%s: pe_commit_weights has not been called", what);
-    if (!e->prec->ranged()) return fail(e, PE_ERR_INVALID, "%s: precision %d has no range scales (only 2, 4, 5 and 6 have)", what, e->cfg.precision);
-    const size_t nc = e->plan.convs.size();
-    if (e->bias_true.size() != nc || e->bias_true[0].empty() || e->hw[0].w.empty())
-        return fail(e, PE_ERR_STATE, "%s: this handle received its weights by broadcast / sharing: calibrate the handle that owns them", what);
-    if (e->packed_owner.use_count() > 1)
-        return fail(e, PE_ERR_STATE, "%s: this handle already shares its weights with another handle, which would keep the old scales: "
-                    "calibrate before pe_share_weights", what);
-    return PE_OK;
-}
-
 // The engine's table: every conv layer that stores an activation, with its stored kind and log2 scale
 static CalibTable engine_table(pe_engine* e) {
     CalibTable t;
@@ -1676,9 +1673,7 @@ static CalibTable engine_table(pe_engine* e) {
     t.weights = e->weights_hash;
     for (size_t i = 0; i < e->plan.convs.size(); i++) {
         if (e->plan.convs[i].out_act < 0) continue;
-        int ex = 0;
-        frexpf(e->conv_scale[i], &ex);
-        t.layers.push_back({e->plan.convs[i].name, elem_name({e->prec->fmt.planes, conv_out_elem(e, (int)i)}), ex - 1});
+        t.layers.push_back({e->plan.convs[i].name, elem_name({e->prec->fmt.planes, conv_out_elem(e, (int)i)}), log2_of_scale(e->conv_scale[i])});
     }
     return t;
 }
@@ -1693,13 +1688,7 @@ static int apply_scales(pe_engine* e, const std::vector<float>& s, int* changed)
     e->conv_scale = s;
     int moved = 0;
     for (size_t i = 0; i < s.size(); i++) moved += s[i] != old[i];
-    int rc;
-    for (size_t i = 0; i < s.size(); i++) {
-        bool repack = false;
-        for (int pc : e->plan.convs[i].cin_prod) if (pc >= 0 && s[pc] != old[pc]) repack = true;
-        if (repack && (rc = upload_weights(e, (int)i))) return rc;
-        if ((rc = upload_fields(e, (int)i))) return rc;
-    }
+    for (size_t i = 0; i < s.size(); i++) { const int rc = refresh_layer(e, (int)i, old); if (rc) return rc; }
     CK(e, cudaMemsetAsync(e->d_range, 0, s.size() * sizeof(unsigned), e->stream));
     CK(e, cudaStreamSynchronize(e->stream));
     e->calibrated = true;
@@ -1736,12 +1725,8 @@ extern "C" int pe_calibrate_end(pe_engine* e, int* changed) {
     fold_range(e, bits);
     e->collecting = false;
     std::vector<float> s = e->conv_scale;
-    for (size_t i = 0; i < nc; i++) {
-        if (e->plan.convs[i].out_act < 0) continue;
-        const float m = e->collect_max[i];   // pe_calibrate's rule: m * s in [2^(top-1), 2^top) of the stored kind's row; 0 keeps the scale
-        const int top = out_row(e, (int)i).range_top;
-        if (m > 0.f && m < 3e38f) { int ex = 0; frexpf(m, &ex); s[i] = ldexpf(1.f, std::max(-100, std::min(100, top - ex))); }
-    }
+    for (size_t i = 0; i < nc; i++)   // pe_calibrate's rule; a layer that recorded nothing keeps its scale
+        if (e->plan.convs[i].out_act >= 0) s[i] = pow2_for(e->collect_max[i], out_row(e, (int)i).range_top, s[i]);
     return apply_scales(e, s, changed);
 }
 
@@ -1750,7 +1735,7 @@ extern "C" int pe_calibration_get(const pe_engine* ce, char* buf, int cap) {
     pe_engine* e = const_cast<pe_engine*>(ce);   // the error text and the cached weights hash
     if (!e->committed) return -fail(e, PE_ERR_STATE, "pe_calibration_get: pe_commit_weights has not been called");
     if (!e->prec->ranged()) return -fail(e, PE_ERR_INVALID, "pe_calibration_get: precision %d has no range scales", e->cfg.precision);
-    if (e->bias_true.size() != e->plan.convs.size() || e->bias_true[0].empty() || e->hw[0].w.empty())
+    if (!owns_weights(e))
         return -fail(e, PE_ERR_STATE, "pe_calibration_get: this handle received its weights by broadcast / sharing: ask the handle that owns them");
     for (const ConvSpec& c : e->plan.convs)
         if (c.name.find_first_of(" \t\r\n#") != std::string::npos)
@@ -1941,10 +1926,10 @@ extern "C" int pe_blob_log2_scale(pe_engine* e, const char* blob_name, int* k) {
     if (!e->prec->ranged()) return fail(e, PE_ERR_INVALID, "this precision has no range scales");
     for (const BlobRef& b : e->plan.blobs) {
         if (b.name != blob_name) continue;
-        int ex = 0;
-        const float f = frexpf(blob_scale(e, b), &ex);   // a power of two: f = 0.5
-        if (f != 0.5f) return fail(e, PE_ERR_STATE, "blob %s: scale is not a power of two", blob_name);
-        *k = ex - 1;
+        const float s = blob_scale(e, b);
+        const int ex = log2_of_scale(s);
+        if (ldexpf(1.f, ex) != s) return fail(e, PE_ERR_STATE, "blob %s: scale is not a power of two", blob_name);
+        *k = ex;
         return PE_OK;
     }
     return fail(e, PE_ERR_INVALID, "unknown blob %s", blob_name);

@@ -769,8 +769,7 @@ static bool create_engines(int num_gpu, int per_gpu, int precision, const std::s
         engines.push_back(e);
     }
     if (load_weights(engines[0], Fi("start_device"))) return false;
-    const bool calibrate = Fb("calibrate_range") && (precision == PE_PREC_F16X2 || precision == PE_PREC_F16X1 || precision == PE_PREC_E4M3X1 ||
-                                                     precision == PE_PREC_S8X1);
+    const bool calibrate = Fb("calibrate_range") && ranged_precision(precision);
     auto calibrate_engine = [&](pe_engine* e, int dev) {
         std::vector<uint8_t> probe;
         synthetic_frame(0, global.disp_w, global.disp_h, probe);

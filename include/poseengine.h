@@ -142,7 +142,9 @@ int pe_commit_weights(pe_engine* e);
  * layer's largest |output| in fp32 and sets the scales so that the stored maxima sit in [32, 64) - after that a net of any
  * magnitude (e.g. the prototxt's gaussian(0.01) filler, whose maps are ~3e-11) keeps fp32-level parity.  Exact: scales are powers
  * of two folded into the epilogue's bias / factor.  Call it on the handle that owns the weights, before pe_broadcast_weights /
- * pe_share_weights (the scales travel inside the packed buffer).  Results of the calibration forward are fetchable as usual.
+ * pe_share_weights (the scales travel inside the packed buffer): a receiving handle, or an owner whose weights are already shared,
+ * gets PE_ERR_STATE.  The frames take pe_forward_frames' path to the net input; results of the calibration forward are fetchable
+ * as usual.
  * pe_range_status: since the previous call, largest |stored value| / 65504 over all layers; PE_ERR_RANGE (and pe_last_error names
  * the layer) if a layer reached the fp16 limit or shrank below 2^-10.  With the environment variable PE_CHECK_RANGE=1 every
  * pe_fetch(idx 0) performs this check, so range problems are errors instead of silent inf / zeros. */

@@ -75,6 +75,24 @@ def test_one_pass_after_pe_calibrate_changes_nothing(mode):
 
 
 @pytest.mark.parametrize("mode", list(MODES))
+def test_pe_calibrate_after_a_net_input_forward_sees_only_its_frames(mode):
+    # the planar route writes the input's lo planes; the calibration forward must clear them as pe_forward_frames does
+    F = synth.make_frame(6, DISP_H, DISP_W)
+    ref = make(mode)
+    ref.calibrate([F])
+    want = ref.fetch_maps(1), ref.calibration_table()
+    ref.close()
+    eng = make(mode)
+    eng.set_calibration_table(eng.calibration_table())   # scale 1 everywhere, as created; lets S8X1 forward
+    x = np.random.default_rng(6).standard_normal((eng.cfg.num_scales, 3, NET_H, NET_W)).astype(np.float32) * 100
+    eng.forward_net_input(x)
+    eng.calibrate([F])
+    assert np.array_equal(eng.fetch_maps(1), want[0])
+    assert eng.calibration_table() == want[1]
+    eng.close()
+
+
+@pytest.mark.parametrize("mode", list(MODES))
 def test_low_contrast_calibration_is_repaired_by_passes_over_the_set(mode):
     H = synth.make_frame(0, DISP_H, DISP_W)
     L = low_contrast(H)
@@ -189,6 +207,9 @@ def test_refusals(tmp_path):
         for call in (eng.calibrate_begin, eng.calibrate_end):
             with pytest.raises(engine.PoseEngineError, match="error 3:"):
                 call()
+    # pe_calibrate on the owner would re-pack the buffer recv runs on while recv keeps the old scales
+    with pytest.raises(engine.PoseEngineError, match="error 3:.*shares its weights"):
+        a.calibrate([F])
     # modes without range scales
     for prec in (engine.PREC_FP32_SIMT, engine.PREC_BF16X1, engine.PREC_BF16X3):
         e = engine.PoseEngine(engine.COCO_18, NET_W, NET_H, DISP_W, DISP_H, precision=prec)

@@ -212,3 +212,15 @@ def test_refusals_launch_nothing():
         assert L.pe_forward_pixels(e._h, C.byref(pf), (C.c_void_p * 1)(other.data_ptr()), 1, C.byref(s)) == 1
         assert "GPU 1" in L.pe_last_error(e._h).decode()
     e.close()
+
+
+def test_forward_frames_checks_every_pointer_before_copying():
+    # a pageable frame sends the batch through the staging copy: the null pointer after it must be refused, not read
+    e = make_engine(max_batch=2)
+    L = engine.lib()
+    frame = np.zeros((DISP_H, DISP_W, 3), np.uint8)
+    before = L.pe_launch_count(e._h)
+    assert L.pe_forward_frames(e._h, (C.c_void_p * 2)(frame.ctypes.data, None), 2) == 1
+    assert "null frame 1" in L.pe_last_error(e._h).decode()
+    assert L.pe_launch_count(e._h) == before
+    e.close()
