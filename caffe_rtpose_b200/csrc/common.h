@@ -99,6 +99,16 @@ int build_plan_from_net(const NetDef& net, const PlanFormats& f, NetPlan& out, s
 // One element kind throughout, Concat slots 8-aligned
 int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& out, std::string& err);
 
+// The packed K order of conv c's weights (engine.cu packs in it): K index kk = tap * c.in_cused + engine input channel, Concat
+// slots at their aligned offsets (cin_map), conv1_1 the 27 values of its im2col'ed input.  Returns the index of weight (co, kk)
+// in the Caffe blob [cout][cin][k][k], or -1 for a zero pad.
+long long conv_weight_index(const ConvSpec& c, int co, int kk);
+// 2:4 structured sparsity in that order: every aligned group of four packed weights of every output channel of w (Caffe
+// layout) holds at most two non-zeros.  Padding is zero.
+bool conv_weights_2to4(const ConvSpec& c, const float* w);
+// Magnitude pruning to 2:4 in that grouping, in place: each group keeps its two largest |w|, the lower K index on a tie.
+void conv_prune_2to4(const ConvSpec& c, float* w);
+
 // ---------------------------------------------------------------------------------------------
 // kernel argument blocks
 // ---------------------------------------------------------------------------------------------

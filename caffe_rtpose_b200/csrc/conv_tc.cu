@@ -96,6 +96,20 @@ int tc_layer_create(const TcLayerDesc& d, TcLayer& out, std::string& err) {
     memset(maps, 0, 3 * sizeof(CUtensorMap));
     const cuuint64_t K = (cuuint64_t)d.ksize * d.ksize * d.in_cused;
     const cuuint64_t P = (cuuint64_t)d.fmt.planes;
+    if (d.sparse) {   // conv_s8_sparse.cu: windows {128 ch, N + 8 rows} at N = 128 and 64; compressed values {64 B, 128 rows}, SWIZZLE_64B
+        if (!d.fmt.s8() || d.cout_pad % 128) { err = "sparse layers are s8 with 128-channel output blocks"; free(maps); return -1; }
+        int r = 0;
+        for (int m = 0; m < 2 && !r; m++)
+            r = encode(enc, &maps[2 * m], d.fmt.elem, d.in, d.in_cused, d.geo.M, 1, (cuuint64_t)d.in_pitch, (cuuint64_t)d.in_plane,
+                       d.ksize == 1 ? 128 >> m : (128 >> m) + TC_KMAX - 1, 1, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+        cuuint64_t dims[3] = {K / 2, (cuuint64_t)d.cout_pad, 1}, strides[2] = {K / 2, K / 2 * d.cout_pad};
+        cuuint32_t box[3] = {64, 128, 1}, es[3] = {1, 1, 1};
+        if (!r) r = (int)enc(&maps[1], CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, (void*)d.w, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                             CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        if (r) { err = "cuTensorMapEncodeTiled failed: " + std::to_string(r); free(maps); return -1; }
+        out.maps = maps;
+        return 0;
+    }
     // A: [planes][M][pitch], box {channel block, window rows, planes}
     int r = encode(enc, &maps[0], d.fmt.elem, d.in, d.in_cused, d.geo.M, P, (cuuint64_t)d.in_pitch * eb, (cuuint64_t)d.in_plane * eb,
                    tc_window_rows(d.ksize), d.fmt.planes,
@@ -118,6 +132,7 @@ void tc_layer_destroy(TcLayer& l) {
 
 int tc_layer_launch(const TcLayer& l, int nimg, cudaStream_t st, int share) {
     const TcLayerDesc& d = l.d;
+    if (d.sparse) return tc_sparse_launch(l, nimg, st, share);   // conv_s8_sparse.cu
     TcArgs a;
     a.bias = d.bias;
     a.out = d.out; a.out_pitch = d.out_pitch; a.out_coff = d.out_coff; a.out_plane = d.out_plane;

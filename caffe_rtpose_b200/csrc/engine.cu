@@ -19,6 +19,7 @@
 #include "precision.h"
 #include "e4m3.h"
 #include "s8.h"
+#include "s8_sparse.h"
 #include "jpeg_coefs.h"
 #include "jpeg_entropy.cuh"
 #include "pixels.cuh"
@@ -64,6 +65,8 @@ struct pe_engine {
     uint64_t weights_hash = 0; bool weights_hash_valid = false;   // of hw (calibration tables); reset by pe_commit_weights
     std::vector<size_t> w_off, b_off;
     std::vector<int> cout_pad, cin_pad;
+    std::vector<char> sparse;       // per conv: runs the 2:4-sparse s8 kernel (chosen at pe_commit_weights, see sparse_eligible)
+    bool force_sparse = false;      // pe_test_force_sparse: lift rule 4 of sparse_eligible at the next pe_commit_weights
     std::vector<TcLayer> tc;        // wgmma per-conv launch state
     // io
     cudaStream_t stream = nullptr;
@@ -267,12 +270,8 @@ static void set_post_params(pe_engine* e) {
     p.num_scales = c.num_scales;
 }
 
-// Host-only view of the execution plan a prototxt (or, with path == NULL, the built-in graph of `model`) produces: one
-// line per op, "conv <name> cout cin k relu level in_act in_cused out_act out_coff planar_coff", "pool <name> in out",
-// "copy src dst channels", then "gap level g" per resolution level (the flat layout's gap, common.h), "nms threshold
-// max_peaks num_parts" and "resize start_scale scale_gap".  No GPU needed.
-extern "C" int pe_plan_describe(int model, const char* prototxt_path, char* buf, int cap) {
-    NetDef net;
+// The net of a host-only query: the prototxt at `prototxt_path`, or with NULL the built-in graph of `model`.  0 or -PE_ERR_*.
+static int query_net(int model, const char* prototxt_path, NetDef& net) {
     std::string err;
     if (prototxt_path) {
         if (parse_prototxt_file(prototxt_path, net, err)) return -fail(nullptr, PE_ERR_IO, "%s: %s", prototxt_path, err.c_str());
@@ -280,6 +279,17 @@ extern "C" int pe_plan_describe(int model, const char* prototxt_path, char* buf,
         if (model != PE_MODEL_MPI_15 && model != PE_MODEL_COCO_18) return -fail(nullptr, PE_ERR_INVALID, "unknown model %d", model);
         net = builtin_netdef(model, 6);
     }
+    return 0;
+}
+
+// Host-only view of the execution plan a prototxt (or, with path == NULL, the built-in graph of `model`) produces: one
+// line per op, "conv <name> cout cin k relu level in_act in_cused out_act out_coff planar_coff", "pool <name> in out",
+// "copy src dst channels", then "gap level g" per resolution level (the flat layout's gap, common.h), "nms threshold
+// max_peaks num_parts" and "resize start_scale scale_gap".  No GPU needed.
+extern "C" int pe_plan_describe(int model, const char* prototxt_path, char* buf, int cap) {
+    NetDef net;
+    std::string err;
+    if (const int rc = query_net(model, prototxt_path, net)) return rc;
     NetPlan p;
     if (build_plan_from_net(net, 64, 64, p, err)) return -fail(nullptr, PE_ERR_INVALID, "%s", err.c_str());
     std::string s = "model " + std::to_string(p.model) + "\n";
@@ -344,12 +354,7 @@ extern "C" int pe_plan_formats(int model, const char* prototxt_path, int prec, c
     NetDef net;
     std::string err;
     if (prec < 0 || prec >= NUM_PRECISIONS) return -fail(nullptr, PE_ERR_INVALID, "unknown precision %d", prec);
-    if (prototxt_path) {
-        if (parse_prototxt_file(prototxt_path, net, err)) return -fail(nullptr, PE_ERR_IO, "%s: %s", prototxt_path, err.c_str());
-    } else {
-        if (model != PE_MODEL_MPI_15 && model != PE_MODEL_COCO_18) return -fail(nullptr, PE_ERR_INVALID, "unknown model %d", model);
-        net = builtin_netdef(model, 6);
-    }
+    if (const int rc = query_net(model, prototxt_path, net)) return rc;
     NetPlan p;
     if (plan_for(net, prec, f16_layers, p, err)) return -fail(nullptr, PE_ERR_INVALID, "%s", err.c_str());
     const int planes = precision(prec).fmt.planes;
@@ -367,6 +372,27 @@ extern "C" int pe_plan_formats(int model, const char* prototxt_path, int prec, c
     }
     if (buf && (int)s.size() < cap) memcpy(buf, s.c_str(), s.size() + 1);
     return (int)s.size();
+}
+
+// Magnitude pruning to 2:4 in the packed K order of the PE_PREC_S8X1 plan (plan.cpp, conv_prune_2to4): the grouping the engine
+// tests at pe_commit_weights to pick the sparse kernel.
+extern "C" int pe_prune_2to4(int model, const char* prototxt_path, const char* layer, float* w, int cout, int cin, int k) {
+    if (!layer || !w) return -fail(nullptr, PE_ERR_INVALID, "pe_prune_2to4: null layer name or weights");
+    NetDef net;
+    std::string err;
+    if (const int rc = query_net(model, prototxt_path, net)) return rc;
+    NetPlan p;
+    if (plan_for(net, PE_PREC_S8X1, nullptr, p, err)) return -fail(nullptr, PE_ERR_INVALID, "%s", err.c_str());
+    for (const ConvSpec& c : p.convs) {
+        if (c.name != layer) continue;
+        if (c.im2col_input) return -fail(nullptr, PE_ERR_INVALID, "pe_prune_2to4: layer %s reads the im2col'ed net input and always runs dense", layer);
+        if (c.cout != cout || c.cin != cin || c.k != k)
+            return -fail(nullptr, PE_ERR_INVALID, "pe_prune_2to4: layer %s is %d x %d x %dx%d, not %d x %d x %dx%d", layer, c.cout, c.cin, c.k, c.k,
+                         cout, cin, k, k);
+        conv_prune_2to4(c, w);
+        return PE_OK;
+    }
+    return -fail(nullptr, PE_ERR_INVALID, "pe_prune_2to4: unknown conv layer %s", layer);
 }
 
 static int create_impl(const pe_config* cfg, const char* prototxt_path, const char* f16_layers, pe_engine** out);
@@ -647,7 +673,14 @@ static inline void split_fp16(float x, int planes, uint16_t* out) {   // IEEE fp
     }
 }
 
-// byte layout of the packed weight buffer (a function of the plan and the precision only, so replicas agree on it)
+static size_t conv_k(const pe_engine* e, int i) { return (size_t)(e->plan.convs[i].im2col_input ? 1 : e->plan.convs[i].k * e->plan.convs[i].k) * e->cin_pad[i]; }
+// bytes of conv i's packed weights: the planes [P][cout_pad][K], or the compressed values and metadata of a sparse layer
+static size_t weight_bytes(const pe_engine* e, int i) {
+    return e->sparse[i] ? s8_sparse_bytes(e->cout_pad[i], conv_k(e, i)) : conv_k(e, i) * e->cout_pad[i] * fmt_bytes(conv_wfmt(e, i));
+}
+
+// byte layout of the packed weight buffer (a function of the plan, the precision and the sparse layers only, so replicas that
+// take the sender's sparse layers agree on it)
 static size_t packed_layout(pe_engine* e) {
     const size_t nc = e->plan.convs.size();
     e->w_off.assign(nc, 0); e->b_off.assign(nc, 0); e->cout_pad.assign(nc, 0); e->cin_pad.assign(nc, 0);
@@ -656,10 +689,9 @@ static size_t packed_layout(pe_engine* e) {
     for (size_t i = 0; i < nc; i++) {
         const ConvSpec& c = e->plan.convs[i];
         e->cin_pad[i] = c.in_cused;
-        e->cout_pad[i] = e->prec->fmt.planes ? tc_cout_pad(c.cout) : (c.cout + 63) / 64 * 64;
-        const size_t K = (size_t)(c.im2col_input ? 1 : c.k * c.k) * e->cin_pad[i];
+        e->cout_pad[i] = e->sparse[i] ? (c.cout + SP_BM - 1) / SP_BM * SP_BM : e->prec->fmt.planes ? tc_cout_pad(c.cout) : (c.cout + 63) / 64 * 64;
         e->w_off[i] = total;
-        total = align256(total + K * e->cout_pad[i] * fmt_bytes(conv_wfmt(e, (int)i)));
+        total = align256(total + weight_bytes(e, (int)i));
         e->b_off[i] = total;
         total = align256(total + epi_floats(e, (int)i) * 4);
     }
@@ -702,7 +734,7 @@ static void fill_epilogue_fields(const pe_engine* e, int i, float* B) {
 // Weights of conv i into `dst` (the layer's region of the packed buffer, host copy): fp32 [K][cout_pad] for the SIMT mode, else
 // P 16-bit planes [P][cout_pad][K] (K-major rows: the wgmma B operand) of w * 2^k, the per-channel range ratios folded in.
 // Sets e->wsi[i] = 2^-k.  S8X1: one s8 plane [cout_pad][K], each output channel quantised on its own (s8.h); sets e->wsig[i].
-static void pack_conv_weights(pe_engine* e, int i, uint8_t* dst) {
+static int pack_conv_weights(pe_engine* e, int i, uint8_t* dst) {
     const ConvSpec& c = e->plan.convs[i];
     const HostWeights& hw = e->hw[i];
     const int taps = c.im2col_input ? 1 : c.k * c.k, cp = e->cin_pad[i], cop = e->cout_pad[i];
@@ -711,27 +743,27 @@ static void pack_conv_weights(pe_engine* e, int i, uint8_t* dst) {
     std::vector<float> chan(cp, 1.f);   // s_ref / s(ci) per engine input channel
     for (int ec = 0; ec < cp && ec < (int)c.cin_prod.size(); ec++)
         if (c.cin_prod[ec] >= 0) chan[ec] = s_ref / e->conv_scale[c.cin_prod[ec]];
-    auto src = [&](int co, int kk) -> float {  // engine K index -> Caffe weight (co, ci, r, s)
-        if (c.im2col_input) {
-            if (kk >= 27) return 0.f;
-            const int tap = kk / 3, ci = kk % 3;
-            return hw.w[((size_t)co * 3 + ci) * 9 + tap];
-        }
-        const int tap = kk / cp, ec = kk % cp;
-        const int ci = ec < (int)c.cin_map.size() ? c.cin_map[ec] : -1;
-        if (ci < 0) return 0.f;
-        return hw.w[((size_t)co * c.cin + ci) * c.k * c.k + tap] * chan[ec];
+    auto src = [&](int co, int kk) -> float {  // engine K index -> Caffe weight (co, ci, r, s) (plan.cpp)
+        const long long wi = conv_weight_index(c, co, kk);
+        return wi < 0 ? 0.f : c.im2col_input ? hw.w[wi] : hw.w[wi] * chan[kk % cp];
     };
     const PlaneFmt wf = conv_wfmt(e, i);
-    memset(dst, 0, K * cop * fmt_bytes(wf));
+    memset(dst, 0, weight_bytes(e, i));
     float wscale_inv = 1.f;
     if (wf.s8()) {
+        // a sparse layer quantises into a dense plane first and stores it compressed (s8_sparse.h); quantisation only adds zeros
+        std::vector<int8_t> dense(e->sparse[i] ? K * cop : 0);
+        int8_t* q = e->sparse[i] ? dense.data() : (int8_t*)dst;
         std::vector<float> wc(K);
         e->wsig[i].assign(cop, 0.f);
         for (int co = 0; co < c.cout; co++) {
             for (size_t kk = 0; kk < K; kk++) wc[kk] = src(co, (int)kk);
-            e->wsig[i][co] = s8_quantize_channel(wc.data(), K, (int8_t*)dst + (size_t)co * K);
+            e->wsig[i][co] = s8_quantize_channel(wc.data(), K, q + (size_t)co * K);
         }
+        // the sparse choice was made from these fp32 weights, and quantisation only adds zeros: a group with three non-zeros here
+        // means the choice and the weights disagree, and the compressed bytes would be wrong
+        if (e->sparse[i] && !s8_sparse_compress(q, cop, K, dst))
+            return fail(e, PE_ERR_STATE, "layer %s: its weights are not 2:4 but the layer was chosen to run sparse", c.name.c_str());
     } else if (wf.planes == 0) {  // fp32 [K][cout_pad]
         float* W = (float*)dst;
         for (size_t kk = 0; kk < K; kk++)
@@ -763,6 +795,7 @@ static void pack_conv_weights(pe_engine* e, int i, uint8_t* dst) {
         }
     }
     e->wsi[i] = wscale_inv;
+    return PE_OK;
 }
 
 // per-layer launch state (TMA descriptors) over the packed buffer the handle currently points at
@@ -783,7 +816,7 @@ static int bind_packed(pe_engine* e) {
             d.w = (char*)e->d_packed + e->w_off[i]; d.bias = (const float*)((char*)e->d_packed + e->b_off[i]);
             d.cout = c.cout; d.cout_pad = e->cout_pad[i]; d.ksize = c.im2col_input ? 1 : c.k; d.pad = c.im2col_input ? 0 : c.pad;
             d.relu = c.relu; d.fmt = conv_wfmt(e, (int)i); d.geo = g; d.out_scale = d.bias + e->cout_pad[i];
-            d.out_elem = conv_out_elem(e, (int)i); d.chunked = conv_row(e, (int)i).chunked;
+            d.out_elem = conv_out_elem(e, (int)i); d.chunked = conv_row(e, (int)i).chunked; d.sparse = e->sparse[i];
             d.range = (e->prec->ranged() && e->d_range) ? e->d_range + i : nullptr;
             if (c.out_act >= 0) {
                 d.out = e->acts[c.out_act]; d.out_pitch = e->plan.acts[c.out_act].C; d.out_coff = c.out_coff; d.out_plane = e->act_plane[c.out_act];
@@ -801,7 +834,30 @@ static int bind_packed(pe_engine* e) {
     return PE_OK;
 }
 
-extern "C" int pe_commit_weights(pe_engine* e) {
+// Layers that may run the 2:4-sparse kernel (conv_s8_sparse.cu) when their weights are 2:4 in the packed K order:
+//   1. s8 arithmetic with an s8 or fp32-map output (not the fp16 layers of a mixed engine, nor their s8 -> fp16 boundary layers);
+//   2. not conv1_1, whose im2col'ed input is no conv window;
+//   4. the shape rule: only a layer class where the sparse kernel measures faster than the dense one.  As built it is slower in
+//      every class of the shipped nets (DESIGN.md section 5: 7x7, first 7x7 of a stage, VGG 3x3, stage-1 3x3, conv1_x and 1x1,
+//      1.2-2.2x the dense kernel's time), and no other shape has been measured, so no class qualifies and every layer runs dense.
+//      pe_test_force_sparse lifts this rule, so that tests and tools/sparse_s8.py can run and measure the kernel.
+// (Rule 3, the 2:4 weights, is checked by commit.)
+static bool sparse_eligible(const pe_engine* e, int i) {
+    const ConvSpec& c = e->plan.convs[i];
+    return e->force_sparse && conv_wfmt(e, i).s8() && conv_out_elem(e, i) == ELEM_S8 && !c.im2col_input;
+}
+
+// Test hook, not part of the public header: with on != 0 the next pe_commit_weights of e picks the sparse kernel for every layer
+// that rules 1-3 of sparse_eligible admit, ignoring the shape rule.  Returns 0, or PE_ERR_INVALID for a null handle.
+extern "C" int pe_test_force_sparse(pe_engine* e, int on) {
+    if (!e) return PE_ERR_INVALID;
+    e->force_sparse = on != 0;
+    return PE_OK;
+}
+
+// pe_commit_weights; `sparse_from`: the sparse layers to take (a broadcast replica, which has no weights to decide from), or null
+// to choose them from the fp32 weights.  The choice is made before quantisation, so re-packing keeps it.
+static int commit(pe_engine* e, const std::vector<char>* sparse_from) {
     if (!e) return PE_ERR_INVALID;
     if (e->collecting) return fail(e, PE_ERR_STATE, "a calibration collection is running: call pe_calibrate_end first");
     CK(e, cudaSetDevice(e->cfg.device));
@@ -813,6 +869,9 @@ extern "C" int pe_commit_weights(pe_engine* e) {
             return fail(e, PE_ERR_STATE, "weights of layer %s were never set%s", c.name.c_str(),
                         e->committed ? " on this handle (a broadcast replica keeps no fp32 copy: set every layer again)" : "");
     }
+    e->sparse.assign(nc, 0);
+    for (size_t i = 0; i < nc; i++)
+        e->sparse[i] = sparse_from ? (*sparse_from)[i] : sparse_eligible(e, (int)i) && conv_weights_2to4(e->plan.convs[i], e->hw[i].w.data());
     const size_t total = packed_layout(e);
     e->calibrated = false;
     e->wsi.assign(nc, 1.f);
@@ -820,7 +879,10 @@ extern "C" int pe_commit_weights(pe_engine* e) {
     e->conv_scale.assign(nc, 1.f);
     std::vector<uint8_t> host(total, 0);
     for (size_t i = 0; i < nc; i++) {
-        pack_conv_weights(e, (int)i, host.data() + e->w_off[i]);
+        if (pack_conv_weights(e, (int)i, host.data() + e->w_off[i])) {
+            e->committed = false;   // the layout changed under the bound buffer: no forward until a commit succeeds
+            return PE_ERR_STATE;
+        }
         fill_epilogue_fields(e, (int)i, (float*)(host.data() + e->b_off[i]));   // travels with the packed buffer (weight broadcast)
     }
     e->packed_owner.reset();
@@ -834,6 +896,7 @@ extern "C" int pe_commit_weights(pe_engine* e) {
     e->packed_bytes = total;
     return bind_packed(e);
 }
+extern "C" int pe_commit_weights(pe_engine* e) { return commit(e, nullptr); }
 
 // Net::ShareTrainedLayersWith (src/caffe/net.cpp:682-706): a second net on the SAME GPU uses the first one's weights instead of
 // loading them again - here the packed device buffer itself (no copy; it lives until the last handle that uses it is destroyed).
@@ -851,7 +914,15 @@ extern "C" int pe_share_weights(pe_engine* from, pe_engine* to) {
     }
     CK(to, cudaSetDevice(to->cfg.device));
     CK(to, cudaStreamSynchronize(to->stream));
-    if (packed_layout(to) != from->packed_bytes) return fail(from, PE_ERR_STATE, "packed layouts differ");
+    // the receiver runs the sender's packed buffer, sparse layers included; on a layout mismatch it keeps its own layout
+    const std::vector<char> own_sparse = to->sparse;
+    const std::vector<size_t> own_w = to->w_off, own_b = to->b_off;
+    const std::vector<int> own_cout = to->cout_pad, own_cin = to->cin_pad;
+    to->sparse = from->sparse;
+    if (packed_layout(to) != from->packed_bytes) {
+        to->sparse = own_sparse; to->w_off = own_w; to->b_off = own_b; to->cout_pad = own_cout; to->cin_pad = own_cin;
+        return fail(from, PE_ERR_STATE, "packed layouts differ");
+    }
     to->packed_owner = from->packed_owner;
     to->d_packed = from->d_packed;
     to->packed_bytes = from->packed_bytes;
@@ -881,14 +952,15 @@ extern "C" int pe_broadcast_weights(pe_engine* const* engines, int n) {
         bool same = e->plan.convs.size() == root->plan.convs.size();
         for (size_t l = 0; same && l < e->plan.convs.size(); l++) same = e->plan.convs[l].elem == root->plan.convs[l].elem;
         if (!same) return fail(root, PE_ERR_INVALID, "engine %d is not a replica of engine 0 (the fp16 layers differ)", i);
-        if (!e->committed) {   // allocate the packed buffer + TMA maps with the same layout (values arrive by broadcast)
+        // allocate the packed buffer + TMA maps with the same layout and sparse layers (values arrive by broadcast)
+        if (!e->committed || e->sparse != root->sparse) {
             for (size_t l = 0; l < e->plan.convs.size(); l++) {
                 const ConvSpec& c = e->plan.convs[l];
                 e->hw[l].w.assign((size_t)c.cout * c.cin * c.k * c.k, 0.f);
                 e->hw[l].b.assign(c.cout, 0.f);
                 e->hw[l].set = true;
             }
-            const int rc = pe_commit_weights(e);
+            const int rc = commit(e, &root->sparse);
             if (rc) return rc;
             // the replica holds no fp32 copy: a later pe_set_conv_weights on a subset + pe_commit_weights must fail
             // ("weights of layer ... were never set") instead of packing from empty vectors
@@ -931,6 +1003,13 @@ extern "C" int pe_broadcast_weights(pe_engine* const* engines, int n) {
 }
 
 extern "C" size_t pe_packed_weights_bytes(const pe_engine* e) { return e ? e->packed_bytes : 0; }
+
+extern "C" int pe_conv_layer_sparse(const pe_engine* e, int idx) {
+    if (!e) return -PE_ERR_INVALID;
+    if (idx < 0 || idx >= (int)e->plan.convs.size()) return -fail((pe_engine*)e, PE_ERR_INVALID, "conv layer index %d out of range", idx);
+    if (!e->committed) return -fail((pe_engine*)e, PE_ERR_STATE, "pe_conv_layer_sparse: pe_commit_weights has not been called");
+    return e->sparse[idx] ? 1 : 0;
+}
 extern "C" void* pe_packed_weights_device_ptr(pe_engine* e) { return e ? e->d_packed : nullptr; }
 
 // ---------------------------------------------------------------------------------------------
@@ -1522,10 +1601,8 @@ static int upload_fields(pe_engine* e, int i) {
 }
 
 static int upload_weights(pe_engine* e, int i) {   // re-pack layer i with the current input scales (host fp32 copy needed)
-    const ConvSpec& c = e->plan.convs[i];
-    const size_t K = (size_t)(c.im2col_input ? 1 : c.k * c.k) * e->cin_pad[i];
-    std::vector<uint8_t> buf(K * e->cout_pad[i] * fmt_bytes(conv_wfmt(e, i)));
-    pack_conv_weights(e, i, buf.data());
+    std::vector<uint8_t> buf(weight_bytes(e, i));
+    if (const int rc = pack_conv_weights(e, i, buf.data())) return rc;
     CK(e, cudaMemcpyAsync((char*)e->d_packed + e->w_off[i], buf.data(), buf.size(), cudaMemcpyHostToDevice, e->stream));
     CK(e, cudaStreamSynchronize(e->stream));
     return PE_OK;

@@ -5,6 +5,7 @@
 // The plan is not a translation of Caffe's layer list: ReLU is fused into the conv epilogue, Concat is
 // removed (producers write channel slices of a shared buffer), Split disappears, and conv1_1 consumes an
 // im2col'ed input so that it is a K=27 1x1 GEMM.
+#include <math.h>
 #include <stdio.h>
 
 #include <algorithm>
@@ -384,6 +385,45 @@ int build_plan_from_net(const NetDef& net, const PlanFormats& fm, NetPlan& p, st
             if (act == b.act && c0 < b.coff + b.c && b.coff < c1) b.reused_by = who;
         }
     return 0;
+}
+
+long long conv_weight_index(const ConvSpec& c, int co, int kk) {
+    if (c.im2col_input) return kk < 27 ? ((long long)co * 3 + kk % 3) * 9 + kk / 3 : -1;   // tap = kk / 3, channel kk % 3
+    const int tap = kk / c.in_cused, ec = kk % c.in_cused;
+    const int ci = ec < (int)c.cin_map.size() ? c.cin_map[ec] : -1;
+    return ci < 0 ? -1 : ((long long)co * c.cin + ci) * c.k * c.k + tap;
+}
+
+// Calls f(co, idx[4]) for every aligned group of four packed weights (idx: Caffe indices, -1 for padding)
+template <class F> static void for_each_group(const ConvSpec& c, F f) {
+    const int K = (c.im2col_input ? 1 : c.k * c.k) * c.in_cused;
+    for (int co = 0; co < c.cout; co++)
+        for (int g = 0; g + 4 <= K; g += 4) {
+            long long idx[4];
+            for (int i = 0; i < 4; i++) idx[i] = conv_weight_index(c, co, g + i);
+            f(idx);
+        }
+}
+
+bool conv_weights_2to4(const ConvSpec& c, const float* w) {
+    bool ok = true;
+    for_each_group(c, [&](const long long* idx) {
+        int n = 0;
+        for (int i = 0; i < 4; i++) n += idx[i] >= 0 && w[idx[i]] != 0.f;
+        ok = ok && n <= 2;
+    });
+    return ok;
+}
+
+void conv_prune_2to4(const ConvSpec& c, float* w) {
+    for_each_group(c, [&](const long long* idx) {
+        auto mag = [&](int i) { return idx[i] >= 0 ? fabsf(w[idx[i]]) : -1.f; };
+        int a = 0;   // the largest |w|, the lowest index first among equals; then the largest of the others
+        for (int i = 1; i < 4; i++) if (mag(i) > mag(a)) a = i;
+        int b = a == 0 ? 1 : 0;
+        for (int i = 0; i < 4; i++) if (i != a && mag(i) > mag(b)) b = i;
+        for (int i = 0; i < 4; i++) if (i != a && i != b && idx[i] >= 0) w[idx[i]] = 0.f;
+    });
 }
 
 int build_plan_from_net(const NetDef& net, int kp_input, int cpad, NetPlan& p, std::string& err) {

@@ -69,6 +69,7 @@ ABI_SYMBOLS = [
     "pe_compare_results", "pe_jpeg_read_coefs", "pe_jpeg_coefs_to_bgr", "pe_forward_jpeg_coefs", "pe_video_read_coefs",
     "pe_jpeg_read_scan", "pe_jpeg_scan_to_coefs_host", "pe_forward_jpeg_scans", "pe_jpeg_decode_scans", "pe_video_read_scan",
     "pe_forward_pixels", "pe_stream_wait", "pe_pixels_to_bgr", "pe_blob_log2_scale", "pe_create_mixed", "pe_plan_formats",
+    "pe_conv_layer_sparse", "pe_prune_2to4",
 ]
 
 
@@ -94,6 +95,8 @@ def lib():
     L.pe_set_conv_weights.argtypes = [C.c_void_p, C.c_char_p, _f32p, C.c_size_t, _f32p, C.c_size_t]
     L.pe_load_weights_file.argtypes = [C.c_void_p, C.c_char_p]
     L.pe_commit_weights.argtypes = [C.c_void_p]
+    L.pe_conv_layer_sparse.argtypes = [C.c_void_p, C.c_int]
+    L.pe_prune_2to4.argtypes = [C.c_int, C.c_char_p, C.c_char_p, _f32p, C.c_int, C.c_int, C.c_int]
     L.pe_share_weights.argtypes = [C.c_void_p, C.c_void_p]
     L.pe_calibrate.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_int]
     L.pe_range_status.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.c_char_p]
@@ -339,6 +342,17 @@ class PoseEngine:
         for i in range(L.pe_num_conv_layers(self._h)):
             self._ck(L.pe_conv_layer_info(self._h, i, name, C.byref(a), C.byref(b), C.byref(k)))
             out.append((name.value.decode(), a.value, b.value, k.value))
+        return out
+
+    def sparse_layers(self):
+        """Names of the conv layers that run the 2:4-sparse s8 kernel (pe_conv_layer_sparse), after commit_weights."""
+        out = []
+        for i, (name, _, _, _) in enumerate(self.conv_layers()):
+            r = lib().pe_conv_layer_sparse(self._h, i)
+            if r < 0:
+                self._ck(-r)
+            if r:
+                out.append(name)
         return out
 
     def set_weights(self, weights, commit=True):
@@ -608,6 +622,29 @@ def plan_describe(model=None, prototxt=None):
     buf = C.create_string_buffer(n + 1)
     L.pe_plan_describe(-1 if model is None else model, path, buf, n + 1)
     return buf.value.decode()
+
+
+def prune_2to4(weights, model=None, prototxt=None):
+    """A new weights dict {name: (w, b)} whose conv weights are magnitude-pruned to 2:4 in the engine's packed K order
+    (pe_prune_2to4), the grouping in which a PREC_S8X1 engine can run them on the sparse kernel (pe_conv_layer_sparse).  The first layer, which reads the im2col'ed net
+    input and always runs dense, and names the graph does not have are copied unchanged.  Pruning a trained model without
+    fine-tuning changes its outputs."""
+    L = lib()
+    path = os.fsencode(prototxt) if prototxt is not None else None
+    m = -1 if model is None else model
+    convs = [l.split() for l in plan_describe(model, prototxt).splitlines() if l.startswith("conv ")]
+    first_in = convs[0][7]   # in_act of the first layer: the im2col'ed net input
+    dense = {f[1] for f in convs if f[7] == first_in}
+    known = {f[1] for f in convs}
+    out = {}
+    for name, (w, b) in weights.items():
+        w = np.array(w, np.float32, copy=True, order="C")
+        if name in known and name not in dense:
+            rc = L.pe_prune_2to4(m, path, name.encode(), w.reshape(-1), *w.shape[:3])
+            if rc != 0:
+                raise PoseEngineError("pe_prune_2to4 failed (%d): %s" % (-rc, L.pe_last_error(None).decode()))
+        out[name] = (w, np.array(b, np.float32, copy=True))
+    return out
 
 
 def _layer_list(layers):

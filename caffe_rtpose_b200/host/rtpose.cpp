@@ -769,6 +769,12 @@ static bool create_engines(int num_gpu, int per_gpu, int precision, const std::s
         engines.push_back(e);
     }
     if (load_weights(engines[0], Fi("start_device"))) return false;
+    if (precision == PE_PREC_S8X1) {   // layers the 2:4-sparse s8 kernel runs (pe_conv_layer_sparse's rules)
+        const int n = pe_num_conv_layers(engines[0]);
+        int sparse = 0;
+        for (int i = 0; i < n; i++) sparse += pe_conv_layer_sparse(engines[0], i) == 1;
+        LOG_INFO("GPU %d: %d of %d conv layers run 2:4 sparse", Fi("start_device"), sparse, n);
+    }
     const bool calibrate = Fb("calibrate_range") && ranged_precision(precision);
     auto calibrate_engine = [&](pe_engine* e, int dev) {
         std::vector<uint8_t> probe;

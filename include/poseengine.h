@@ -61,7 +61,10 @@ extern "C" {
                              * (padded) exceeds 132104 could overflow s32 and is refused (PE_ERR_INVALID).  Needs pe_calibrate
                              * (it puts each layer's largest stored value in [32, 64)): a forward before it is PE_ERR_STATE.
                              * pe_range_status reports the largest stored value / 127 and PE_ERR_RANGE when a layer reaches 127
-                             * (saturates) or stays below 4.  DESIGN.md section 6. */
+                             * (saturates) or stays below 4.  The engine has a 2:4-sparse s8 kernel (wgmma.sp on compressed weights,
+                             * the dense kernel's bits), chosen from the weights at pe_commit_weights by pe_conv_layer_sparse's
+                             * rules; as built it is slower than the dense kernel in every measured layer class, so its shape
+                             * rule keeps every layer dense.  DESIGN.md section 6. */
 
 #define PE_MAX_PEOPLE 96   /* RENDER_MAX_PEOPLE, renderFunctions.h:6 / rtpose.cpp:88 */
 
@@ -134,6 +137,21 @@ int pe_caffemodel_blob(const pe_caffemodel* m, int layer, int blob, const float*
 const char* pe_caffemodel_last_error(void);
 /* pack + upload; must be called once after the weights are set and before any forward */
 int pe_commit_weights(pe_engine* e);
+/* 1 when conv layer idx runs the 2:4-sparse s8 kernel, else 0; -PE_ERR_STATE before pe_commit_weights, -PE_ERR_INVALID for a bad
+ * index.  pe_commit_weights picks it for a PE_PREC_S8X1 layer that (1) computes in s8 and stores s8 or the fp32 maps (not the fp16
+ * layers of pe_create_mixed nor the layers that feed them), (2) does not read the im2col'ed net input (conv1_1), (3) has fp32
+ * weights with at most two non-zeros in every aligned group of four of the engine's packed K order (pe_prune_2to4), and (4) is of
+ * a layer class where the sparse kernel measures faster than the dense one.  As built no class qualifies (DESIGN.md sections 3
+ * and 5: slower in every class of the shipped nets, other shapes not measured), so this returns 0 for every layer.  A sparse
+ * layer's results are bit for bit those of the dense kernel.  It is no option. */
+int pe_conv_layer_sparse(const pe_engine* e, int idx);
+/* host-only: magnitude pruning of conv layer `layer`'s weights w (cout, cin, k, k) in place to 2:4 in the grouping
+ * pe_conv_layer_sparse tests: the packed K order is tap, then engine input channel, with Concat slots at their 16-channel-aligned
+ * offsets and zero padding; each group of four keeps its two largest |w|, the lower index on a tie.  The graph: the prototxt at
+ * prototxt_path, or with NULL the built-in one of `model`.  0, or -PE_ERR_INVALID for an unknown layer, a wrong shape or the
+ * first layer (it reads the im2col'ed net input and always runs dense).  Pruning a trained model without fine-tuning changes
+ * its outputs. */
+int pe_prune_2to4(int model, const char* prototxt_path, const char* layer, float* w, int cout, int cin, int k);
 /* Range management of the fp16 modes (PE_PREC_F16X2, PE_PREC_F16X1), and of the e4m3 and s8 modes (PE_PREC_E4M3X1,
  * PE_PREC_S8X1: stored maxima in [64, 128) and [32, 64), largest values 448 and 127; PE_PREC_S8X1 refuses to forward before
  * pe_calibrate); a no-op in the others.  Their activation planes are fp16 x
@@ -456,7 +474,9 @@ long long pe_launch_count(const pe_engine* e);
 double pe_conv_flops_per_scale(const pe_engine* e);
 /* one-time weight replica broadcast for --num_gpu N frame sharding (rank 0's packed weights -> all):
  * exports / imports the packed device buffer so that the host layer (NCCL via torch.distributed or
- * ncclBroadcast in rtpose.bin) can move it.  Returns size in bytes. */
+ * ncclBroadcast in rtpose.bin) can move it.  Returns size in bytes.  A 2:4-sparse layer is stored compressed, so the buffer
+ * can only move between handles with the same sparse layers (pe_conv_layer_sparse): commit the same weights on both sides.
+ * pe_share_weights and pe_broadcast_weights give the receiving handle the sender's sparse layers. */
 size_t pe_packed_weights_bytes(const pe_engine* e);
 /* single-process --num_gpu N: engines[0]'s committed weights -> engines[1..n-1] (one handle per GPU) with one grouped
  * ncclBroadcast over NVLink instead of N file reads (rtpose.cpp:183-184).  The path's only collective. */
