@@ -88,10 +88,13 @@ struct NetDef;
 // base_elem (conv1_1: input_elem).  "narrow" in f16 stands for every conv layer that reads fewer than 128 channels.
 // layout[k]: channel pad, net input pitch and Concat slot alignment of an activation of element kind k (PlaneElem).
 struct ActLayout { int cpad, kp_input, slot_align; };
+// u8 (PE_PREC_FLAG_U8, base_elem s8): an activation whose every writer stores values >= 0 (conv layers followed by ReLU, and
+// max pools of them) and whose every reader computes in s8 is stored as u8, and its readers compute u8 x s8.
 struct PlanFormats {
     int base_elem = 0, input_elem = 0;
+    bool u8 = false;
     std::vector<std::string> f16;
-    ActLayout layout[4] = {};
+    ActLayout layout[5] = {};   // one per PlaneElem (precision.h)
 };
 // plan from a parsed prototxt / built-in definition; -1 and a message when the graph is outside the supported family or the
 // fp16 list breaks the format rules

@@ -164,12 +164,20 @@ PE_WGMMA_WIDTHS(ELEM_F16, 16, "f32.f16.f16", float, , ", 1, 1, 0, 0")
 PE_WGMMA_WIDTHS(ELEM_BF16, 16, "f32.bf16.bf16", float, , ", 1, 1, 0, 0")
 PE_WGMMA_WIDTHS(ELEM_E4M3, 32, "f32.e4m3.e4m3", float, , ", 1, 1")
 PE_WGMMA_WIDTHS(ELEM_S8, 32, "s32.s8.s8", int, _S32, "")
+PE_WGMMA_WIDTHS(ELEM_U8, 32, "s32.u8.s8", int, _S32, "")   // u8 activations (A) x s8 weights (B), the s8 rate
 
 // fp32 -> s8, round to nearest even, saturating to [-128, 127] (cvt.rni.sat.s8.f32; NaN gives 0)
 __device__ __forceinline__ uint32_t f32_to_s8(float x) {
     int q;
     asm("cvt.rni.sat.s8.f32 %0, %1;" : "=r"(q) : "f"(x));
     return (uint32_t)q & 0xffu;
+}
+
+// fp32 -> u8, round to nearest even, saturating to [0, 255] (cvt.rni.sat.u8.f32; NaN gives 0)
+__device__ __forceinline__ uint32_t f32_to_u8(float x) {
+    uint32_t q;
+    asm("cvt.rni.sat.u8.f32 %0, %1;" : "=r"(q) : "f"(x));
+    return q & 0xffu;
 }
 
 // Range tracking of the 16-bit planes: every epilogue warp folds the largest |value| it stores into one word per layer.  The
@@ -234,7 +242,8 @@ template <int BN, int PLANES> struct TcShape {
 
 // ELEM: element kind of the A windows and weight tiles; OUT: of the stored output planes (conv1_1 of the e4m3 mode reads
 // its fp16 im2col input and writes e4m3).  ELEM = OUT = s8: s32 accumulators over the whole K (the host sets chunk_iters to
-// it), and the per-channel epilogue t = acc * f_c + b'_c (no FMA) before cvt.rni.sat.s8.
+// it), and the per-channel epilogue t = acc * f_c + b'_c (no FMA) before cvt.rni.sat.s8.  ELEM = u8 (PE_PREC_FLAG_U8): the same
+// with u8 x s8 MMAs; OUT = u8: ReLU, then cvt.rni.sat.u8.
 template <int BN, int PLANES, int ELEM, int OUT>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcArgs a) {
@@ -250,8 +259,8 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     uint8_t* const wring = smem;                          // A windows
     uint8_t* const bring = smem + WS * S::A_BYTES;        // B tiles, written by the TMA multicasts of the whole cluster
     __shared__ __align__(8) uint64_t wfull[WS], wempty[WS], bfull[BS], bempty[BS];
-    constexpr bool S8 = ELEM == ELEM_S8;
-    __shared__ float s_bias[S8 ? 2 * BN : BN];   // s8: the biases, then the per-channel factors
+    constexpr bool S8 = ELEM == ELEM_S8 || ELEM == ELEM_U8;   // integer sums and the per-channel epilogue
+    __shared__ float s_bias[S8 ? 2 * BN : BN];   // s8 / u8: the biases, then the per-channel factors
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     // Row tiles start at every image, so none covers only the gap rows after an image's last pixel.  A CTA past the last
@@ -406,6 +415,9 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             } else if constexpr (OUT == ELEM_S8) {
                 if (co < cout8)
                     *(uint16_t*)((int8_t*)a.out + (size_t)m * a.out_pitch + a.out_coff + co) = (uint16_t)(f32_to_s8(v[0]) | f32_to_s8(v[1]) << 8);
+            } else if constexpr (OUT == ELEM_U8) {
+                if (co < cout8)
+                    *(uint16_t*)((uint8_t*)a.out + (size_t)m * a.out_pitch + a.out_coff + co) = (uint16_t)(f32_to_u8(v[0]) | f32_to_u8(v[1]) << 8);
             } else if (OUT == ELEM_E4M3) {
                 // round to nearest, saturating to +-448 as the range check expects (a larger |t| is PE_ERR_RANGE)
                 if (co < cout8)
@@ -459,10 +471,12 @@ static int launch_widths(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStrea
     }
 }
 
-// Layers with e4m3 output (conv_fp8.cu), s8 layers (conv_s8.cu) and the format boundaries of mixed engines (conv_mixed.cu):
+// Layers with e4m3 output (conv_fp8.cu), s8 layers (conv_s8.cu), the format boundaries of mixed engines (conv_mixed.cu) and
+// the layers that read or store u8 (conv_u8.cu):
 // their instances live in translation units of their own.
 int launch_e4m3(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap, int bn);
 int launch_s8(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap, int bn);
 int launch_mixed(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap, int bn);
+int launch_u8(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap, int bn);
 
 }  // namespace pe

@@ -45,6 +45,7 @@ struct pe_engine {
     ModelTables mt_own;     // model tables with the prototxt's nms max_peaks
     Geo geo[4];
     const Precision* prec = nullptr;   // the precision mode's row (precision.h)
+    bool u8 = false;                   // PE_PREC_FLAG_U8 (cfg.precision holds the mode without it): the plan's u8 activations
     std::vector<void*> acts;        // device
     std::vector<long long> act_plane;  // elements per plane
     std::vector<HostWeights> hw;    // per conv
@@ -317,18 +318,30 @@ extern "C" int pe_plan_describe(int model, const char* prototxt_path, char* buf,
 }
 
 static const char* elem_name(PlaneFmt f) {
-    static const char* names[] = {"bf16", "f16", "e4m3", "s8"};
+    static const char* names[] = {"bf16", "f16", "e4m3", "s8", "u8"};
     return f.planes == 0 ? "f32" : names[f.elem];
+}
+
+// A precision argument: the mode, and PE_PREC_FLAG_U8, which applies to PE_PREC_S8X1 only.  The mode alone selects every per-mode
+// fact; the flag only changes the plan's element kinds (plan.cpp).
+static int split_precision(int p, int* mode, bool* u8) {
+    *mode = p & ~PE_PREC_FLAG_U8;
+    *u8 = (p & PE_PREC_FLAG_U8) != 0;
+    if (*mode < 0 || *mode >= NUM_PRECISIONS) return fail(nullptr, PE_ERR_INVALID, "unknown precision %d", p);
+    if (*u8 && *mode != PE_PREC_S8X1)
+        return fail(nullptr, PE_ERR_INVALID, "PE_PREC_FLAG_U8 (u8 activations) applies to PE_PREC_S8X1 (6) only, not to precision %d: u8 "
+                    "activations are read by the integer MMA (u8 x s8)", *mode);
+    return PE_OK;
 }
 
 // The plan of `net` in mode `prec` with the conv layers of `f16_layers` (comma-separated names and "narrow"; NULL or empty: none)
 // in fp16.  Each element kind lays out its activations by its own row (elem_row); plan.cpp applies the format rules.  Mixing is
 // for the one-byte modes E4M3X1 and S8X1 only: the other modes' plane counts or element kinds differ from F16X1's.
-static int plan_for(const NetDef& net, int prec, const char* f16_layers, NetPlan& p, std::string& err) {
+static int plan_for(const NetDef& net, int prec, bool u8, const char* f16_layers, NetPlan& p, std::string& err) {
     const Precision& base = precision(prec);
     PlanFormats f;
-    f.base_elem = base.fmt.elem; f.input_elem = base.input_elem;
-    for (int k = 0; k < 4; k++) {
+    f.base_elem = base.fmt.elem; f.input_elem = base.input_elem; f.u8 = u8;
+    for (int k = 0; k < NUM_ELEMS; k++) {
         const Precision& r = elem_row(base, (PlaneElem)k);
         f.layout[k] = {r.act_cpad, r.kp_input, r.slot_align};
     }
@@ -350,13 +363,15 @@ static int plan_for(const NetDef& net, int prec, const char* f16_layers, NetPlan
 // Host-only view of the element kinds of a plan (DESIGN.md section 3): "act <index> <kind> <channel pitch> <blob or ->" per
 // activation, then "conv <name> <compute kind> <stored kind> <in_act> <out_act>" per conv layer; f32: the planar maps or the
 // FP32_SIMT mode.
-extern "C" int pe_plan_formats(int model, const char* prototxt_path, int prec, const char* f16_layers, char* buf, int cap) {
+extern "C" int pe_plan_formats(int model, const char* prototxt_path, int prec_arg, const char* f16_layers, char* buf, int cap) {
     NetDef net;
     std::string err;
-    if (prec < 0 || prec >= NUM_PRECISIONS) return -fail(nullptr, PE_ERR_INVALID, "unknown precision %d", prec);
+    int prec = 0;
+    bool u8 = false;
+    if (const int rc = split_precision(prec_arg, &prec, &u8)) return -rc;
     if (const int rc = query_net(model, prototxt_path, net)) return rc;
     NetPlan p;
-    if (plan_for(net, prec, f16_layers, p, err)) return -fail(nullptr, PE_ERR_INVALID, "%s", err.c_str());
+    if (plan_for(net, prec, u8, f16_layers, p, err)) return -fail(nullptr, PE_ERR_INVALID, "%s", err.c_str());
     const int planes = precision(prec).fmt.planes;
     std::string s;
     char t[512];
@@ -382,7 +397,7 @@ extern "C" int pe_prune_2to4(int model, const char* prototxt_path, const char* l
     std::string err;
     if (const int rc = query_net(model, prototxt_path, net)) return rc;
     NetPlan p;
-    if (plan_for(net, PE_PREC_S8X1, nullptr, p, err)) return -fail(nullptr, PE_ERR_INVALID, "%s", err.c_str());
+    if (plan_for(net, PE_PREC_S8X1, false, nullptr, p, err)) return -fail(nullptr, PE_ERR_INVALID, "%s", err.c_str());
     for (const ConvSpec& c : p.convs) {
         if (c.name != layer) continue;
         if (c.im2col_input) return -fail(nullptr, PE_ERR_INVALID, "pe_prune_2to4: layer %s reads the im2col'ed net input and always runs dense", layer);
@@ -404,8 +419,9 @@ extern "C" int pe_create_from_prototxt(const pe_config* cfg, const char* prototx
     return create_impl(cfg, prototxt_path, nullptr, out);
 }
 extern "C" int pe_create_mixed(const pe_config* cfg, const char* prototxt_path, const char* f16_layers, pe_engine** out) {
-    if (cfg && cfg->precision != PE_PREC_E4M3X1 && cfg->precision != PE_PREC_S8X1)
-        return fail(nullptr, PE_ERR_INVALID, "pe_create_mixed: the base precision must be PE_PREC_E4M3X1 (5) or PE_PREC_S8X1 (6), not %d", cfg->precision);
+    const int mode = cfg ? cfg->precision & ~PE_PREC_FLAG_U8 : 0;
+    if (cfg && mode != PE_PREC_E4M3X1 && mode != PE_PREC_S8X1)
+        return fail(nullptr, PE_ERR_INVALID, "pe_create_mixed: the base precision must be PE_PREC_E4M3X1 (5) or PE_PREC_S8X1 (6), not %d", mode);
     return create_impl(cfg, prototxt_path, f16_layers, out);
 }
 
@@ -414,14 +430,15 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, const
     *out = nullptr;
     pe_config cfg_copy = *cfg_in;
     pe_config* cfg = &cfg_copy;
-    if (cfg->precision < 0 || cfg->precision >= NUM_PRECISIONS) return fail(nullptr, PE_ERR_INVALID, "unknown precision %d", cfg->precision);
+    bool u8 = false;
+    if (const int rc = split_precision(cfg_in->precision, &cfg->precision, &u8)) return rc;
     const Precision& prec = precision(cfg->precision);
     NetDef netdef;
     NetPlan plan;
     if (prototxt_path) {
         std::string perr;
         if (parse_prototxt_file(prototxt_path, netdef, perr)) return fail(nullptr, PE_ERR_IO, "%s: %s", prototxt_path, perr.c_str());
-        if (plan_for(netdef, cfg->precision, f16_layers, plan, perr))
+        if (plan_for(netdef, cfg->precision, u8, f16_layers, plan, perr))
             return fail(nullptr, PE_ERR_INVALID, "%s: %s", prototxt_path, perr.c_str());
         if (cfg->model >= 0 && cfg->model != plan.model)
             return fail(nullptr, PE_ERR_INVALID, "%s describes the %s model (nms num_parts %d), the configuration asks for model %d", prototxt_path,
@@ -431,7 +448,7 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, const
     if (cfg->model != PE_MODEL_MPI_15 && cfg->model != PE_MODEL_COCO_18) return fail(nullptr, PE_ERR_INVALID, "unknown model %d", cfg->model);
     if (!prototxt_path) {
         std::string perr;
-        if (plan_for(builtin_netdef(cfg->model, 6), cfg->precision, f16_layers, plan, perr)) return fail(nullptr, PE_ERR_INVALID, "%s", perr.c_str());
+        if (plan_for(builtin_netdef(cfg->model, 6), cfg->precision, u8, f16_layers, plan, perr)) return fail(nullptr, PE_ERR_INVALID, "%s", perr.c_str());
     }
     if (cfg->net_w <= 0 || cfg->net_h <= 0 || cfg->net_w % 8 || cfg->net_h % 8)
         return fail(nullptr, PE_ERR_INVALID, "net resolution %dx%d must be positive multiples of 8", cfg->net_w, cfg->net_h);
@@ -452,6 +469,7 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, const
     if (prototxt_path) e->mt_own.max_peaks = plan.nms_max_peaks;   // nms_param.max_peaks (NmsLayer::GetMaxPeaks, rtpose.cpp:195)
     e->mt = &e->mt_own;
     e->prec = &prec;
+    e->u8 = u8;
     if (const char* g = getenv("PE_CHECK_RANGE")) e->check_range = atoi(g) != 0;
     e->start_scale_f = (float)cfg->start_scale;  // ImResizeLayer::SetStartScale(float)
     e->scale_gap_f = (float)cfg->scale_gap;
@@ -469,12 +487,14 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, const
 
     // the plan first: each level's gap is the largest pad of its convolutions (common.h)
     e->plan = plan;
-    for (const ConvSpec& c : e->plan.convs)   // the s8 bound of the layers that compute in s8
+    for (const ConvSpec& c : e->plan.convs)   // the s32 bound of the layers that compute in s8 or u8
         if (const long long max_k = elem_row(prec, (PlaneElem)c.elem).max_k) {
             const long long K = (long long)(c.im2col_input ? 1 : c.k * c.k) * c.in_cused;
+            const bool cu8 = c.elem == ELEM_U8;
             if (K > max_k) {
-                fail(e, PE_ERR_INVALID, "layer %s: K = %lld (%dx%d taps x %d padded input channels) exceeds %lld, the largest K whose s8 sums "
-                     "stay inside s32 (|acc| <= 128 x 127 x K): PE_PREC_S8X1 cannot run it", c.name.c_str(), K, c.k, c.k, c.in_cused, max_k);
+                fail(e, PE_ERR_INVALID, "layer %s: K = %lld (%dx%d taps x %d padded input channels) exceeds %lld, the largest K whose %s sums "
+                     "stay inside s32 (|acc| <= %s x 127 x K): PE_PREC_S8X1%s cannot run it", c.name.c_str(), K, c.k, c.k, c.in_cused, max_k,
+                     cu8 ? "u8 x s8" : "s8", cu8 ? "255" : "128", cu8 ? " with u8 activations" : "");
                 return bail(PE_ERR_INVALID);
             }
         }
@@ -750,7 +770,7 @@ static int pack_conv_weights(pe_engine* e, int i, uint8_t* dst) {
     const PlaneFmt wf = conv_wfmt(e, i);
     memset(dst, 0, weight_bytes(e, i));
     float wscale_inv = 1.f;
-    if (wf.s8()) {
+    if (wf.s8() || wf.u8()) {   // a u8 layer's weights are s8 too: its MMA is u8 x s8
         // a sparse layer quantises into a dense plane first and stores it compressed (s8_sparse.h); quantisation only adds zeros
         std::vector<int8_t> dense(e->sparse[i] ? K * cop : 0);
         int8_t* q = e->sparse[i] ? dense.data() : (int8_t*)dst;
@@ -841,16 +861,19 @@ static int bind_packed(pe_engine* e) {
 //      every class of the shipped nets (DESIGN.md section 5: 7x7, first 7x7 of a stage, VGG 3x3, stage-1 3x3, conv1_x and 1x1,
 //      1.2-2.2x the dense kernel's time), and no other shape has been measured, so no class qualifies and every layer runs dense.
 //      pe_test_force_sparse lifts this rule, so that tests and tools/sparse_s8.py can run and measure the kernel.
-// (Rule 3, the 2:4 weights, is checked by commit.)
+// (Rule 3, the 2:4 weights, is checked by commit.)  An engine with u8 activations (PE_PREC_FLAG_U8) runs every layer dense: the
+// sparse kernel is s8 x s8 only.
 static bool sparse_eligible(const pe_engine* e, int i) {
     const ConvSpec& c = e->plan.convs[i];
-    return e->force_sparse && conv_wfmt(e, i).s8() && conv_out_elem(e, i) == ELEM_S8 && !c.im2col_input;
+    return e->force_sparse && !e->u8 && conv_wfmt(e, i).s8() && conv_out_elem(e, i) == ELEM_S8 && !c.im2col_input;
 }
 
 // Test hook, not part of the public header: with on != 0 the next pe_commit_weights of e picks the sparse kernel for every layer
-// that rules 1-3 of sparse_eligible admit, ignoring the shape rule.  Returns 0, or PE_ERR_INVALID for a null handle.
+// that rules 1-3 of sparse_eligible admit, ignoring the shape rule.  Returns 0, or PE_ERR_INVALID for a null handle or an engine
+// with u8 activations.
 extern "C" int pe_test_force_sparse(pe_engine* e, int on) {
     if (!e) return PE_ERR_INVALID;
+    if (e->u8 && on) return fail(e, PE_ERR_INVALID, "pe_test_force_sparse: an engine with u8 activations runs no layer sparse (the sparse kernel is s8 x s8)");
     e->force_sparse = on != 0;
     return PE_OK;
 }
@@ -907,6 +930,7 @@ extern "C" int pe_share_weights(pe_engine* from, pe_engine* to) {
     if (to->cfg.device != from->cfg.device) return fail(from, PE_ERR_INVALID, "handles are on different GPUs (use pe_broadcast_weights)");
     if (to->cfg.model != from->cfg.model || to->cfg.precision != from->cfg.precision || to->plan.convs.size() != from->plan.convs.size())
         return fail(from, PE_ERR_INVALID, "the handles run different nets (model / precision / graph)");
+    if (to->u8 != from->u8) return fail(from, PE_ERR_INVALID, "one handle has u8 activations (PE_PREC_FLAG_U8), the other not");
     for (size_t i = 0; i < to->plan.convs.size(); i++) {
         const ConvSpec &a = from->plan.convs[i], &b = to->plan.convs[i];
         if (a.name != b.name || a.cout != b.cout || a.cin != b.cin || a.k != b.k) return fail(from, PE_ERR_INVALID, "layer %s differs between the handles", a.name.c_str());
@@ -949,6 +973,7 @@ extern "C" int pe_broadcast_weights(pe_engine* const* engines, int n) {
         if (!e || e->cfg.model != root->cfg.model || e->cfg.precision != root->cfg.precision || e->cfg.net_w != root->cfg.net_w ||
             e->cfg.net_h != root->cfg.net_h)
             return fail(root, PE_ERR_INVALID, "engine %d is not a replica of engine 0 (model / precision / net size differ)", i);
+        if (e->u8 != root->u8) return fail(root, PE_ERR_INVALID, "engine %d is not a replica of engine 0 (u8 activations in one only)", i);
         bool same = e->plan.convs.size() == root->plan.convs.size();
         for (size_t l = 0; same && l < e->plan.convs.size(); l++) same = e->plan.convs[l].elem == root->plan.convs[l].elem;
         if (!same) return fail(root, PE_ERR_INVALID, "engine %d is not a replica of engine 0 (the fp16 layers differ)", i);
@@ -1685,7 +1710,7 @@ static void fold_range(pe_engine* e, const std::vector<unsigned>& bits) {
 
 // Largest |stored value| / range_limit (precision.h) over the conv layers since the last call.  PE_ERR_RANGE when a layer
 // reached that limit, or when a layer's maximum fell below range_floor; both from the row of the kind the layer stores (out_row).
-// s8: the largest stored value is rint(max |t|).  *layer64 names the worst layer.
+// s8, u8: the largest stored value is rint(max |t|).  *layer64 names the worst layer.
 extern "C" int pe_range_status(pe_engine* e, float* worst_ratio, char* layer64) {
     if (!e) return PE_ERR_INVALID;
     if (worst_ratio) *worst_ratio = 0.f;
@@ -1705,7 +1730,7 @@ extern "C" int pe_range_status(pe_engine* e, float* worst_ratio, char* layer64) 
         const Precision& p = out_row(e, (int)i);
         float m; memcpy(&m, &bits[i], 4);
         if (bits[i] == 0) continue;                   // layer did not run since the last call
-        if (p.fmt.s8() && m <= 3e38f) m = rintf(m);   // the kernels track |t| before the rounding: the stored value
+        if ((p.fmt.s8() || p.fmt.u8()) && m <= 3e38f) m = rintf(m);   // the kernels track |t| before the rounding: the stored value
         if (!(m <= 3e38f) || m / p.range_limit > worst) { worst = (m <= 3e38f) ? m / p.range_limit : 2.f; iw = (int)i; }
         if (m / p.range_floor < lowest) { lowest = m / p.range_floor; smallest = m; is = (int)i; }
     }
@@ -1735,7 +1760,7 @@ extern "C" int pe_range_status(pe_engine* e, float* worst_ratio, char* layer64) 
 // The engine's table: every conv layer that stores an activation, with its stored kind and log2 scale
 static CalibTable engine_table(pe_engine* e) {
     CalibTable t;
-    t.precision = e->cfg.precision;
+    t.precision = e->cfg.precision | (e->u8 ? PE_PREC_FLAG_U8 : 0);   // an S8X1 table and a u8 table refuse each other
     if (!e->weights_hash_valid) {   // name, fp32 weights, fp32 biases of every conv layer in plan order
         Fnv1a64 h;
         for (size_t i = 0; i < e->plan.convs.size(); i++) {

@@ -212,6 +212,23 @@ int build_plan_from_net(const NetDef& net, const PlanFormats& fm, NetPlan& p, st
         auto it = group_elem.find(root(blob));
         return it == group_elem.end() ? fm.base_elem : it->second;
     };
+    // u8 (PlanFormats::u8): a group of kind s8 - every conv layer that reads it computes in s8 - whose every writer is a conv layer
+    // followed by ReLU (a pool writes into its input's group) holds values >= 0 only: it is stored as u8.  The net input (p - 128)
+    // and a group that a layer without ReLU writes (the Concat buffers with the stage outputs, and so conv4_4_CPM's output) stay s8.
+    if (fm.u8) {
+        std::map<std::string, bool> nonneg;   // group -> every writer so far is a conv layer followed by ReLU
+        nonneg[root(input_blob)] = false;
+        for (int i = 0; i < NL; i++) {
+            const ProtoLayer& l = net.layers[i];
+            if (l.type != "Convolution") continue;
+            bool relu = false;
+            for (int u : consumers[l.tops[0]]) relu = relu || net.layers[u].type == "ReLU";
+            const std::string g = root(l.tops[0]);
+            nonneg[g] = (nonneg.count(g) ? nonneg[g] : true) && relu;
+        }
+        for (const auto& g : nonneg)
+            if (g.second && elem_of(g.first) == ELEM_S8) group_elem[g.first] = ELEM_U8;
+    }
     const int cc_elem = concats.empty() ? fm.base_elem : elem_of(net.layers[concats[0]].tops[0]);
     const int cpad = fm.layout[cc_elem].cpad, slot_align = fm.layout[cc_elem].slot_align;   // of the concat buffers
 
@@ -293,7 +310,8 @@ int build_plan_from_net(const NetDef& net, const PlanFormats& fm, NetPlan& p, st
             c.name = l.name; c.cout = l.num_output; c.k = l.kernel; c.pad = l.pad; c.level = level[top];
             c.relu = 0;
             for (int u : consumers[top]) if (net.layers[u].type == "ReLU") c.relu = 1;
-            c.planar_coff = 0; c.out_coff = 0; c.flops_per_image = 0; c.im2col_input = 0; c.elem = conv_elem(i);
+            c.planar_coff = 0; c.out_coff = 0; c.flops_per_image = 0; c.im2col_input = 0;
+            c.elem = elem_of(l.bottoms[0]) == ELEM_U8 ? (int)ELEM_U8 : conv_elem(i);   // a reader of u8 computes u8 x s8
             // input
             if (l.bottoms[0] == input_blob) {
                 if (l.kernel != 3) return fail("layer " + l.name + ": the first convolution must be 3x3 (it consumes the im2col'ed input)");

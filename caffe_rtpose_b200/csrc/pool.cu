@@ -84,10 +84,12 @@ __global__ void __launch_bounds__(256) pool_planes_kernel(PoolArgs a) {
         *((uint4*)((__nv_bfloat16*)a.out + (size_t)p * a.out_plane + mo * a.C) + g) = o[p];
 }
 
-// e4m3 / s8 (one byte per channel): 16 channels per thread.  Rounding is monotone, so the max of the stored values is the stored
-// max: the winner's byte is copied.
-template <bool S8> __device__ __forceinline__ float byte_value(uint8_t b) { return S8 ? (float)(int8_t)b : e4m3_to_float(b); }
-template <bool S8>
+// e4m3 / s8 / u8 (one byte per channel): 16 channels per thread.  Rounding is monotone, so the max of the stored values is the
+// stored max: the winner's byte is copied.
+template <int ELEM> __device__ __forceinline__ float byte_value(uint8_t b) {
+    return ELEM == ELEM_S8 ? (float)(int8_t)b : ELEM == ELEM_U8 ? (float)b : e4m3_to_float(b);
+}
+template <int ELEM>
 __global__ void __launch_bounds__(256) pool_bytes_kernel(PoolArgs a) {
     const unsigned cv = a.C / 16;
     const int n = blockIdx.y;
@@ -112,11 +114,11 @@ __global__ void __launch_bounds__(256) pool_bytes_kernel(PoolArgs a) {
 #pragma unroll
     for (int j = 0; j < 16; j++) {
         uint8_t b = ((const uint8_t*)&v[0])[j];
-        float best = byte_value<S8>(b);
+        float best = byte_value<ELEM>(b);
 #pragma unroll
         for (int w = 1; w < 4; w++) {
             const uint8_t c = ((const uint8_t*)&v[w])[j];
-            const float f = byte_value<S8>(c);
+            const float f = byte_value<ELEM>(c);
             if (ok[w] && f > best) { best = f; b = c; }
         }
         ((uint8_t*)&o)[j] = b;
@@ -130,10 +132,12 @@ int launch_pool(const PoolArgs& a, cudaStream_t st) {
     if (f.planes == 0) {
         const long long total = rows_out * (a.C / 4);
         pool_f32_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(a);
-    } else if (f.e4m3() || f.s8()) {
+    } else if (f.e4m3() || f.s8() || f.u8()) {
         const unsigned per = (unsigned)a.Hso * a.Wpo * (a.C / 16);
-        if (f.s8()) pool_bytes_kernel<true><<<dim3((per + 255) / 256, a.N), 256, 0, st>>>(a);
-        else pool_bytes_kernel<false><<<dim3((per + 255) / 256, a.N), 256, 0, st>>>(a);
+        const dim3 grid((per + 255) / 256, a.N);
+        if (f.s8()) pool_bytes_kernel<ELEM_S8><<<grid, 256, 0, st>>>(a);
+        else if (f.u8()) pool_bytes_kernel<ELEM_U8><<<grid, 256, 0, st>>>(a);
+        else pool_bytes_kernel<ELEM_E4M3><<<grid, 256, 0, st>>>(a);
     } else {
         const unsigned per = (unsigned)a.Hso * a.Wpo * (a.C / 8);
         const dim3 grid((per + 255) / 256, a.N);
@@ -180,6 +184,7 @@ __global__ void __launch_bounds__(256) act_to_nchw_kernel(const void* act, int p
     if (fmt.planes == 0) v = ((const float*)act)[m * pitch + coff + ch];
     else if (fmt.e4m3()) v = e4m3_to_float(((const uint8_t*)act)[m * pitch + coff + ch]);
     else if (fmt.s8()) v = (float)((const int8_t*)act)[m * pitch + coff + ch];
+    else if (fmt.u8()) v = (float)((const uint8_t*)act)[m * pitch + coff + ch];
     else for (int p = 0; p < fmt.planes; p++) {
         const uint16_t h = ((const uint16_t*)act)[p * plane + m * pitch + coff + ch];
         v += fmt.f16() ? plane_to_float<true>(h) : plane_to_float<false>(h);

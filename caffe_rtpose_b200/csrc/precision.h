@@ -9,8 +9,10 @@
 namespace pe {
 
 // Element kind of a storage plane.  Facts that depend on the kind alone are functions of it.
-enum PlaneElem { ELEM_BF16 = 0, ELEM_F16 = 1, ELEM_E4M3 = 2, ELEM_S8 = 3 };
-__host__ __device__ constexpr int elem_size(PlaneElem e) { return e == ELEM_E4M3 || e == ELEM_S8 ? 1 : 2; }   // bytes
+// ELEM_U8: the non-negative activations of PE_PREC_S8X1 | PE_PREC_FLAG_U8 (plan.cpp), read as u8 against s8 weights.
+enum PlaneElem { ELEM_BF16 = 0, ELEM_F16 = 1, ELEM_E4M3 = 2, ELEM_S8 = 3, ELEM_U8 = 4 };
+constexpr int NUM_ELEMS = 5;
+__host__ __device__ constexpr int elem_size(PlaneElem e) { return e == ELEM_E4M3 || e == ELEM_S8 || e == ELEM_U8 ? 1 : 2; }   // bytes
 // pack_conv_weights scales a layer's weights by a power of two so that max|w| lies in [2^(top-1), 2^top): fp16 [2^13, 2^14) keeps
 // the lo plane of small weights out of the subnormals, e4m3 [128, 256) stays below the largest finite 448 and keeps weights down to
 // max|w| * 2^-13 normal.  0: no scaling (bf16 has fp32's range; s8 scales each output channel, s8.h).  A fact of the element kind,
@@ -23,6 +25,7 @@ struct PlaneFmt {
     __host__ __device__ bool f16() const { return elem == ELEM_F16; }
     __host__ __device__ bool e4m3() const { return elem == ELEM_E4M3; }
     __host__ __device__ bool s8() const { return elem == ELEM_S8; }
+    __host__ __device__ bool u8() const { return elem == ELEM_U8; }
     __host__ __device__ int elem_bytes() const { return planes == 0 ? 4 : elem_size(elem); }
 };
 
@@ -68,10 +71,20 @@ constexpr int NUM_PRECISIONS = sizeof PRECISIONS / sizeof PRECISIONS[0];
 static_assert(NUM_PRECISIONS == PE_PREC_S8X1 + 1, "one row per PE_PREC_* mode");
 inline const Precision& precision(int pe_prec) { return PRECISIONS[pe_prec]; }   // pe_prec in [0, NUM_PRECISIONS)
 
+// The u8 activations of PE_PREC_S8X1 | PE_PREC_FLAG_U8 (plan.cpp: post-ReLU values read only by integer layers), outside
+// PRECISIONS since they are no mode of their own.  S8X1's layout and per-channel epilogue; u8 x s8 sums, |acc| <= 255 x 127 x K,
+// stay inside s32 up to K = 66311.  Calibration target [64, 128): the sign bit s8 spends on these values goes to one more bit
+// of magnitude, with the 2-4x headroom of S8X1's [32, 64).  Range limit 255, floor 8 (under 3 bits, as S8X1's 4).
+inline constexpr Precision U8_ACTIVATIONS =
+    {{1, ELEM_U8}, ELEM_S8, 128, 128, 16, false, 7, 255.f, 8.f, "8", "the u8 planes", 256.f, true, 66311, true};
+static_assert(255LL * 127 * 66311 <= 2147483647LL && 255LL * 127 * 66312 > 2147483647LL, "66311: the largest K of a u8 layer");
+
 // The row of a layer or activation of element kind k in an engine of mode `base`.  The one-plane 16-bit and 8-bit modes give
-// each kind one row - fp16: F16X1, e4m3: E4M3X1, s8: S8X1 - so that a layer of another kind than the mode's (E4M3X1's fp16 net
-// input, the fp16 layers of pe_create_mixed) follows its own kind's arithmetic, pads and range.  Other modes: their own row.
+// each kind one row - fp16: F16X1, e4m3: E4M3X1, s8: S8X1, u8: U8_ACTIVATIONS - so that a layer of another kind than the mode's
+// (E4M3X1's fp16 net input, the fp16 layers of pe_create_mixed, the u8 layers of PE_PREC_FLAG_U8) follows its own kind's
+// arithmetic, pads and range.  Other modes: their own row.
 inline const Precision& elem_row(const Precision& base, PlaneElem k) {
+    if (k == ELEM_U8) return U8_ACTIVATIONS;
     if (base.fmt.planes != 1 || k == ELEM_BF16) return base;
     return precision(k == ELEM_F16 ? PE_PREC_F16X1 : k == ELEM_E4M3 ? PE_PREC_E4M3X1 : PE_PREC_S8X1);
 }

@@ -23,6 +23,7 @@ PREC_F16X2 = PREC_BF16X2   # the parity mode: 2 fp16 planes, chunked round-to-ne
 PREC_F16X1 = 4             # the fast mode: the parity mode's hi plane alone, one MMA per MAC (poseengine.h)
 PREC_E4M3X1 = 5            # the FP8 mode: one e4m3 plane, one FP8 MMA per MAC; needs calibrate() (poseengine.h)
 PREC_S8X1 = 6              # the INT8 mode: one s8 plane, one s8 MMA per MAC, exact s32 sums; forward needs calibrate() first
+PREC_FLAG_U8 = 0x100       # PREC_S8X1 only: post-ReLU activations stored as u8, their layers u8 x s8 (poseengine.h)
 MAX_PEOPLE = 96
 # pixel formats of forward_pixels / pixels_to_bgr (PE_PIX_*, poseengine.h)
 PIX_BGR, PIX_RGB, PIX_YUYV, PIX_NV12, PIX_I420 = 0, 1, 2, 3, 4
@@ -285,14 +286,17 @@ class PoseEngine:
     """One GPU worker (the reference's NetCopy + warmup(), rtpose.cpp:133-142, 173-237)."""
 
     def __init__(self, model=COCO_18, net_w=656, net_h=368, disp_w=1280, disp_h=720, num_scales=1, start_scale=1.0,
-                 scale_gap=0.3, device=0, max_batch=1, precision=PREC_BF16X2, prototxt=None, f16_layers=None):
+                 scale_gap=0.3, device=0, max_batch=1, precision=PREC_BF16X2, prototxt=None, f16_layers=None,
+                 u8_activations=False):
         """prototxt: path of a deploy prototxt (`new caffe::Net(proto, TEST)`, rtpose.cpp:183); model may then be None
         and follows the Nms layer's num_parts (rtpose.cpp:212-229).  Without it the built-in graph of `model` is used.
         f16_layers: conv layer names (a list or a comma-separated string, "narrow" included) that run with PREC_F16X1's
-        arithmetic inside a PREC_E4M3X1 or PREC_S8X1 engine (pe_create_mixed); see plan_formats."""
+        arithmetic inside a PREC_E4M3X1 or PREC_S8X1 engine (pe_create_mixed); see plan_formats.
+        u8_activations: with PREC_S8X1, store the activations that only hold values >= 0 (post-ReLU, read only by integer
+        layers) as u8 and run their readers u8 x s8 (PE_PREC_FLAG_U8); any other precision refuses it."""
         L = lib()
         cfg = _Config(device, -1 if model is None else model, net_w, net_h, disp_w, disp_h, num_scales, start_scale, scale_gap,
-                      max_batch, precision)
+                      max_batch, precision | (PREC_FLAG_U8 if u8_activations else 0))
         h = C.c_void_p()
         if f16_layers is not None:
             path = os.fsencode(prototxt) if prototxt is not None else None
@@ -651,10 +655,12 @@ def _layer_list(layers):
     return (layers if isinstance(layers, str) else ",".join(layers)).encode()
 
 
-def plan_formats(model=None, precision=PREC_E4M3X1, f16_layers=None, prototxt=None):
+def plan_formats(model=None, precision=PREC_E4M3X1, f16_layers=None, prototxt=None, u8_activations=False):
     """Element kinds of the plan pe_create_mixed builds (host only, no GPU): {"acts": [(kind, channel pitch, blob or None)],
-    "convs": {name: (compute kind, stored kind, in_act, out_act)}}.  f16_layers None or empty: the plain plan of `precision`."""
+    "convs": {name: (compute kind, stored kind, in_act, out_act)}}.  f16_layers None or empty: the plain plan of `precision`.
+    u8_activations: the plan of PoseEngine(..., u8_activations=True)."""
     L = lib()
+    precision |= PREC_FLAG_U8 if u8_activations else 0
     path = os.fsencode(prototxt) if prototxt is not None else None
     layers = _layer_list(f16_layers) if f16_layers is not None else None
     m = -1 if model is None else model

@@ -30,6 +30,7 @@
 #include <memory>
 #include <mutex>
 #include <queue>
+#include <sstream>
 #include <string>
 #include <thread>
 #include <vector>
@@ -98,6 +99,9 @@ static void define_flags() {
     define("f16_layers", "", "[extension] with --precision 5 or 6: comma-separated conv layers that run in fp16 with --precision 4's arithmetic "
            "while the others keep the FP8 / INT8 format; 'narrow' = the layers that read fewer than 128 channels (conv1_1, conv1_2, conv2_1). "
            "Layers that read one buffer go together (pe_create_mixed); empty = none");
+    define("u8_activations", "false", "[extension] with --precision 6 and --calibrate_range: store the activations that hold only values >= 0 "
+           "(post-ReLU, read only by INT8 layers) as u8 and run the layers that read them as u8 x s8 MMAs, one more bit at the s8 rate "
+           "(PE_PREC_FLAG_U8); --f16_layers, --calibration_*, --save_calibration and --audit_every work with it", true);
     define("batch", "0", "[extension] frames per forward per GPU: 1 = the reference's behaviour, 0 = automatic (file / synthetic sources "
            "fill two waves of 128-row tiles on the GPU, e.g. 9 frames at 656x368; results do not depend on it)");
     define("engines_per_gpu", "0", "[extension] worker handles per GPU: 1 = the reference's topology (one Net per GPU), 0 = automatic (2 when "
@@ -714,7 +718,9 @@ static int load_weights(pe_engine* e, int device) {   // CopyTrainedLayersFrom (
 struct CalibImage { int w, h; std::vector<uint8_t> bgr; };
 static std::vector<CalibImage> g_calib_images;
 
-static bool ranged_precision(int p) { return p == PE_PREC_F16X2 || p == PE_PREC_F16X1 || p == PE_PREC_E4M3X1 || p == PE_PREC_S8X1; }
+static bool ranged_precision(int p) {
+    p &= ~PE_PREC_FLAG_U8;
+    return p == PE_PREC_F16X2 || p == PE_PREC_F16X1 || p == PE_PREC_E4M3X1 || p == PE_PREC_S8X1; }
 
 static std::string calibration_table_of(pe_engine* e) {
     const int n = pe_calibration_get(e, nullptr, 0);
@@ -752,6 +758,9 @@ static bool calibrate_on_images(pe_engine* e, int dev) {
     return false;
 }
 
+// --precision with PE_PREC_FLAG_U8 when --u8_activations is set
+static int serve_precision() { return Fi("precision") | (Fb("u8_activations") ? PE_PREC_FLAG_U8 : 0); }
+
 static bool create_engines(int num_gpu, int per_gpu, int precision, const std::string& f16_layers, std::vector<pe_engine*>& engines,
                            bool serving) {
     const int batch = global.batch;
@@ -769,11 +778,28 @@ static bool create_engines(int num_gpu, int per_gpu, int precision, const std::s
         engines.push_back(e);
     }
     if (load_weights(engines[0], Fi("start_device"))) return false;
-    if (precision == PE_PREC_S8X1) {   // layers the 2:4-sparse s8 kernel runs (pe_conv_layer_sparse's rules)
+    if ((precision & ~PE_PREC_FLAG_U8) == PE_PREC_S8X1) {   // layers the 2:4-sparse s8 kernel runs (pe_conv_layer_sparse's rules)
         const int n = pe_num_conv_layers(engines[0]);
         int sparse = 0;
         for (int i = 0; i < n; i++) sparse += pe_conv_layer_sparse(engines[0], i) == 1;
         LOG_INFO("GPU %d: %d of %d conv layers run 2:4 sparse", Fi("start_device"), sparse, n);
+    }
+    if (precision & PE_PREC_FLAG_U8) {   // conv layers that read u8 activations: "conv <name> u8 ..." lines of the plan
+        const std::string path = F("caffeproto");
+        const char* proto = global.proto_readable ? path.c_str() : nullptr;
+        const int len = pe_plan_formats(global.model, proto, precision, f16_layers.c_str(), nullptr, 0);
+        std::string text(len > 0 ? len + 1 : 1, '\0');
+        int u8 = 0, n = 0;
+        if (len > 0 && pe_plan_formats(global.model, proto, precision, f16_layers.c_str(), &text[0], len + 1) == len) {
+            std::istringstream in(text.c_str());
+            for (std::string line; std::getline(in, line);) {
+                std::istringstream f(line);
+                std::string what, name, kind;
+                f >> what >> name >> kind;
+                if (what == "conv") { n++; u8 += kind == "u8"; }
+            }
+        }
+        LOG_INFO("GPU %d: %d of %d conv layers read u8 activations", Fi("start_device"), u8, n);
     }
     const bool calibrate = Fb("calibrate_range") && ranged_precision(precision);
     auto calibrate_engine = [&](pe_engine* e, int dev) {
@@ -1213,6 +1239,10 @@ int main(int argc, char** argv) {
     }
     if (F("frame_format") != "jpg" && F("frame_format") != "bmp") { LOG_ERROR("--frame_format must be jpg or bmp"); return 1; }
     if (Fi("audit_every") < 0) { LOG_ERROR("--audit_every must be 0 (off) or a positive number of batches"); return 1; }
+    if (Fb("u8_activations") && (Fi("precision") != PE_PREC_S8X1 || !Fb("calibrate_range"))) {
+        LOG_ERROR("--u8_activations is a variant of the INT8 mode on calibrated range scales: it needs --precision 6 with --calibrate_range");
+        return 1;
+    }
     if (Fi("precision") == PE_PREC_S8X1 && !Fb("calibrate_range")) {
         LOG_ERROR("--precision 6 (INT8) runs on calibrated per-layer range scales: at scale 1 almost every activation quantises to 0; drop --nocalibrate_range");
         return 1;
@@ -1299,7 +1329,7 @@ int main(int argc, char** argv) {
     if (global.proto_readable) LOG_INFO("Net built from %s", F("caffeproto").c_str());
     global.model = model;
     if (!F("f16_layers").empty() &&   // unknown names and lists that split a shared buffer, before any GPU call
-        pe_plan_formats(model, global.proto_readable ? F("caffeproto").c_str() : nullptr, Fi("precision"), F("f16_layers").c_str(), nullptr, 0) < 0) {
+        pe_plan_formats(model, global.proto_readable ? F("caffeproto").c_str() : nullptr, serve_precision(), F("f16_layers").c_str(), nullptr, 0) < 0) {
         LOG_ERROR("--f16_layers %s: %s", F("f16_layers").c_str(), pe_last_error(nullptr));
         return 1;
     }
@@ -1326,7 +1356,7 @@ int main(int argc, char** argv) {
     const int num_gpu = std::max(1, Fi("num_gpu"));
     std::vector<pe_engine*> engines, audit;
     const int per_gpu = global.engines_per_gpu, num_workers = num_gpu * per_gpu;
-    if (!create_engines(num_gpu, per_gpu, Fi("precision"), F("f16_layers"), engines, true) ||
+    if (!create_engines(num_gpu, per_gpu, serve_precision(), F("f16_layers"), engines, true) ||
         (Fi("audit_every") > 0 && !create_engines(num_gpu, per_gpu, PE_PREC_F16X2, "", audit, false))) {
         for (pe_engine* e : engines) pe_destroy(e);
         for (pe_engine* e : audit) pe_destroy(e);

@@ -65,6 +65,20 @@ extern "C" {
                              * the dense kernel's bits), chosen from the weights at pe_commit_weights by pe_conv_layer_sparse's
                              * rules; as built it is slower than the dense kernel in every measured layer class, so its shape
                              * rule keeps every layer dense.  DESIGN.md section 6. */
+#define PE_PREC_FLAG_U8 0x100 /* opt-in flag on PE_PREC_S8X1 (cfg->precision = PE_PREC_S8X1 | PE_PREC_FLAG_U8; with any other mode
+                             * PE_ERR_INVALID): u8 activations.  An activation is stored as u8 when every value written into it is
+                             * >= 0 - its producers are conv layers followed by ReLU, or max pools of such activations - and every
+                             * conv layer that reads it computes in the 8-bit integer kind (not the fp16 layers of pe_create_mixed).
+                             * The conv layers that read it run wgmma k32 u8 x s8 -> s32 (the s8 rate); weights stay s8, quantised
+                             * per channel as above.  Every other activation keeps its kind: the net input, the Concat buffers of
+                             * the stages (their L1 / L2 maps are signed) and conv4_4_CPM's output, which lives in them, stay s8.
+                             * A layer that stores u8 runs the same epilogue t = acc * f_c + b'_c without FMA, ReLU, then
+                             * cvt.rni.sat.u8 (round to nearest even into [0, 255]).  u8 activations are calibrated into [64, 128),
+                             * one more bit than s8's [32, 64) at the same 2-4x headroom; pe_range_status reports u8 layers against
+                             * 255 and a floor of 8.  |acc| <= 255 x 127 x K, so a layer that reads u8 with K > 66311 is refused
+                             * (PE_ERR_INVALID, the layer named).  No layer runs the 2:4-sparse kernel.  Calibration tables record
+                             * the precision with the flag (262): an S8X1 table and a u8 table refuse each other.  pe_share_weights
+                             * and pe_broadcast_weights need the flag on both sides.  DESIGN.md section 6. */
 
 #define PE_MAX_PEOPLE 96   /* RENDER_MAX_PEOPLE, renderFunctions.h:6 / rtpose.cpp:88 */
 
@@ -108,7 +122,8 @@ int pe_plan_describe(int model, const char* prototxt_path, char* buf, int cap);
 int pe_create_mixed(const pe_config* cfg, const char* prototxt_path, const char* f16_layers, pe_engine** out);
 /* host-only: the element kinds pe_create_mixed (or, with f16_layers NULL or "", pe_create / pe_create_from_prototxt of any
  * precision) gives the plan: "act <index> <kind> <channel pitch> <blob or ->" per activation, then "conv <name> <compute kind>
- * <stored kind> <in_act> <out_act>" per conv layer; kinds are f32, bf16, f16, e4m3, s8 (f32: the planar maps).  Returns the
+ * <stored kind> <in_act> <out_act>" per conv layer; kinds are f32, bf16, f16, e4m3, s8, u8 (f32: the planar maps; u8: precision
+ * PE_PREC_S8X1 | PE_PREC_FLAG_U8, whose flag is accepted here as by pe_create).  Returns the
  * text length as pe_plan_describe does, or -PE_ERR_INVALID with the reason in pe_last_error(NULL) for a list the rules refuse. */
 int pe_plan_formats(int model, const char* prototxt_path, int precision, const char* f16_layers, char* buf, int cap);
 void pe_destroy(pe_engine* e);

@@ -13,8 +13,8 @@ pe_compare_results against the parity mode at the north-star tolerance (1e-3 net
 the prototxt-filler net (gaussian(0.01) weights, maps ~3e-11), calibrated with pe_calibrate on the first frame.  The He-init
 maps are noise with thousands of near-tie NMS decisions, so these pose statistics are a worst case, not what a trained
 model shows.  FM_MODES also takes mixed-precision entries "<base>+<fp16 layers>" (pe_create_mixed), e.g. e4m3x1+narrow or
-s8x1+conv1_1+conv1_2: calibrated like their base and reported like the other modes.  Prints the card, its power limit and SM
-clocks, then one JSON line."""
+s8x1+conv1_1+conv1_2: calibrated like their base and reported like the other modes.  s8x1u8 is PE_PREC_S8X1 with u8 activations
+(PE_PREC_FLAG_U8), calibrated like s8x1.  Prints the card, its power limit and SM clocks, then one JSON line."""
 import json
 import os
 import statistics
@@ -33,8 +33,8 @@ from layer_times import klass  # noqa: E402
 
 MODEL, NET_W, NET_H, DISP_W, DISP_H, B = engine.COCO_18, 656, 368, 1280, 720, 9
 MODES = {"f16x2": engine.PREC_F16X2, "f16x1": engine.PREC_F16X1, "e4m3x1": engine.PREC_E4M3X1, "s8x1": engine.PREC_S8X1,
-         "bf16x1": engine.PREC_BF16X1}
-CALIBRATED = ("e4m3x1", "s8x1")
+         "bf16x1": engine.PREC_BF16X1, "s8x1u8": engine.PREC_S8X1 | engine.PREC_FLAG_U8}
+CALIBRATED = ("e4m3x1", "s8x1", "s8x1u8")
 
 
 def mode_spec(m):
@@ -162,7 +162,7 @@ def main():
     batch = [host[lb * B + k] for k in range(B)]
     filler = {}
     for m in MODES:
-        if m.partition("+")[0] in ("f16x2", "f16x1", "e4m3x1", "s8x1"):
+        if m.partition("+")[0] in ("f16x2", "f16x1") + CALIBRATED:
             e = make_engines(MODES[m], Wc, n=1, calibrate=[host[0]])[0]
             e.forward_frames(batch)
             filler[m] = results(e)
