@@ -43,7 +43,7 @@ extern "C" int pe_yuyv_to_bgr(const uint8_t* yuyv, int w, int h, long long strid
     for (int y = 0; y < h; y++) {
         const uint8_t* s = yuyv + (size_t)y * (size_t)stride;
         uint8_t* d = bgr + (size_t)y * w * 3;
-        for (int x = 0; x < w; x += 2, s += 4, d += 6) pe_pix::yuyv_pair(s, d);
+        for (int x = 0; x < w; x += 2, s += 4, d += 6) pe_pix::pair422(pe_pix::BT601_STUDIO, s, 0, d);
     }
     return PE_OK;
 }

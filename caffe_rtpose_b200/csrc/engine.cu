@@ -1419,6 +1419,8 @@ extern "C" int pe_forward_pixels(pe_engine* e, const pe_pixel_format* fmt, const
     bool any_host = false, any_pageable = false;
     for (int i = 0; i < n; i++) {
         if (!frames[i]) return fail(e, PE_ERR_INVALID, "null frame %d", i);
+        if (L.format == PE_PIX_P016 && ((uintptr_t)frames[i] & 1))
+            return fail(e, PE_ERR_INVALID, "odd P016 frame pointer %d: samples are 2 bytes", i);
         cudaPointerAttributes at;
         if (cudaPointerGetAttributes(&at, frames[i]) != cudaSuccess) { cudaGetLastError(); at.type = cudaMemoryTypeUnregistered; }
         if (at.type == cudaMemoryTypeDevice && at.device != e->cfg.device)
@@ -1439,7 +1441,7 @@ extern "C" int pe_forward_pixels(pe_engine* e, const pe_pixel_format* fmt, const
     }
     if (any_host && !bgr) { rc = grow_buffer(e, &e->d_pix, &e->pix_cap, stride * e->cfg.max_batch, false); if (rc) return rc; }
     PixArgs a;
-    a.dst = dst; a.pitch = L.pitch; a.chroma = L.chroma; a.format = L.format; a.w = L.w; a.h = L.h;
+    a.dst = dst; a.pitch = L.pitch; a.chroma = L.chroma; a.format = L.format; a.w = L.w; a.h = L.h; a.col = L.col;
     for (int i = 0; i < n; i++) {
         const uint8_t* src = (const uint8_t*)frames[i];
         if (kind[i] == PAGEABLE) { memcpy(e->h_raw + i * stride, src, span); src = e->h_raw + i * stride; }
@@ -1475,9 +1477,11 @@ extern "C" int pe_pixels_to_bgr(const pe_pixel_format* fmt, const void* frame, u
     std::string why;
     if (!pe_pix::layout_of(fmt, &L, &why)) return fail(nullptr, PE_ERR_INVALID, "%s", why.c_str());
     if (!frame || !bgr) return fail(nullptr, PE_ERR_INVALID, "null frame or output");
+    if (L.format == PE_PIX_P016 && ((uintptr_t)frame & 1)) return fail(nullptr, PE_ERR_INVALID, "odd P016 frame pointer: samples are 2 bytes");
     if (cap < 3LL * L.w * L.h) return fail(nullptr, PE_ERR_INVALID, "cap %lld is below the %lld bytes of the BGR frame", cap, 3LL * L.w * L.h);
     PixArgs a;
     a.src[0] = (const uint8_t*)frame; a.dst = bgr; a.pitch = L.pitch; a.chroma = L.chroma; a.format = L.format; a.w = L.w; a.h = L.h;
+    a.col = L.col;
     pixels_to_bgr_host(a);
     return PE_OK;
 }

@@ -3,6 +3,7 @@
 #include <cuda_fp8.h>
 
 #include "common.h"
+#include "pixels.cuh"    // pe_pix::Colour: the matrix and range of a decoder-format frame
 #include "precision.h"   // PlaneFmt: the storage format of the conv stack's activations and packed weights
 
 namespace pe {
@@ -128,9 +129,10 @@ struct PixArgs {
     const uint8_t* src[PIX_MAX_FRAMES];             // [n] frame starts (device pointers; the host reference reads src[0])
     uint8_t* dst;                                   // [n][h][w][3]
     long long pitch, chroma;                        // a checked pe_pix::Layout's
-    int format, w, h;
+    int format, w, h;                               // format: PE_PIX_* without the colour flags
+    pe_pix::Colour col;                             // the matrix and range the flags chose
 };
-int launch_pixels_to_bgr(const PixArgs& a, int n, cudaStream_t st);   // PE_PIX_RGB, _YUYV, _NV12, _I420
+int launch_pixels_to_bgr(const PixArgs& a, int n, cudaStream_t st);   // every format but PE_PIX_BGR
 void pixels_to_bgr_host(const PixArgs& a);                         // every format, frame src[0]
 
 // ---- convolution / pooling (conv_simt.cu, conv_tc.cu, pool.cu)

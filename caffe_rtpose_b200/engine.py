@@ -27,6 +27,11 @@ PREC_FLAG_U8 = 0x100       # PREC_S8X1 only: post-ReLU activations stored as u8,
 MAX_PEOPLE = 96
 # pixel formats of forward_pixels / pixels_to_bgr (PE_PIX_*, poseengine.h)
 PIX_BGR, PIX_RGB, PIX_YUYV, PIX_NV12, PIX_I420 = 0, 1, 2, 3, 4
+PIX_NV21, PIX_YV12, PIX_UYVY, PIX_P016, PIX_RGBP = 16, 17, 18, 19, 20
+# colour flags OR'ed into a YUV format (PE_PIX_FLAG_*): what forward_pixels's matrix= and full_range= set
+PIX_FLAG_BT709, PIX_FLAG_FULL_RANGE = 0x100, 0x200
+_PIX_FORMATS = (PIX_BGR, PIX_RGB, PIX_YUYV, PIX_NV12, PIX_I420, PIX_NV21, PIX_YV12, PIX_UYVY, PIX_P016, PIX_RGBP)
+_PIX_420 = (PIX_NV12, PIX_I420, PIX_NV21, PIX_YV12, PIX_P016)
 
 _f32p = np.ctypeslib.ndpointer(dtype=np.float32, flags="C_CONTIGUOUS")
 
@@ -425,19 +430,21 @@ class PoseEngine:
         self._ck(fn(self._h, ptrs, len(bufs), C.byref(s)))
         return s.value
 
-    def forward_pixels(self, frames, fmt, chroma_offset=None):
-        """frames: numpy arrays or torch tensors (host or CUDA) of one format and size, in cv2's shapes: (h*3/2, w) for PIX_NV12 /
-        PIX_I420, (h, w, 2) for PIX_YUYV, (h, w, 3) for PIX_RGB / PIX_BGR.  The row stride is the pitch, so a column slice of a
-        wider allocation is read in place (an I420 array of that shape is copied unless tight: its chroma rows are not pitch/2
-        apart).  chroma_offset (NV12 / I420): the frames are the (h, w) luma planes, the row stride is the pitch, and the chroma plane
-        starts chroma_offset bytes after each frame's start, e.g. pitch * 1088 in a 1080p NVDEC surface; the caller vouches that
-        the allocation reaches that far.  Converted to BGR on the GPU
-        as cv2.cvtColor does, then as forward_camera_frames.  CUDA frames are read on the engine's stream after the work queued so
-        far on torch's current stream.  Returns frame.scale."""
-        views = [_pixel_view(f, fmt, chroma_offset) for f in frames]
-        pf = views[0][1]
-        if any((v[1].width, v[1].height, v[1].pitch) != (pf.width, pf.height, pf.pitch) for v in views):
-            raise ValueError("forward_pixels: the frames of one call share their size and row stride")
+    def forward_pixels(self, frames, fmt, chroma_offset=None, matrix="bt601", full_range=False):
+        """frames: numpy arrays or torch tensors (host or CUDA) of one format and size, in cv2's shapes: (h*3/2, w) uint8 for
+        PIX_NV12 / PIX_NV21 / PIX_I420 / PIX_YV12, (h*3/2, w) uint16 for PIX_P016 (P010 / P012 / P016), (h, w, 2) for PIX_YUYV /
+        PIX_UYVY, (h, w, 3) for PIX_RGB / PIX_BGR, and (3, h, w) for PIX_RGBP (torch's planar RGB).  The row stride is the pitch
+        (and for PIX_RGBP the plane stride the plane distance), so a slice of a wider allocation is read in place (an I420 / YV12
+        array of that shape is copied unless tight: its chroma rows are not pitch/2 apart).  chroma_offset (the 4:2:0 formats):
+        the frames are the (h, w) luma planes, the row stride is the pitch, and the chroma plane starts chroma_offset bytes after
+        each frame's start, e.g. pitch * 1088 in a 1080p NVDEC surface; the caller vouches that the allocation reaches that far.
+        matrix ("bt601" or "bt709") and full_range describe YUV frames (e.g. "bt709" for HD video, full_range for FFmpeg's
+        yuvj420p); the default is BT.601 studio range.  Converted to BGR on the GPU as cv2.cvtColor does, then as
+        forward_camera_frames.  CUDA frames are read on the engine's stream after the work queued so far on torch's current
+        stream.  Returns frame.scale."""
+        flags = _colour_flags(matrix, full_range)
+        views = [_pixel_view(f, fmt, chroma_offset, flags) for f in frames]
+        pf = _batch_format(views)
         for dev in {v[3] for v in views if v[3] is not None and v[3].index == self.cfg.device}:
             import torch
             self._ck(lib().pe_stream_wait(self._h, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
@@ -973,46 +980,81 @@ class VideoCapture:
             pass
 
 
-def _pixel_view(frame, fmt, chroma_offset=None):
-    """(data pointer, _PixelFormat, the object that owns the pixels, torch device of a CUDA tensor or None) of a uint8 frame in
+def _colour_flags(matrix, full_range):
+    if matrix not in ("bt601", "bt709"):
+        raise ValueError("matrix %r is not 'bt601' or 'bt709'" % (matrix,))
+    return (PIX_FLAG_BT709 if matrix == "bt709" else 0) | (PIX_FLAG_FULL_RANGE if full_range else 0)
+
+
+def _pixel_view(frame, fmt, chroma_offset=None, flags=0):
+    """(data pointer, _PixelFormat, the object that owns the pixels, torch device of a CUDA tensor or None) of a frame in
     forward_pixels's shapes.  Frames whose pixels or channels are not adjacent in memory are copied first."""
-    if fmt not in (PIX_BGR, PIX_RGB, PIX_YUYV, PIX_NV12, PIX_I420):
-        raise ValueError("pixel format %r is not one of PIX_BGR .. PIX_I420" % (fmt,))
-    planar = fmt in (PIX_NV12, PIX_I420)
-    ch = 1 if planar else (2 if fmt == PIX_YUYV else 3)
+    if fmt not in _PIX_FORMATS:
+        raise ValueError("pixel format %r is not one of PIX_BGR .. PIX_I420, PIX_NV21 .. PIX_RGBP" % (fmt,))
+    planar, rgbp = fmt in _PIX_420, fmt == PIX_RGBP
+    if rgbp and chroma_offset is not None:
+        raise ValueError("chroma_offset is for the 4:2:0 formats; a (3, h, w) RGBP frame's plane stride is its stride(0)")
+    ch = 1 if planar or rgbp else (2 if fmt in (PIX_YUYV, PIX_UYVY) else 3)
     is_np = isinstance(frame, np.ndarray)
     if not is_np:
         import torch
         if not torch.is_tensor(frame):
             raise TypeError("frames are numpy arrays or torch tensors")
-    if (frame.dtype != np.uint8) if is_np else (frame.dtype != torch.uint8):
-        raise TypeError("frames are uint8, not %s" % frame.dtype)
+    dtype = "uint16" if fmt == PIX_P016 else "uint8"
+    if (frame.dtype != np.dtype(dtype)) if is_np else (frame.dtype != getattr(torch, dtype)):
+        raise TypeError("%s frames are %s, not %s" % ("P016" if fmt == PIX_P016 else "these", dtype, frame.dtype))
+    es = 2 if fmt == PIX_P016 else 1   # bytes per sample
     shape = tuple(frame.shape)
-    if shape[2:] != (() if planar else (ch,)) or len(shape) < 2:
+    if (len(shape) != 3 or shape[0] != 3) if rgbp else (shape[2:] != (() if planar else (ch,)) or len(shape) < 2):
         raise ValueError("frame shape %s does not fit format %d" % (shape, fmt))
 
-    def strides(f):
-        return tuple(f.strides) if is_np else tuple(f.stride())
+    def strides(f):   # in bytes
+        return tuple(f.strides) if is_np else tuple(s * es for s in f.stride())
+    if rgbp:
+        _, h, w = shape
+        st = strides(frame)
+        # rows of each plane, then planes at least a plane apart (the planes of a permuted HWC tensor interleave: copied)
+        if (w > 1 and st[2] != 1) or (h > 1 and st[1] < w) or st[0] < (st[1] if h > 1 else w) * h:
+            frame = np.ascontiguousarray(frame) if is_np else frame.contiguous()
+            st = strides(frame)
+        pitch = st[1] if h > 1 else w
+        return _frame_view(frame, is_np, _PixelFormat(fmt | flags, w, h, pitch, st[0]))
     h, w = shape[0], shape[1]
     st = strides(frame)
     # In cv2's (h*3/2, w) I420 array one row holds two chroma rows, so only a tight one has the layout's pitch/2 chroma rows
-    tight_i420 = fmt == PIX_I420 and chroma_offset is None
-    if (w > 1 and st[1] != ch) or (not planar and st[2] != 1) or (h > 1 and st[0] < w * ch) or (tight_i420 and h > 1 and st[0] != w):
+    tight_i420 = fmt in (PIX_I420, PIX_YV12) and chroma_offset is None
+    if ((w > 1 and st[1] != ch * es) or (not planar and st[2] != 1) or (h > 1 and st[0] < w * ch * es)
+            or (tight_i420 and h > 1 and st[0] != w)):
         frame = np.ascontiguousarray(frame) if is_np else frame.contiguous()
         st = strides(frame)
     if planar and chroma_offset is None:
         if h % 3:
-            raise ValueError("a %s frame has h*3/2 rows, not %d" % ("NV12" if fmt == PIX_NV12 else "I420", h))
+            raise ValueError("a 4:2:0 frame has h*3/2 rows, not %d" % h)
         h = h * 2 // 3
-    pitch = st[0] if shape[0] > 1 else w * ch
+    pitch = st[0] if shape[0] > 1 else w * ch * es
+    return _frame_view(frame, is_np, _PixelFormat(fmt | flags, w, h, pitch, chroma_offset or 0))
+
+
+def _batch_format(views):
+    """the _PixelFormat of every frame of one pe_forward_pixels call, which reads all of them with one layout: ValueError unless
+    the views agree on it (PIX_RGBP takes its plane stride from each frame's stride(0), so that must match as well)"""
+    key = lambda pf: (pf.format, pf.width, pf.height, pf.pitch, pf.chroma_offset)
+    pf = views[0][1]
+    if any(key(v[1]) != key(pf) for v in views):
+        raise ValueError("forward_pixels: the frames of one call share their size, row stride and plane stride")
+    return pf
+
+
+def _frame_view(frame, is_np, pf):
     ptr = frame.ctypes.data if is_np else frame.data_ptr()
     dev = None if is_np or not frame.is_cuda else frame.device
-    return ptr, _PixelFormat(fmt, w, h, pitch, chroma_offset or 0), frame, dev
+    return ptr, pf, frame, dev
 
 
-def pixels_to_bgr(frame, fmt):
-    """cv2.cvtColor of a host frame in forward_pixels's shapes to uint8 BGR (h, w, 3): the host reference of the GPU conversion."""
-    ptr, pf, frame, dev = _pixel_view(frame, fmt)
+def pixels_to_bgr(frame, fmt, matrix="bt601", full_range=False):
+    """cv2.cvtColor of a host frame in forward_pixels's shapes to uint8 BGR (h, w, 3): the host reference of the GPU conversion.
+    matrix and full_range: as forward_pixels."""
+    ptr, pf, frame, dev = _pixel_view(frame, fmt, None, _colour_flags(matrix, full_range))
     if dev is not None:
         raise ValueError("pixels_to_bgr takes host frames")
     out = np.empty((pf.height, pf.width, 3), np.uint8)

@@ -254,19 +254,39 @@ int pe_jpeg_decode_scans(pe_engine* e, const void* const* scans, int n, int subs
 int pe_forward_frames_device(pe_engine* e, const void* d_frames, int n);
 
 /* ---- frames as video decoders hand them out (NVDEC, FFmpeg / PyAV, V4L2, PIL / torchvision), converted to BGR on the GPU with
- * the arithmetic of cv::cvtColor (ITU-R BT.601 studio range, OpenCV's 20-bit fixed point; 4:2:0 chroma nearest-neighbour). */
+ * the arithmetic of cv::cvtColor (OpenCV's 20-bit fixed point).  YUV is ITU-R BT.601 studio range unless flags say otherwise.
+ * 4:2:0 and 4:2:2 chroma is nearest-neighbour, as in OpenCV: a quad or pair of pixels shares one chroma sample.  FFmpeg's swscale
+ * interpolates chroma, so its RGB output differs from these conversions near colour edges. */
 #define PE_PIX_BGR  0   /* packed uint8 B,G,R (what pe_forward_camera_frames takes)                       */
 #define PE_PIX_RGB  1   /* packed uint8 R,G,B            = cv::cvtColor(COLOR_RGB2BGR)                     */
 #define PE_PIX_YUYV 2   /* packed 4:2:2 Y0 U Y1 V        = COLOR_YUV2BGR_YUYV; even width                 */
 #define PE_PIX_NV12 3   /* Y plane, then interleaved U,V at half size = COLOR_YUV2BGR_NV12; even w, h     */
 #define PE_PIX_I420 4   /* Y, then U, then V planes at half size     = COLOR_YUV2BGR_I420; even w, h      */
+/* 5 .. 15 are not formats */
+#define PE_PIX_NV21 16  /* Y plane, then interleaved V,U at half size = COLOR_YUV2BGR_NV21; even w, h     */
+#define PE_PIX_YV12 17  /* Y, then V, then U planes at half size     = COLOR_YUV2BGR_YV12; even w, h      */
+#define PE_PIX_UYVY 18  /* packed 4:2:2 U Y0 V Y1        = COLOR_YUV2BGR_UYVY; even width                 */
+#define PE_PIX_P016 19  /* NV12's layout with little-endian 16-bit samples, significant bits at the top, so P010 and P012
+                           (NVDEC's 10- and 12-bit output) are this format; even w, h; pitch, chroma_offset and the frame
+                           pointer even.  Rounded to 8-bit BGR. */
+#define PE_PIX_RGBP 20  /* planar uint8 R, G, B: three planes of `height` rows `pitch` apart, plane k at k * chroma_offset
+                           (a torch (3, h, w) tensor: chroma_offset = stride(0), pitch = stride(1)) */
+/* Colour flags, OR'ed into format, valid on the YUV formats (PE_PIX_YUYV, _NV12, _I420, _NV21, _YV12, _UYVY, _P016) and
+ * PE_ERR_INVALID on BGR, RGB and RGBP, as is any other bit above 0xff.  No flag: BT.601 studio range, as above.
+ *   BT.601 full range = cv::cvtColor(COLOR_YCrCb2BGR) per pixel (FFmpeg's yuvj420p, JPEG);
+ *   BT.709 (HD video), studio or full range: the same fixed point with constants rounded from Kr = 0.2126, Kb = 0.0722,
+ *   within 1 of the exact conversion.  Studio-range luma below 16 counts as black, as in OpenCV's BT.601 formula. */
+#define PE_PIX_FLAG_BT709      0x100
+#define PE_PIX_FLAG_FULL_RANGE 0x200
 typedef struct pe_pixel_format {
-    int format;              /* PE_PIX_* */
+    int format;              /* PE_PIX_*, with PE_PIX_FLAG_* OR'ed in */
     int width, height;       /* frame size in pixels, 1 .. 16384 */
-    long long pitch;         /* bytes between rows of the first plane; 0 = tight (3w, 2w or w); I420: even */
-    long long chroma_offset; /* NV12 / I420: bytes from the frame start to the first chroma plane; 0 = pitch * height (an NVDEC
-                                surface: pitch * the aligned height).  NV12 chroma rows are `pitch` apart; I420 chroma rows are
-                                pitch/2 apart, and V follows U at chroma_offset + (pitch/2) * (height/2).  Ignored otherwise. */
+    long long pitch;         /* bytes between rows of the first plane; 0 = tight (3w, 2w or w; P016 2w); I420, YV12, P016: even */
+    long long chroma_offset; /* NV12 / NV21 / P016 / I420 / YV12: bytes from the frame start to the first chroma plane; 0 = pitch *
+                                height (an NVDEC surface: pitch * the aligned height).  NV12, NV21 and P016 chroma rows are
+                                `pitch` apart; I420 and YV12 chroma rows are pitch/2 apart, and the second chroma plane follows
+                                the first at chroma_offset + (pitch/2) * (height/2).  RGBP: bytes between the planes, at least
+                                pitch * height; 0 = pitch * height.  P016: even.  Ignored otherwise. */
 } pe_pixel_format;
 /* n <= max_batch frames of one format and size, one pointer per frame.  Each pointer is classified as pe_forward_frames does:
  * device memory on the engine's device (or managed memory) is read in place, asynchronously on the engine's stream; page-locked
@@ -275,7 +295,8 @@ typedef struct pe_pixel_format {
  * writes them on another stream is ordered before the forward with pe_stream_wait.  A frame of the display size is converted into
  * the display frame (*scale = 1); any other size is converted at its own size and then warped as pe_forward_camera_frames warps
  * (*scale = frame.scale).  pe_render with display_bgr == NULL draws on the converted display frame.  A format pe_pixels_to_bgr
- * rejects is PE_ERR_INVALID, with the reason in pe_last_error, before anything is queued. */
+ * rejects, or a P016 frame pointer that is not 2-byte aligned, is PE_ERR_INVALID, with the reason in pe_last_error, before
+ * anything is queued. */
 int pe_forward_pixels(pe_engine* e, const pe_pixel_format* fmt, const void* const* frames, int n, double* scale);
 /* later work on e waits for the work queued on cuda_stream (a cudaStream_t of the engine's device; NULL = the legacy default
  * stream) so far: cudaEventRecord there, cudaStreamWaitEvent on the engine's stream.  Nothing blocks the host. */
