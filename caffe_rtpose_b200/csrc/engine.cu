@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "common.h"
+#include "buffers.h"
 #include "kernels.h"
 #include "conv_tc.h"
 #include "precision.h"
@@ -46,18 +47,19 @@ struct pe_engine {
     Geo geo[4];
     const Precision* prec = nullptr;   // the precision mode's row (precision.h)
     bool u8 = false;                   // PE_PREC_FLAG_U8 (cfg.precision holds the mode without it): the plan's u8 activations
-    std::vector<void*> acts;        // device
+    // What a captured forward graph references (activations, maps, post and result buffers, packed weights, d_range, axis tables) is
+    // allocated once, in pe_create or commit, and never regrown: a replayed graph keeps its pointers.  Only input-route buffers grow.
+    std::vector<DeviceBuffer> acts;
     std::vector<long long> act_plane;  // elements per plane
     std::vector<HostWeights> hw;    // per conv
     bool committed = false;
-    // packed weights (one device buffer): per conv offsets (bytes)
-    void* d_packed = nullptr; size_t packed_bytes = 0;
-    std::shared_ptr<void> packed_owner;   // frees d_packed when the last handle using it goes (pe_share_weights)
+    // packed weights at per-conv offsets (bytes); shared by the handles of pe_share_weights, freed when the last one goes
+    std::shared_ptr<DeviceBuffer> packed;
     // range management of the fp16 and e4m3 modes (F16X2, F16X1, E4M3X1): per-conv-output power-of-two scale s (stored value = true value * s), the
     // weight-scale inverses the packed epilogue fields derive from (with the true biases hw[i].b), and the kernels' running max |stored value| per conv
     std::vector<float> conv_scale, wsi;   // per conv: scale of its stored output; inverse of the power of two folded into its weights
     std::vector<std::vector<float>> wsig;   // S8X1: per conv, the per-output-channel weight step sigma_c of pack_conv_weights (s8.h)
-    unsigned* d_range = nullptr;
+    DeviceBuffer d_range;
     bool calibrated = false, check_range = false;
     // pe_calibrate_begin .. _end: per conv, the largest true |output| (recorded / conv_scale) over the forwards since begin
     bool collecting = false;
@@ -80,35 +82,31 @@ struct pe_engine {
     std::vector<cudaEvent_t> conv_done;          // per conv: recorded after its launch when another lane waits for it
     int last_lane1_conv = -1;
     cudaEvent_t ev[16] = {};
-    uint8_t* d_frames = nullptr; uint8_t* d_resized = nullptr;
-    uint8_t* h_frames = nullptr; size_t h_frames_cap = 0;   // pinned staging for pageable frames (upload_host)
-    float* d_planar = nullptr; float* h_planar = nullptr;
-    std::vector<void*> d_tabs;
-    PreArgs pre;
-    float* d_maps = nullptr; float* h_maps = nullptr;
-    PostDev post;
-    float* h_joints = nullptr; int* h_num_people = nullptr; float* h_peaks = nullptr;
+    DeviceBuffer d_frames, d_resized, d_planar, d_maps;
+    std::vector<DeviceBuffer> d_tabs;
+    PreArgs pre{};
+    DeviceBuffer d_post;   // the post-processing arrays of post and the axis tables d_xtab, d_ytab
+    PostDev post{};
     AxisTap *d_xtab = nullptr, *d_ytab = nullptr;
+    PinnedBuffer h_results;   // h_joints, h_num_people, h_peaks
+    float* h_joints = nullptr; int* h_num_people = nullptr; float* h_peaks = nullptr;
+    PinnedBuffer h_stage;   // staging of host input and of pe_fetch_maps: a forward uses it at most once, the host writes it after a drain
     float start_scale_f, scale_gap_f;
     int last_n = 0;
-    // raw camera frames (any size) -> display image: warpAffine tables for the last (orig_w, orig_h)
-    uint8_t* d_raw = nullptr; size_t raw_cap = 0; uint8_t* h_raw = nullptr; size_t h_raw_cap = 0;
+    // raw camera frames (any size) -> display image: warpAffine source, and tables (d_warp) for the last (orig_w, orig_h)
+    DeviceBuffer d_raw, d_warp;
     int warp_w = 0, warp_h = 0; double warp_scale = 1.0;
     int *d_wa = nullptr, *d_wb = nullptr, *d_wx0 = nullptr, *d_wy0 = nullptr; short* d_wtab = nullptr;
     // decoder-format host frames (pe_forward_pixels) copied to the device before conversion; pe_stream_wait's event
-    uint8_t* d_pix = nullptr; size_t pix_cap = 0;
+    DeviceBuffer d_pix;
     cudaEvent_t ev_wait = nullptr;
     bool input_lo_dirty = false;   // the planar-input path wrote non-zero lo planes / channels >= 32 of the input buffer
-    // JPEG coefficient images (pe_forward_jpeg_coefs): device copies, pinned staging for pageable callers, component planes
-    uint8_t* d_jcoef = nullptr; size_t jcoef_cap = 0; uint8_t* h_jcoef = nullptr; size_t h_jcoef_cap = 0;
-    uint8_t* d_jplanes = nullptr; size_t jplanes_cap = 0;
-    // JPEG scan images (pe_forward_jpeg_scans): device copies, pinned staging, the decoder's work space, per-frame status
-    uint8_t* d_jscan = nullptr; size_t jscan_cap = 0; uint8_t* h_jscan = nullptr; size_t h_jscan_cap = 0;
-    uint8_t* d_jwork = nullptr; size_t jwork_cap = 0;
-    uint8_t* h_jstatus = nullptr; size_t h_jstatus_cap = 0;
+    DeviceBuffer d_jcoef, d_jplanes;   // JPEG coefficient images (pe_forward_jpeg_coefs): device copies, component planes
+    DeviceBuffer d_jscan, d_jwork;     // JPEG scan images (pe_forward_jpeg_scans): device copies, the decoder's work space
+    PinnedBuffer h_jstatus;            // and its per-frame status
     int jstatus_n = 0;   // frames of the last forward whose status h_jstatus holds (0: the last forward was not from scan images)
-    // renderers: canvas, uint8 image, heat-map scratch (allocated on first pe_render); display frames of the last forward
-    float* d_canvas = nullptr; uint8_t* d_render_u8 = nullptr; uint8_t* d_render_src = nullptr; float* d_heat = nullptr; size_t heat_cap = 0;
+    // renderers: canvas, uint8 image and display frame (d_render, on first pe_render), heat-map scratch; display frames of the last forward
+    DeviceBuffer d_render, d_heat;
     const uint8_t* last_frames = nullptr;
     // CUDA graphs of the steady-state forward (92 conv + pool/copy + 5 parse kernels + result copies), one per batch
     // size; the first forward of a size runs eagerly, the second is captured, later ones replay.  Invalidated by
@@ -186,11 +184,10 @@ static void area_table(int ssize, int dsize, double scale, std::vector<int>& ofs
 
 template <typename T>
 static int upload(pe_engine* e, const std::vector<T>& v, const T** out) {
-    void* d = nullptr;
-    CK(e, cudaMalloc(&d, std::max<size_t>(v.size(), 1) * sizeof(T)));
-    CK(e, cudaMemcpy(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
-    e->d_tabs.push_back(d);
-    *out = (const T*)d;
+    DeviceBuffer& d = e->d_tabs.emplace_back();
+    CK(e, d.reserve(std::max<size_t>(v.size(), 1) * sizeof(T)));
+    CK(e, cudaMemcpy(d.get(), v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
+    *out = d.get<const T>();
     return PE_OK;
 }
 
@@ -462,8 +459,6 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, const
     if (cfg->device < 0 || cfg->device >= ndev) return fail(nullptr, PE_ERR_INVALID, "device %d out of range (%d visible)", cfg->device, ndev);
 
     pe_engine* e = new pe_engine();
-    memset(&e->post, 0, sizeof e->post);   // PODs: every pointer must be null for pe_destroy on an early failure
-    memset(&e->pre, 0, sizeof e->pre);
     e->cfg = *cfg;
     e->mt_own = model_tables(cfg->model);
     if (prototxt_path) e->mt_own.max_peaks = plan.nms_max_peaks;   // nms_param.max_peaks (NmsLayer::GetMaxPeaks, rtpose.cpp:195)
@@ -515,30 +510,26 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, const
         e->flops_per_scale += c.flops_per_image;
     }
     // activations
-    e->acts.assign(e->plan.acts.size(), nullptr);
+    e->acts.resize(e->plan.acts.size());
     e->act_plane.assign(e->plan.acts.size(), 0);
     for (size_t i = 0; i < e->plan.acts.size(); i++) {
         const ActSpec& a = e->plan.acts[i];
         const Geo& g = e->geo[a.level];
         e->act_plane[i] = g.M * a.C;
         const size_t bytes = (size_t)e->act_plane[i] * fmt_bytes(act_fmt(e, (int)i));
-        CKC(cudaMalloc(&e->acts[i], bytes));
-        CKC(cudaMemsetAsync(e->acts[i], 0, bytes, e->stream));
+        CKC(e->acts[i].reserve(bytes));
+        CKC(cudaMemsetAsync(e->acts[i].get(), 0, bytes, e->stream));
     }
     // io buffers
-    const size_t frame_bytes = (size_t)cfg->disp_w * cfg->disp_h * 3;
-    CKC(cudaMalloc(&e->d_frames, frame_bytes * cfg->max_batch));
-    CKC(cudaMalloc(&e->d_resized, (size_t)N * cfg->net_w * cfg->net_h * 3));
-    const size_t planar_n = (size_t)N * 3 * cfg->net_w * cfg->net_h;
-    CKC(cudaMalloc(&e->d_planar, planar_n * sizeof(float)));
-    CKC(cudaMallocHost(&e->h_planar, planar_n * sizeof(float)));
-    const size_t maps_n = (size_t)N * e->mt->num_maps * e->geo[3].W * e->geo[3].H;
-    CKC(cudaMalloc(&e->d_maps, maps_n * sizeof(float)));
-    CKC(cudaMemsetAsync(e->d_maps, 0, maps_n * sizeof(float), e->stream));
-    CKC(cudaMallocHost(&e->h_maps, maps_n * sizeof(float)));
+    CKC(e->d_frames.reserve((size_t)cfg->disp_w * cfg->disp_h * 3 * cfg->max_batch));
+    CKC(e->d_resized.reserve((size_t)N * cfg->net_w * cfg->net_h * 3));
+    CKC(e->d_planar.reserve((size_t)N * 3 * cfg->net_w * cfg->net_h * sizeof(float)));
+    const size_t maps_bytes = (size_t)N * e->mt->num_maps * e->geo[3].W * e->geo[3].H * sizeof(float);
+    CKC(e->d_maps.reserve(maps_bytes));
+    CKC(cudaMemsetAsync(e->d_maps.get(), 0, maps_bytes, e->stream));
     if (build_pre_tables(e)) return bail(PE_ERR_INVALID);
-    e->pre.frames = e->d_frames; e->pre.resized = e->d_resized;
-    e->pre.out = e->acts[e->plan.input_act]; e->pre.kp = e->plan.kp_input;
+    e->pre.frames = e->d_frames.get(); e->pre.resized = e->d_resized.get();
+    e->pre.out = e->acts[e->plan.input_act].get(); e->pre.kp = e->plan.kp_input;
     e->pre.out_plane = e->act_plane[e->plan.input_act]; e->pre.fmt = act_fmt(e, e->plan.input_act);
     e->pre.Wp = e->geo[0].Wp; e->pre.Hs = e->geo[0].Hs;
 
@@ -554,30 +545,23 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, const
         else { p.nms_threshold = 0.05f; p.inter_threshold = 0.050f; p.inter_min_above = 9; }
     }
     for (int i = 0; i < 2 * e->mt->num_limbs; i++) { pd.md.limb_seq[i] = e->mt->limb_seq[i]; pd.md.map_idx[i] = e->mt->map_idx[i]; }
-    const int B = cfg->max_batch, P = e->mt->num_parts, MP = e->mt->max_peaks, NL = e->mt->num_limbs;
-    pd.maps = e->d_maps;
-    CKC(cudaMalloc(&e->d_xtab, sizeof(AxisTap) * cfg->num_scales * cfg->net_w));
-    CKC(cudaMalloc(&e->d_ytab, sizeof(AxisTap) * cfg->num_scales * cfg->net_h));
-    pd.xtab = e->d_xtab; pd.ytab = e->d_ytab;
-    const int wpr = (cfg->net_w + 31) / 32;
-    CKC(cudaMalloc(&pd.flags, sizeof(unsigned) * (size_t)B * P * cfg->net_h * wpr));
-    CKC(cudaMalloc(&pd.peaks, sizeof(float) * (size_t)B * P * (MP + 1) * 3));
-    CKC(cudaMalloc(&pd.cands, sizeof(Cand) * (size_t)B * NL * MP * MP));
-    CKC(cudaMalloc(&pd.cand_count, sizeof(int) * (size_t)B * NL));
+    const size_t B = cfg->max_batch, P = e->mt->num_parts, MP = e->mt->max_peaks, NL = e->mt->num_limbs;
+    pd.maps = e->d_maps.get<float>();
     pd.sort_stride = 1;
-    while (pd.sort_stride < MP * MP) pd.sort_stride <<= 1;
+    while (pd.sort_stride < (int)(MP * MP)) pd.sort_stride <<= 1;
     CKC(post_set_smem_limits());
-    CKC(cudaMalloc(&pd.conns, sizeof(Conn) * (size_t)B * NL * MP));
-    CKC(cudaMalloc(&pd.conn_count, sizeof(int) * (size_t)B * NL));
-    CKC(cudaMemset(pd.conn_count, 0, sizeof(int) * (size_t)B * NL));
-    pd.p.max_subset_rows = NL * MP;
-    CKC(cudaMalloc(&pd.subset, sizeof(double) * (size_t)B * pd.p.max_subset_rows * (P + 3)));
-    CKC(cudaMalloc(&pd.subset_rows, sizeof(int) * B));
-    CKC(cudaMalloc(&pd.joints, sizeof(float) * (size_t)B * PE_MAX_PEOPLE * P * 3));
-    CKC(cudaMalloc(&pd.num_people, sizeof(int) * B));
-    CKC(cudaMallocHost(&e->h_joints, sizeof(float) * (size_t)B * PE_MAX_PEOPLE * P * 3));
-    CKC(cudaMallocHost(&e->h_num_people, sizeof(int) * B));
-    CKC(cudaMallocHost(&e->h_peaks, sizeof(float) * (size_t)B * P * (MP + 1) * 3));
+    pd.p.max_subset_rows = (int)(NL * MP);
+    CKC(reserve_carved(e->d_post, [&](Carver& d) {   // the post-processing arrays and the axis tables
+        pd.xtab = e->d_xtab = d.take<AxisTap>((size_t)cfg->num_scales * cfg->net_w); pd.ytab = e->d_ytab = d.take<AxisTap>((size_t)cfg->num_scales * cfg->net_h);
+        pd.flags = d.take<unsigned>(B * P * cfg->net_h * ((cfg->net_w + 31) / 32)); pd.peaks = d.take<float>(B * P * (MP + 1) * 3);
+        pd.cands = d.take<Cand>(B * NL * MP * MP); pd.cand_count = d.take<int>(B * NL);
+        pd.conns = d.take<Conn>(B * NL * MP); pd.conn_count = d.take<int>(B * NL);
+        pd.subset = d.take<double>(B * pd.p.max_subset_rows * (P + 3)); pd.subset_rows = d.take<int>(B);
+        pd.joints = d.take<float>(B * PE_MAX_PEOPLE * P * 3); pd.num_people = d.take<int>(B);
+    }));
+    CKC(reserve_carved(e->h_results, [&](Carver& r) { e->h_joints = r.take<float>(B * PE_MAX_PEOPLE * P * 3); e->h_num_people = r.take<int>(B);
+                                                       e->h_peaks = r.take<float>(B * P * (MP + 1) * 3); }));
+    CKC(cudaMemset(pd.conn_count, 0, sizeof(int) * B * NL));
     launch_axis_tables(e->d_xtab, e->d_ytab, pd.p, e->stream);
     e->launches += 2;
     CKC(cudaStreamSynchronize(e->stream));
@@ -590,26 +574,13 @@ extern "C" void pe_destroy(pe_engine* e) {
     cudaSetDevice(e->cfg.device);
     if (e->stream) cudaStreamSynchronize(e->stream);
     drop_graphs(e);
-    for (void* p : e->acts) if (p) cudaFree(p);
-    for (void* p : e->d_tabs) cudaFree(p);
     for (auto& t : e->tc) tc_layer_destroy(t);
-    cudaFree(e->d_jcoef); cudaFreeHost(e->h_jcoef); cudaFree(e->d_jplanes);
-    cudaFree(e->d_jscan); cudaFreeHost(e->h_jscan); cudaFree(e->d_jwork); cudaFreeHost(e->h_jstatus);
-    cudaFree(e->d_pix); if (e->ev_wait) cudaEventDestroy(e->ev_wait);
-    cudaFree(e->d_raw); cudaFreeHost(e->h_raw); cudaFree(e->d_wa); cudaFree(e->d_wb); cudaFree(e->d_wx0); cudaFree(e->d_wy0); cudaFree(e->d_wtab);
-    e->packed_owner.reset(); cudaFree(e->d_range); cudaFree(e->d_frames); cudaFree(e->d_resized); cudaFree(e->d_planar); cudaFree(e->d_maps);
-    cudaFreeHost(e->h_frames); cudaFreeHost(e->h_planar); cudaFreeHost(e->h_maps);
-    cudaFree(e->d_xtab); cudaFree(e->d_ytab);
-    cudaFree(e->d_canvas); cudaFree(e->d_render_u8); cudaFree(e->d_render_src); cudaFree(e->d_heat);
-    PostDev& pd = e->post;
-    cudaFree(pd.flags); cudaFree(pd.peaks); cudaFree(pd.cands); cudaFree(pd.cand_count); cudaFree(pd.conns);
-    cudaFree(pd.conn_count); cudaFree(pd.subset); cudaFree(pd.subset_rows); cudaFree(pd.joints); cudaFree(pd.num_people);
-    cudaFreeHost(e->h_joints); cudaFreeHost(e->h_num_people); cudaFreeHost(e->h_peaks);
+    if (e->ev_wait) cudaEventDestroy(e->ev_wait);
     for (cudaEvent_t ev : e->conv_done) if (ev) cudaEventDestroy(ev);
     if (e->stream2) { cudaStreamSynchronize(e->stream2); cudaStreamDestroy(e->stream2); }
     for (int i = 0; i < 16; i++) if (e->ev[i]) cudaEventDestroy(e->ev[i]);
     if (e->stream) cudaStreamDestroy(e->stream);
-    delete e;
+    delete e;   // the buffers free themselves, on the device set above (packed weights: on their own device)
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -821,10 +792,7 @@ static int pack_conv_weights(pe_engine* e, int i, uint8_t* dst) {
 // per-layer launch state (TMA descriptors) over the packed buffer the handle currently points at
 static int bind_packed(pe_engine* e) {
     const size_t nc = e->plan.convs.size();
-    if (e->prec->ranged() && !e->d_range) {
-        CK(e, cudaMalloc(&e->d_range, nc * sizeof(unsigned)));
-        CK(e, cudaMemset(e->d_range, 0, nc * sizeof(unsigned)));
-    }
+    if (e->prec->ranged() && !e->d_range.size()) { CK(e, e->d_range.reserve(nc * sizeof(unsigned))); CK(e, cudaMemset(e->d_range.get(), 0, nc * sizeof(unsigned))); }
     if (e->prec->fmt.planes) {
         for (auto& t : e->tc) tc_layer_destroy(t);
         e->tc.assign(nc, TcLayer());
@@ -832,18 +800,18 @@ static int bind_packed(pe_engine* e) {
             const ConvSpec& c = e->plan.convs[i];
             const Geo& g = e->geo[c.level];
             TcLayerDesc d;
-            d.in = e->acts[c.in_act]; d.in_pitch = e->plan.acts[c.in_act].C; d.in_cused = c.in_cused; d.in_plane = e->act_plane[c.in_act];
-            d.w = (char*)e->d_packed + e->w_off[i]; d.bias = (const float*)((char*)e->d_packed + e->b_off[i]);
+            d.in = e->acts[c.in_act].get(); d.in_pitch = e->plan.acts[c.in_act].C; d.in_cused = c.in_cused; d.in_plane = e->act_plane[c.in_act];
+            d.w = e->packed->get() + e->w_off[i]; d.bias = (const float*)(e->packed->get() + e->b_off[i]);
             d.cout = c.cout; d.cout_pad = e->cout_pad[i]; d.ksize = c.im2col_input ? 1 : c.k; d.pad = c.im2col_input ? 0 : c.pad;
             d.relu = c.relu; d.fmt = conv_wfmt(e, (int)i); d.geo = g; d.out_scale = d.bias + e->cout_pad[i];
             d.out_elem = conv_out_elem(e, (int)i); d.chunked = conv_row(e, (int)i).chunked; d.sparse = e->sparse[i];
-            d.range = (e->prec->ranged() && e->d_range) ? e->d_range + i : nullptr;
+            d.range = e->prec->ranged() ? e->d_range.get<unsigned>() + i : nullptr;
             if (c.out_act >= 0) {
-                d.out = e->acts[c.out_act]; d.out_pitch = e->plan.acts[c.out_act].C; d.out_coff = c.out_coff; d.out_plane = e->act_plane[c.out_act];
+                d.out = e->acts[c.out_act].get(); d.out_pitch = e->plan.acts[c.out_act].C; d.out_coff = c.out_coff; d.out_plane = e->act_plane[c.out_act];
                 d.planar = nullptr; d.planar_C = 0; d.planar_coff = 0;
             } else {
                 d.out = nullptr; d.out_pitch = 0; d.out_coff = 0; d.out_plane = 0;
-                d.planar = e->d_maps; d.planar_C = e->mt->num_maps; d.planar_coff = c.planar_coff;
+                d.planar = e->d_maps.get<float>(); d.planar_C = e->mt->num_maps; d.planar_coff = c.planar_coff;
             }
             std::string err;
             if (tc_layer_create(d, e->tc[i], err)) return fail(e, PE_ERR_CUDA, "layer %s: %s", c.name.c_str(), err.c_str());
@@ -892,6 +860,7 @@ static int commit(pe_engine* e, const std::vector<char>* sparse_from) {
             return fail(e, PE_ERR_STATE, "weights of layer %s were never set%s", c.name.c_str(),
                         e->committed ? " on this handle (a broadcast replica keeps no fp32 copy: set every layer again)" : "");
     }
+    e->committed = false;   // the layout changes under the bound buffer: no forward until this commit succeeds
     e->sparse.assign(nc, 0);
     for (size_t i = 0; i < nc; i++)
         e->sparse[i] = sparse_from ? (*sparse_from)[i] : sparse_eligible(e, (int)i) && conv_weights_2to4(e->plan.convs[i], e->hw[i].w.data());
@@ -902,21 +871,13 @@ static int commit(pe_engine* e, const std::vector<char>* sparse_from) {
     e->conv_scale.assign(nc, 1.f);
     std::vector<uint8_t> host(total, 0);
     for (size_t i = 0; i < nc; i++) {
-        if (pack_conv_weights(e, (int)i, host.data() + e->w_off[i])) {
-            e->committed = false;   // the layout changed under the bound buffer: no forward until a commit succeeds
-            return PE_ERR_STATE;
-        }
+        if (pack_conv_weights(e, (int)i, host.data() + e->w_off[i])) return PE_ERR_STATE;
         fill_epilogue_fields(e, (int)i, (float*)(host.data() + e->b_off[i]));   // travels with the packed buffer (weight broadcast)
     }
-    e->packed_owner.reset();
-    e->d_packed = nullptr;
-    void* dp = nullptr;
-    CK(e, cudaMalloc(&dp, total));
-    const int dev = e->cfg.device;
-    e->packed_owner = std::shared_ptr<void>(dp, [dev](void* q) { int cur = 0; cudaGetDevice(&cur); cudaSetDevice(dev); cudaFree(q); cudaSetDevice(cur); });
-    e->d_packed = dp;
-    CK(e, cudaMemcpy(e->d_packed, host.data(), total, cudaMemcpyHostToDevice));
-    e->packed_bytes = total;
+    e->packed.reset();   // the old buffer goes first (unless another handle still uses it)
+    e->packed = std::shared_ptr<DeviceBuffer>(new DeviceBuffer(), [dev = e->cfg.device](DeviceBuffer* b) { int cur = 0; cudaGetDevice(&cur); cudaSetDevice(dev); delete b; cudaSetDevice(cur); });
+    CK(e, e->packed->reserve(total));
+    CK(e, cudaMemcpy(e->packed->get(), host.data(), total, cudaMemcpyHostToDevice));
     return bind_packed(e);
 }
 extern "C" int pe_commit_weights(pe_engine* e) { return commit(e, nullptr); }
@@ -943,13 +904,11 @@ extern "C" int pe_share_weights(pe_engine* from, pe_engine* to) {
     const std::vector<size_t> own_w = to->w_off, own_b = to->b_off;
     const std::vector<int> own_cout = to->cout_pad, own_cin = to->cin_pad;
     to->sparse = from->sparse;
-    if (packed_layout(to) != from->packed_bytes) {
+    if (packed_layout(to) != from->packed->size()) {
         to->sparse = own_sparse; to->w_off = own_w; to->b_off = own_b; to->cout_pad = own_cout; to->cin_pad = own_cin;
         return fail(from, PE_ERR_STATE, "packed layouts differ");
     }
-    to->packed_owner = from->packed_owner;
-    to->d_packed = from->d_packed;
-    to->packed_bytes = from->packed_bytes;
+    to->packed = from->packed;
     for (auto& h : to->hw) { std::vector<float>().swap(h.w); std::vector<float>().swap(h.b); h.set = false; }
     to->conv_scale = from->conv_scale; to->calibrated = from->calibrated;
     return bind_packed(to);
@@ -991,7 +950,7 @@ extern "C" int pe_broadcast_weights(pe_engine* const* engines, int n) {
             // ("weights of layer ... were never set") instead of packing from empty vectors
             for (auto& h : e->hw) { std::vector<float>().swap(h.w); std::vector<float>().swap(h.b); h.set = false; }
         }
-        if (e->packed_bytes != root->packed_bytes) return fail(root, PE_ERR_STATE, "packed layouts differ");
+        if (e->packed->size() != root->packed->size()) return fail(root, PE_ERR_STATE, "packed layouts differ");
     }
     void* h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_GLOBAL);
     if (!h) h = dlopen("libnccl.so", RTLD_NOW | RTLD_GLOBAL);
@@ -1015,7 +974,7 @@ extern "C" int pe_broadcast_weights(pe_engine* const* engines, int n) {
     gstart();
     for (int i = 0; i < n && !rc; i++) {
         cudaSetDevice(devs[i]);
-        rc = bcast(root->d_packed, engines[i]->d_packed, root->packed_bytes, 0 /*ncclChar*/, 0, comms[i], engines[i]->stream);
+        rc = bcast(root->packed->get(), engines[i]->packed->get(), root->packed->size(), 0 /*ncclChar*/, 0, comms[i], engines[i]->stream);
     }
     const int rc2 = gend();
     for (int i = 0; i < n; i++) { cudaSetDevice(devs[i]); cudaStreamSynchronize(engines[i]->stream); }
@@ -1027,7 +986,7 @@ extern "C" int pe_broadcast_weights(pe_engine* const* engines, int n) {
     return PE_OK;
 }
 
-extern "C" size_t pe_packed_weights_bytes(const pe_engine* e) { return e ? e->packed_bytes : 0; }
+extern "C" size_t pe_packed_weights_bytes(const pe_engine* e) { return e && e->packed ? e->packed->size() : 0; }
 
 extern "C" int pe_conv_layer_sparse(const pe_engine* e, int idx) {
     if (!e) return -PE_ERR_INVALID;
@@ -1035,7 +994,7 @@ extern "C" int pe_conv_layer_sparse(const pe_engine* e, int idx) {
     if (!e->committed) return -fail((pe_engine*)e, PE_ERR_STATE, "pe_conv_layer_sparse: pe_commit_weights has not been called");
     return e->sparse[idx] ? 1 : 0;
 }
-extern "C" void* pe_packed_weights_device_ptr(pe_engine* e) { return e ? e->d_packed : nullptr; }
+extern "C" void* pe_packed_weights_device_ptr(pe_engine* e) { return e && e->packed ? e->packed->get() : nullptr; }
 
 // ---------------------------------------------------------------------------------------------
 // layer accessors
@@ -1102,10 +1061,10 @@ static int run_op(pe_engine* e, const OpRef& op, int nimg, cudaStream_t st = nul
         }
         ConvArgs a;
         memset(&a, 0, sizeof a);
-        a.in = e->acts[c.in_act]; a.in_pitch = e->plan.acts[c.in_act].C;
-        a.w = (char*)e->d_packed + e->w_off[op.idx]; a.bias = (const float*)((char*)e->d_packed + e->b_off[op.idx]);
-        if (c.out_act >= 0) { a.out = e->acts[c.out_act]; a.out_pitch = e->plan.acts[c.out_act].C; a.out_coff = c.out_coff; }
-        else { a.planar = e->d_maps; a.planar_C = e->mt->num_maps; a.planar_coff = c.planar_coff; }
+        a.in = e->acts[c.in_act].get(); a.in_pitch = e->plan.acts[c.in_act].C;
+        a.w = e->packed->get() + e->w_off[op.idx]; a.bias = (const float*)(e->packed->get() + e->b_off[op.idx]);
+        if (c.out_act >= 0) { a.out = e->acts[c.out_act].get(); a.out_pitch = e->plan.acts[c.out_act].C; a.out_coff = c.out_coff; }
+        else { a.planar = e->d_maps.get<float>(); a.planar_C = e->mt->num_maps; a.planar_coff = c.planar_coff; }
         a.cin_pad = e->cin_pad[op.idx]; a.cout = c.cout; a.cout_pad = e->cout_pad[op.idx];
         a.ksize = c.im2col_input ? 1 : c.k; a.pad = c.im2col_input ? 0 : c.pad; a.relu = c.relu;
         a.W = g.W; a.H = g.H; a.Wp = g.Wp; a.Hs = g.Hs; a.N = nimg; a.M = M;
@@ -1114,7 +1073,7 @@ static int run_op(pe_engine* e, const OpRef& op, int nimg, cudaStream_t st = nul
         const PoolSpec& p = e->plan.pools[op.idx];
         const Geo& gi = e->geo[p.level_in]; const Geo& go = e->geo[p.level_in + 1];
         PoolArgs a;
-        a.in = e->acts[p.in_act]; a.out = e->acts[p.out_act]; a.C = e->plan.acts[p.in_act].C;
+        a.in = e->acts[p.in_act].get(); a.out = e->acts[p.out_act].get(); a.C = e->plan.acts[p.in_act].C;
         a.in_plane = e->act_plane[p.in_act]; a.out_plane = e->act_plane[p.out_act]; a.fmt = act_fmt(e, p.in_act);
         a.Wi = gi.W; a.Hi = gi.H; a.Wpi = gi.Wp; a.Hsi = gi.Hs; a.Wo = go.W; a.Ho = go.H; a.Wpo = go.Wp; a.Hso = go.Hs; a.N = nimg;
         e->launches += launch_pool(a, st);
@@ -1122,7 +1081,7 @@ static int run_op(pe_engine* e, const OpRef& op, int nimg, cudaStream_t st = nul
         const CopySpec& c = e->plan.copies[op.idx];
         const Geo& g = e->geo[3];
         CopyArgs a;
-        a.src = e->acts[c.src_act]; a.dst = e->acts[c.dst_act]; a.pitch = e->plan.acts[c.src_act].C; a.channels = c.channels;
+        a.src = e->acts[c.src_act].get(); a.dst = e->acts[c.dst_act].get(); a.pitch = e->plan.acts[c.src_act].C; a.channels = c.channels;
         a.fmt = act_fmt(e, c.src_act); a.elem_bytes = a.fmt.elem_bytes(); a.M = (long long)nimg * g.Hs * g.Wp; a.plane = e->act_plane[c.src_act];
         e->launches += launch_copy_channels(a, st);
     }
@@ -1130,7 +1089,7 @@ static int run_op(pe_engine* e, const OpRef& op, int nimg, cudaStream_t st = nul
 }
 
 static int run_post_and_return(pe_engine* e, int n) {
-    e->post.maps = e->d_maps;
+    e->post.maps = e->d_maps.get<float>();
     e->launches += launch_post(e->post, n, e->stream);
     const int P = e->mt->num_parts, MP = e->mt->max_peaks;
     CK(e, cudaMemcpyAsync(e->h_joints, e->post.joints, sizeof(float) * (size_t)n * PE_MAX_PEOPLE * P * 3, cudaMemcpyDeviceToHost, e->stream));
@@ -1252,21 +1211,20 @@ static int check_n(pe_engine* e, int n) {
     return PE_OK;
 }
 
-// (re)allocates *p to hold at least `need` bytes; the stream is drained first because queued work may still use the old buffer
-static int grow_buffer(pe_engine* e, uint8_t** p, size_t* cap, size_t need, bool host) {
-    if (*cap >= need) return PE_OK;
+// (re)allocates b to hold at least `need` bytes; the stream is drained first because queued work may still use the old buffer
+template <class B>
+static int grow_buffer(pe_engine* e, B& b, size_t need) {
+    if (b.size() >= need) return PE_OK;
     CK(e, cudaStreamSynchronize(e->stream));
-    if (host) { cudaFreeHost(*p); *p = nullptr; CK(e, cudaMallocHost((void**)p, need)); }
-    else { cudaFree(*p); *p = nullptr; CK(e, cudaMalloc((void**)p, need)); }
-    *cap = need;
+    CK(e, b.reserve(need));
     return PE_OK;
 }
+// The pinned staging buffer with at least `need` bytes.  The stream is drained first, grown or not: queued copies may still read it.
+static int stage(pe_engine* e, size_t need) { CK(e, cudaStreamSynchronize(e->stream)); return grow_buffer(e, e->h_stage, need); }
 
 // n host buffers (bytes[i] bytes from src[i]) to dst + i * stride.  Every pointer is checked before anything is copied.  When all are
-// page-locked (pe_host_alloc) they are DMA'd directly, fully asynchronously; otherwise they go through the pinned staging buffer
-// *staging in one copy of stride * n bytes, which drains the stream first because queued work may still read that buffer.
-static int upload_host(pe_engine* e, const void* const* src, const std::vector<size_t>& bytes, int n, size_t stride, uint8_t* dst,
-                       uint8_t** staging, size_t* staging_cap, const char* what) {
+// page-locked (pe_host_alloc) they are DMA'd directly, fully asynchronously; otherwise they go through staging in one copy.
+static int upload_host(pe_engine* e, const void* const* src, const std::vector<size_t>& bytes, int n, size_t stride, uint8_t* dst, const char* what) {
     bool pinned = true;
     for (int i = 0; i < n; i++) {
         if (!src[i]) return fail(e, PE_ERR_INVALID, "null %s %d", what, i);
@@ -1277,10 +1235,9 @@ static int upload_host(pe_engine* e, const void* const* src, const std::vector<s
         for (int i = 0; i < n; i++) CK(e, cudaMemcpyAsync(dst + i * stride, src[i], bytes[i], cudaMemcpyHostToDevice, e->stream));
         return PE_OK;
     }
-    CK(e, cudaStreamSynchronize(e->stream));
-    int rc = grow_buffer(e, staging, staging_cap, stride * n, true); if (rc) return rc;
-    for (int i = 0; i < n; i++) memcpy(*staging + i * stride, src[i], bytes[i]);
-    CK(e, cudaMemcpyAsync(dst, *staging, stride * n, cudaMemcpyHostToDevice, e->stream));
+    if (const int rc = stage(e, stride * n)) return rc;
+    for (int i = 0; i < n; i++) memcpy(e->h_stage.get() + i * stride, src[i], bytes[i]);
+    CK(e, cudaMemcpyAsync(dst, e->h_stage.get(), stride * n, cudaMemcpyHostToDevice, e->stream));
     return PE_OK;
 }
 
@@ -1290,7 +1247,7 @@ static int preprocess_frames(pe_engine* e, const uint8_t* d_frames, int n) {
     a.frames = d_frames; a.nframes = n;
     if (e->input_lo_dirty) {   // the uint8 path only writes the hi plane; drop what the planar path left behind
         const size_t bytes = (size_t)e->act_plane[e->plan.input_act] * fmt_bytes(act_fmt(e, e->plan.input_act));
-        CK(e, cudaMemsetAsync(e->acts[e->plan.input_act], 0, bytes, e->stream));
+        CK(e, cudaMemsetAsync(e->acts[e->plan.input_act].get(), 0, bytes, e->stream));
         e->input_lo_dirty = false;
     }
     e->launches += launch_preprocess(a, e->stream);
@@ -1308,14 +1265,14 @@ extern "C" int pe_forward_frames_device(pe_engine* e, const void* d_frames, int 
 static int upload_frames(pe_engine* e, const uint8_t* const* frames, int n) {
     if (!frames) return fail(e, PE_ERR_INVALID, "null frames");
     const size_t fb = (size_t)e->cfg.disp_w * e->cfg.disp_h * 3;
-    return upload_host(e, (const void* const*)frames, std::vector<size_t>(n, fb), n, fb, e->d_frames, &e->h_frames, &e->h_frames_cap, "frame");
+    return upload_host(e, (const void* const*)frames, std::vector<size_t>(n, fb), n, fb, e->d_frames.get(), "frame");
 }
 extern "C" int pe_forward_frames(pe_engine* e, const uint8_t* const* frames, int n) {
     NvtxRange r("pe_forward_frames (H2D)");
     int rc = check_n(e, n); if (rc) return rc;
     CK(e, cudaSetDevice(e->cfg.device));
     if ((rc = upload_frames(e, frames, n))) return rc;
-    return pe_forward_frames_device(e, e->d_frames, n);
+    return pe_forward_frames_device(e, e->d_frames.get(), n);
 }
 // bicubic weight table of OpenCV's fixed-point remap (initInterTab2D(INTER_CUBIC, fixpt)): a = -0.75, 15-bit shorts,
 // each 4x4 kernel normalised to sum 2^15 by nudging the largest/smallest central coefficient
@@ -1350,7 +1307,7 @@ static void build_warp_tab(std::vector<short>& tab) {
 }
 
 static int prepare_warp(pe_engine* e, int ow, int oh) {
-    if (e->warp_w == ow && e->warp_h == oh && e->d_wa) return PE_OK;
+    if (e->warp_w == ow && e->warp_h == oh) return PE_OK;
     const int dw = e->cfg.disp_w, dh = e->cfg.disp_h;
     // rtpose.cpp:474-480
     const double s = (ow / (double)oh > dw / (double)dh) ? dw / (double)ow : dh / (double)oh;
@@ -1364,15 +1321,13 @@ static int prepare_warp(pe_engine* e, int ow, int oh) {
     std::vector<int> ad(dw), bd(dw), x0(dh), y0(dh);
     for (int x = 0; x < dw; x++) { ad[x] = (int)lrint(M[0] * x * 1024); bd[x] = (int)lrint(M[3] * x * 1024); }
     for (int y = 0; y < dh; y++) { x0[y] = (int)lrint((M[1] * y + M[2]) * 1024) + 16; y0[y] = (int)lrint((M[4] * y + M[5]) * 1024) + 16; }
-    if (!e->d_wa) {
-        std::vector<short> tab;
-        build_warp_tab(tab);
-        CK(e, cudaMalloc(&e->d_wa, dw * sizeof(int))); CK(e, cudaMalloc(&e->d_wb, dw * sizeof(int)));
-        CK(e, cudaMalloc(&e->d_wx0, dh * sizeof(int))); CK(e, cudaMalloc(&e->d_wy0, dh * sizeof(int)));
-        CK(e, cudaMalloc(&e->d_wtab, tab.size() * sizeof(short)));
-        CK(e, cudaMemcpy(e->d_wtab, tab.data(), tab.size() * sizeof(short), cudaMemcpyHostToDevice));
-    }
+    std::vector<short> tab; build_warp_tab(tab);
+    e->warp_w = e->warp_h = 0;   // until every table below holds this size
+    CK(e, reserve_carved(e->d_warp, [&](Carver& k) {   // one size per engine: allocated once, never while queued work reads it
+        e->d_wa = k.take<int>(dw); e->d_wb = k.take<int>(dw); e->d_wx0 = k.take<int>(dh); e->d_wy0 = k.take<int>(dh); e->d_wtab = k.take<short>(tab.size());
+    }));
     CK(e, cudaStreamSynchronize(e->stream));
+    CK(e, cudaMemcpy(e->d_wtab, tab.data(), tab.size() * sizeof(short), cudaMemcpyHostToDevice));
     CK(e, cudaMemcpy(e->d_wa, ad.data(), dw * sizeof(int), cudaMemcpyHostToDevice));
     CK(e, cudaMemcpy(e->d_wb, bd.data(), dw * sizeof(int), cudaMemcpyHostToDevice));
     CK(e, cudaMemcpy(e->d_wx0, x0.data(), dh * sizeof(int), cudaMemcpyHostToDevice));
@@ -1386,24 +1341,24 @@ static int prepare_warp(pe_engine* e, int ow, int oh) {
 // display frames when needed and runs the net.
 static int frame_target(pe_engine* e, int W, int H, uint8_t** dst, double* scale) {
     if (W == e->cfg.disp_w && H == e->cfg.disp_h) {
-        *dst = e->d_frames;
+        *dst = e->d_frames.get();
         if (scale) *scale = 1.0;
         return PE_OK;
     }
     int rc = prepare_warp(e, W, H); if (rc) return rc;
-    rc = grow_buffer(e, &e->d_raw, &e->raw_cap, (size_t)W * H * 3 * e->cfg.max_batch, false); if (rc) return rc;
-    *dst = e->d_raw;
+    rc = grow_buffer(e, e->d_raw, (size_t)W * H * 3 * e->cfg.max_batch); if (rc) return rc;
+    *dst = e->d_raw.get();
     if (scale) *scale = e->warp_scale;
     return PE_OK;
 }
 static int finish_frames(pe_engine* e, int n, int W, int H) {
     if (W != e->cfg.disp_w || H != e->cfg.disp_h) {
         WarpArgs w;
-        w.src = e->d_raw; w.dst = e->d_frames; w.sw = W; w.sh = H; w.dw = e->cfg.disp_w; w.dh = e->cfg.disp_h;
+        w.src = e->d_raw.get(); w.dst = e->d_frames.get(); w.sw = W; w.sh = H; w.dw = e->cfg.disp_w; w.dh = e->cfg.disp_h;
         w.adelta = e->d_wa; w.bdelta = e->d_wb; w.x0 = e->d_wx0; w.y0 = e->d_wy0; w.tab = e->d_wtab;
         e->launches += launch_warp_affine(w, n, e->stream);
     }
-    return pe_forward_frames_device(e, e->d_frames, n);
+    return pe_forward_frames_device(e, e->d_frames.get(), n);
 }
 
 extern "C" int pe_forward_pixels(pe_engine* e, const pe_pixel_format* fmt, const void* const* frames, int n, double* scale) {
@@ -1433,25 +1388,21 @@ extern "C" int pe_forward_pixels(pe_engine* e, const pe_pixel_format* fmt, const
     rc = frame_target(e, L.w, L.h, &dst, scale); if (rc) return rc;
     const bool bgr = L.format == PE_PIX_BGR;
     const size_t fb = (size_t)L.w * L.h * 3, span = (size_t)L.span, stride = (span + 255) & ~(size_t)255;
-    // Pageable frames are staged in h_raw, which the queued work may still be reading: the stream is drained first.  Host frames
-    // other than BGR are copied whole to d_pix, and the kernel converts them there.
-    if (any_pageable) {
-        rc = grow_buffer(e, &e->h_raw, &e->h_raw_cap, stride * e->cfg.max_batch, true); if (rc) return rc;
-        CK(e, cudaStreamSynchronize(e->stream));
-    }
-    if (any_host && !bgr) { rc = grow_buffer(e, &e->d_pix, &e->pix_cap, stride * e->cfg.max_batch, false); if (rc) return rc; }
+    // Pageable frames go through the staging buffer.  Host frames other than BGR are copied whole to d_pix and converted there.
+    if (any_pageable && (rc = stage(e, stride * e->cfg.max_batch))) return rc;
+    if (any_host && !bgr && (rc = grow_buffer(e, e->d_pix, stride * e->cfg.max_batch))) return rc;
     PixArgs a;
     a.dst = dst; a.pitch = L.pitch; a.chroma = L.chroma; a.format = L.format; a.w = L.w; a.h = L.h; a.col = L.col;
     for (int i = 0; i < n; i++) {
         const uint8_t* src = (const uint8_t*)frames[i];
-        if (kind[i] == PAGEABLE) { memcpy(e->h_raw + i * stride, src, span); src = e->h_raw + i * stride; }
+        if (kind[i] == PAGEABLE) { memcpy(e->h_stage.get() + i * stride, src, span); src = e->h_stage.get() + i * stride; }
         if (bgr) {   // BGR needs no conversion: the copy into place drops the pitch
             CK(e, cudaMemcpy2DAsync(dst + i * fb, (size_t)L.w * 3, src, (size_t)L.pitch, (size_t)L.w * 3, L.h, cudaMemcpyDefault, e->stream));
         } else if (kind[i] == DEVICE) {
             a.src[i] = src;
         } else {
-            CK(e, cudaMemcpyAsync(e->d_pix + i * stride, src, span, cudaMemcpyHostToDevice, e->stream));
-            a.src[i] = e->d_pix + i * stride;
+            CK(e, cudaMemcpyAsync(e->d_pix.get() + i * stride, src, span, cudaMemcpyHostToDevice, e->stream));
+            a.src[i] = e->d_pix.get() + i * stride;
         }
     }
     if (!bgr) e->launches += launch_pixels_to_bgr(a, n, e->stream);
@@ -1510,8 +1461,8 @@ extern "C" int pe_forward_jpeg_coefs(pe_engine* e, const void* const* coefs, int
         max_blocks = std::max(max_blocks, (long long)(hd.total_bytes - (long long)sizeof hd) / 128);
     }
     const size_t stride = ((size_t)max_bytes + 255) & ~(size_t)255;
-    rc = grow_buffer(e, &e->d_jcoef, &e->jcoef_cap, stride * n, false); if (rc) return rc;
-    rc = upload_host(e, coefs, bytes, n, stride, e->d_jcoef, &e->h_jcoef, &e->h_jcoef_cap, "coefficient image"); if (rc) return rc;
+    rc = grow_buffer(e, e->d_jcoef, stride * n); if (rc) return rc;
+    rc = upload_host(e, coefs, bytes, n, stride, e->d_jcoef.get(), "coefficient image"); if (rc) return rc;
     return reconstruct_and_forward(e, n, W, H, stride, max_blocks, scale);
 }
 
@@ -1520,9 +1471,9 @@ static int reconstruct_and_forward(pe_engine* e, int n, int W, int H, size_t str
     uint8_t* dst;
     int rc = frame_target(e, W, H, &dst, scale); if (rc) return rc;
     const size_t pstride = ((size_t)max_blocks * 64 + 255) & ~(size_t)255;
-    rc = grow_buffer(e, &e->d_jplanes, &e->jplanes_cap, pstride * n, false); if (rc) return rc;
+    rc = grow_buffer(e, e->d_jplanes, pstride * n); if (rc) return rc;
     JpegArgs ja;
-    ja.coefs = e->d_jcoef; ja.coef_stride = (long long)stride; ja.planes = e->d_jplanes; ja.plane_stride = (long long)pstride;
+    ja.coefs = e->d_jcoef.get(); ja.coef_stride = (long long)stride; ja.planes = e->d_jplanes.get(); ja.plane_stride = (long long)pstride;
     ja.dst = dst; ja.W = W; ja.H = H; ja.n = n; ja.max_blocks = max_blocks;
     e->launches += launch_jpeg_reconstruct(ja, e->stream);
     return finish_frames(e, n, W, H);
@@ -1550,31 +1501,28 @@ static int decode_scans(pe_engine* e, const void* const* scans, int n, int S, in
         max_seg = std::max(max_seg, (long long)hd.num_segments);
         max_sub = std::max(max_sub, subs);
     }
-    auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-    const size_t sstride = al((size_t)max_scan);
-    *cstride = al((size_t)max_coef);
+    const size_t sstride = ((size_t)max_scan + 255) & ~(size_t)255;
+    *cstride = ((size_t)max_coef + 255) & ~(size_t)255;
     const int ctas = (int)((max_sub + pe_jpeg::SYNC_THREADS - 1) / pe_jpeg::SYNC_THREADS);
-    const size_t tab_b = al(jpeg_huff_tables_bytes() * n), seg_b = al((size_t)(max_seg + 1) * 4 * n), pub_b = al((size_t)ctas * 16 * n),
-                 flag_b = al((size_t)ctas * 4 * n), small_b = al((size_t)4 * n);
-    int rc = grow_buffer(e, &e->d_jcoef, &e->jcoef_cap, *cstride * n, false); if (rc) return rc;
-    rc = grow_buffer(e, &e->d_jscan, &e->jscan_cap, sstride * n, false); if (rc) return rc;
-    rc = grow_buffer(e, &e->d_jwork, &e->jwork_cap, tab_b + seg_b + pub_b + flag_b + 2 * small_b, false); if (rc) return rc;
-    rc = grow_buffer(e, &e->h_jstatus, &e->h_jstatus_cap, (size_t)4 * e->cfg.max_batch, true); if (rc) return rc;
-    rc = upload_host(e, scans, bytes, n, sstride, e->d_jscan, &e->h_jscan, &e->h_jscan_cap, "scan image"); if (rc) return rc;
-    CK(e, cudaMemsetAsync(e->d_jcoef, 0, *cstride * n, e->stream));
     JpegScanArgs a;
-    a.scans = e->d_jscan; a.scan_stride = (long long)sstride;
-    a.coefs = e->d_jcoef; a.coef_stride = (long long)*cstride;
-    uint8_t* w = e->d_jwork;
-    a.tabs = w; w += tab_b;
-    a.seg_sub = (int*)w; a.seg_stride = max_seg + 1; w += seg_b;
-    a.pub = (unsigned long long*)w; w += pub_b;
-    a.flags = (int*)w; w += flag_b;
-    a.tickets = (int*)w; w += small_b;
-    a.status = (int*)w;
-    a.ctas_max = ctas; a.n = n; a.S = S;
+    auto work = [&](Carver& k) {   // the decoder's work space
+        a.tabs = k.take<uint8_t>(jpeg_huff_tables_bytes() * n); a.seg_sub = k.take<int>((size_t)(max_seg + 1) * n);
+        a.pub = k.take<unsigned long long>((size_t)ctas * 2 * n); a.flags = k.take<int>((size_t)ctas * n); a.tickets = k.take<int>(n); a.status = k.take<int>(n);
+    };
+    Carver work_size(nullptr);
+    work(work_size);
+    int rc = grow_buffer(e, e->d_jcoef, *cstride * n); if (rc) return rc;
+    rc = grow_buffer(e, e->d_jscan, sstride * n); if (rc) return rc;
+    rc = grow_buffer(e, e->d_jwork, work_size.used()); if (rc) return rc;
+    rc = grow_buffer(e, e->h_jstatus, (size_t)4 * e->cfg.max_batch); if (rc) return rc;
+    rc = upload_host(e, scans, bytes, n, sstride, e->d_jscan.get(), "scan image"); if (rc) return rc;
+    CK(e, cudaMemsetAsync(e->d_jcoef.get(), 0, *cstride * n, e->stream));
+    a.scans = e->d_jscan.get(); a.scan_stride = (long long)sstride;
+    a.coefs = e->d_jcoef.get(); a.coef_stride = (long long)*cstride;
+    CK(e, reserve_carved(e->d_jwork, work));   // grown above: only lays the work space out
+    a.seg_stride = max_seg + 1; a.ctas_max = ctas; a.n = n; a.S = S;
     e->launches += launch_jpeg_entropy(a, e->stream);
-    CK(e, cudaMemcpyAsync(e->h_jstatus, a.status, (size_t)4 * n, cudaMemcpyDeviceToHost, e->stream));
+    CK(e, cudaMemcpyAsync(e->h_jstatus.get(), a.status, (size_t)4 * n, cudaMemcpyDeviceToHost, e->stream));
     CK(e, cudaGetLastError());
     return PE_OK;
 }
@@ -1605,8 +1553,8 @@ extern "C" int pe_jpeg_decode_scans(pe_engine* e, const void* const* scans, int 
     for (int i = 0; i < n; i++) {
         const pe_jpeg_scan_header& hd = *(const pe_jpeg_scan_header*)scans[i];
         if (!coefs_out[i]) return fail(e, PE_ERR_INVALID, "null output buffer %d", i);
-        CK(e, cudaMemcpy(coefs_out[i], e->d_jcoef + i * stride, (size_t)hd.coef.total_bytes, cudaMemcpyDeviceToHost));
-        if (status_out) { int st; memcpy(&st, e->h_jstatus + 4 * i, 4); status_out[i] = st == INT_MAX ? 0 : 1 + st; }
+        CK(e, cudaMemcpy(coefs_out[i], e->d_jcoef.get() + i * stride, (size_t)hd.coef.total_bytes, cudaMemcpyDeviceToHost));
+        if (status_out) { int st; memcpy(&st, e->h_jstatus.get() + 4 * i, 4); status_out[i] = st == INT_MAX ? 0 : 1 + st; }
     }
     return PE_OK;
 }
@@ -1625,14 +1573,14 @@ extern "C" int pe_jpeg_decode_scans(pe_engine* e, const void* const* scans, int 
 static int upload_fields(pe_engine* e, int i) {
     std::vector<float> B(epi_floats(e, i), 0.f);
     fill_epilogue_fields(e, i, B.data());
-    CK(e, cudaMemcpyAsync((char*)e->d_packed + e->b_off[i], B.data(), B.size() * sizeof(float), cudaMemcpyHostToDevice, e->stream));
+    CK(e, cudaMemcpyAsync(e->packed->get() + e->b_off[i], B.data(), B.size() * sizeof(float), cudaMemcpyHostToDevice, e->stream));
     return PE_OK;
 }
 
 static int upload_weights(pe_engine* e, int i) {   // re-pack layer i with the current input scales (host fp32 copy needed)
     std::vector<uint8_t> buf(weight_bytes(e, i));
     if (const int rc = pack_conv_weights(e, i, buf.data())) return rc;
-    CK(e, cudaMemcpyAsync((char*)e->d_packed + e->w_off[i], buf.data(), buf.size(), cudaMemcpyHostToDevice, e->stream));
+    CK(e, cudaMemcpyAsync(e->packed->get() + e->w_off[i], buf.data(), buf.size(), cudaMemcpyHostToDevice, e->stream));
     CK(e, cudaStreamSynchronize(e->stream));
     return PE_OK;
 }
@@ -1661,7 +1609,7 @@ static int calib_owner_check(pe_engine* e, const char* what) {
     if (!e->prec->ranged()) return fail(e, PE_ERR_INVALID, "%s: precision %d has no range scales (only 2, 4, 5 and 6 have)", what, e->cfg.precision);
     if (!owns_weights(e))
         return fail(e, PE_ERR_STATE, "%s: this handle received its weights by broadcast / sharing: calibrate the source handle, which owns them", what);
-    if (e->packed_owner.use_count() > 1)
+    if (e->packed.use_count() > 1)
         return fail(e, PE_ERR_STATE, "%s: this handle already shares its weights with another handle, which would keep the old scales: "
                     "calibrate before pe_share_weights", what);
     return PE_OK;
@@ -1675,7 +1623,7 @@ extern "C" int pe_calibrate(pe_engine* e, const uint8_t* const* frames, int n) {
     if (e->collecting) return fail(e, PE_ERR_STATE, "a calibration collection is running: call pe_calibrate_end first");
     CK(e, cudaSetDevice(e->cfg.device));
     drop_graphs(e);
-    if ((rc = upload_frames(e, frames, n)) || (rc = preprocess_frames(e, e->d_frames, n))) return rc;
+    if ((rc = upload_frames(e, frames, n)) || (rc = preprocess_frames(e, e->d_frames.get(), n))) return rc;
     const std::vector<float> packed_with = e->conv_scale;
     const int nimg = n * e->cfg.num_scales;
     for (const OpRef& op : e->plan.order) {
@@ -1685,10 +1633,10 @@ extern "C" int pe_calibrate(pe_engine* e, const uint8_t* const* frames, int n) {
         if (stores) e->conv_scale[i] = 1.f;   // measure the true output range: fp32 epilogue values, before the fp16 split
         if ((rc = refresh_layer(e, i, packed_with))) return rc;   // its producers are final (plan order)
         if (stores) {
-            CK(e, cudaMemsetAsync(e->d_range + i, 0, sizeof(unsigned), e->stream));
+            CK(e, cudaMemsetAsync(e->d_range.get<unsigned>() + i, 0, sizeof(unsigned), e->stream));
             if ((rc = run_op(e, op, nimg))) return rc;
             unsigned bits = 0;
-            CK(e, cudaMemcpyAsync(&bits, e->d_range + i, sizeof bits, cudaMemcpyDeviceToHost, e->stream));
+            CK(e, cudaMemcpyAsync(&bits, e->d_range.get<unsigned>() + i, sizeof bits, cudaMemcpyDeviceToHost, e->stream));
             CK(e, cudaStreamSynchronize(e->stream));
             float m; memcpy(&m, &bits, 4);
             e->conv_scale[i] = pow2_for(m, out_row(e, i).range_top);
@@ -1696,7 +1644,7 @@ extern "C" int pe_calibrate(pe_engine* e, const uint8_t* const* frames, int n) {
         }
         if ((rc = run_op(e, op, nimg))) return rc;
     }
-    CK(e, cudaMemsetAsync(e->d_range, 0, e->plan.convs.size() * sizeof(unsigned), e->stream));
+    CK(e, cudaMemsetAsync(e->d_range.get(), 0, e->plan.convs.size() * sizeof(unsigned), e->stream));
     e->calibrated = true;
     return run_post_and_return(e, n);
 }
@@ -1719,13 +1667,13 @@ extern "C" int pe_range_status(pe_engine* e, float* worst_ratio, char* layer64) 
     if (!e) return PE_ERR_INVALID;
     if (worst_ratio) *worst_ratio = 0.f;
     if (layer64) layer64[0] = 0;
-    if (!e->d_range) return PE_OK;
+    if (!e->d_range.size()) return PE_OK;
     CK(e, cudaSetDevice(e->cfg.device));
     CK(e, cudaStreamSynchronize(e->stream));
     const size_t nc = e->plan.convs.size();
     std::vector<unsigned> bits(nc);
-    CK(e, cudaMemcpy(bits.data(), e->d_range, nc * sizeof(unsigned), cudaMemcpyDeviceToHost));
-    CK(e, cudaMemset(e->d_range, 0, nc * sizeof(unsigned)));
+    CK(e, cudaMemcpy(bits.data(), e->d_range.get(), nc * sizeof(unsigned), cudaMemcpyDeviceToHost));
+    CK(e, cudaMemset(e->d_range.get(), 0, nc * sizeof(unsigned)));
     fold_range(e, bits);
     float worst = 0.f, smallest = 3e38f, lowest = 3e38f;   // lowest: the smallest maximum relative to its layer's floor
     int iw = -1, is = -1;
@@ -1795,7 +1743,7 @@ static int apply_scales(pe_engine* e, const std::vector<float>& s, int* changed)
     int moved = 0;
     for (size_t i = 0; i < s.size(); i++) moved += s[i] != old[i];
     for (size_t i = 0; i < s.size(); i++) { const int rc = refresh_layer(e, (int)i, old); if (rc) return rc; }
-    CK(e, cudaMemsetAsync(e->d_range, 0, s.size() * sizeof(unsigned), e->stream));
+    CK(e, cudaMemsetAsync(e->d_range.get(), 0, s.size() * sizeof(unsigned), e->stream));
     CK(e, cudaStreamSynchronize(e->stream));
     e->calibrated = true;
     if (changed) *changed = moved;
@@ -1810,7 +1758,7 @@ extern "C" int pe_calibrate_begin(pe_engine* e) {
         return fail(e, PE_ERR_STATE, "pe_calibrate_begin: PE_PREC_S8X1 forwards only on calibrated scales: start with pe_calibrate or pe_calibration_set");
     CK(e, cudaSetDevice(e->cfg.device));
     CK(e, cudaStreamSynchronize(e->stream));
-    CK(e, cudaMemset(e->d_range, 0, e->plan.convs.size() * sizeof(unsigned)));   // maxima of earlier forwards do not count
+    CK(e, cudaMemset(e->d_range.get(), 0, e->plan.convs.size() * sizeof(unsigned)));   // maxima of earlier forwards do not count
     e->collect_max.assign(e->plan.convs.size(), 0.f);
     e->collect_forwards = 0;
     e->collecting = true;
@@ -1827,7 +1775,7 @@ extern "C" int pe_calibrate_end(pe_engine* e, int* changed) {
     CK(e, cudaStreamSynchronize(e->stream));
     const size_t nc = e->plan.convs.size();
     std::vector<unsigned> bits(nc);
-    CK(e, cudaMemcpy(bits.data(), e->d_range, nc * sizeof(unsigned), cudaMemcpyDeviceToHost));
+    CK(e, cudaMemcpy(bits.data(), e->d_range.get(), nc * sizeof(unsigned), cudaMemcpyDeviceToHost));
     fold_range(e, bits);
     e->collecting = false;
     std::vector<float> s = e->conv_scale;
@@ -1872,12 +1820,12 @@ extern "C" int pe_forward_net_input(pe_engine* e, const float* net_input, int n)
     if (!net_input) return fail(e, PE_ERR_INVALID, "null input");
     CK(e, cudaSetDevice(e->cfg.device));
     const size_t cnt = (size_t)n * e->cfg.num_scales * 3 * e->cfg.net_w * e->cfg.net_h;
-    CK(e, cudaStreamSynchronize(e->stream));
-    memcpy(e->h_planar, net_input, cnt * sizeof(float));
-    CK(e, cudaMemcpyAsync(e->d_planar, e->h_planar, cnt * sizeof(float), cudaMemcpyHostToDevice, e->stream));
+    if ((rc = stage(e, cnt * sizeof(float)))) return rc;   // a copy, so the caller may reuse its input when the call returns
+    memcpy(e->h_stage.get(), net_input, cnt * sizeof(float));
+    CK(e, cudaMemcpyAsync(e->d_planar.get(), e->h_stage.get(), cnt * sizeof(float), cudaMemcpyHostToDevice, e->stream));
     PreArgs a = e->pre;
     a.nframes = n;
-    e->launches += launch_input_from_planar(e->d_planar, a, n * e->cfg.num_scales, e->stream);
+    e->launches += launch_input_from_planar(e->d_planar.get<float>(), a, n * e->cfg.num_scales, e->stream);
     e->input_lo_dirty = e->prec->fmt.planes > 0;
     e->last_frames = nullptr;
     return run_net(e, n);
@@ -1887,9 +1835,9 @@ extern "C" int pe_forward_maps(pe_engine* e, const float* maps8, int n) {
     if (!maps8) return fail(e, PE_ERR_INVALID, "null maps");
     CK(e, cudaSetDevice(e->cfg.device));
     const size_t cnt = (size_t)n * e->cfg.num_scales * e->mt->num_maps * e->geo[3].W * e->geo[3].H;
-    CK(e, cudaStreamSynchronize(e->stream));
-    memcpy(e->h_maps, maps8, cnt * sizeof(float));
-    CK(e, cudaMemcpyAsync(e->d_maps, e->h_maps, cnt * sizeof(float), cudaMemcpyHostToDevice, e->stream));
+    if ((rc = stage(e, cnt * sizeof(float)))) return rc;   // a copy, so the caller may reuse its input when the call returns
+    memcpy(e->h_stage.get(), maps8, cnt * sizeof(float));
+    CK(e, cudaMemcpyAsync(e->d_maps.get(), e->h_stage.get(), cnt * sizeof(float), cudaMemcpyHostToDevice, e->stream));
     e->last_frames = nullptr;
     return run_post_and_return(e, n);
 }
@@ -1910,51 +1858,43 @@ extern "C" int pe_render(pe_engine* e, int idx, int part_to_show, int googly_eye
         return fail(e, PE_ERR_STATE, "the last forward had no display frame (net-input / map path): pass display_bgr");
     CK(e, cudaSetDevice(e->cfg.device));
     const size_t px = (size_t)W * H;
-    if (!e->d_canvas) {
-        CK(e, cudaMalloc(&e->d_canvas, px * 3 * sizeof(float)));
-        CK(e, cudaMalloc(&e->d_render_u8, px * 3));
-        CK(e, cudaMalloc(&e->d_render_src, px * 3));
-    }
+    float* d_canvas; uint8_t *d_u8, *d_src;   // one size per engine: allocated by the first call
+    CK(e, reserve_carved(e->d_render, [&](Carver& k) { d_canvas = k.take<float>(px * 3); d_u8 = k.take<uint8_t>(px * 3); d_src = k.take<uint8_t>(px * 3); }));
     const uint8_t* src = e->last_frames ? e->last_frames + (size_t)idx * px * 3 : nullptr;
     if (display_bgr) {
-        CK(e, cudaMemcpyAsync(e->d_render_src, display_bgr, px * 3, cudaMemcpyHostToDevice, e->stream));
-        src = e->d_render_src;
+        CK(e, cudaMemcpyAsync(d_src, display_bgr, px * 3, cudaMemcpyHostToDevice, e->stream));
+        src = d_src;
     }
-    e->launches += launch_canvas_fill(src, e->d_canvas, W, H, e->stream);   // process_and_pad_image(normalize = 0), rtpose.cpp:349,1127
+    e->launches += launch_canvas_fill(src, d_canvas, W, H, e->stream);   // process_and_pad_image(normalize = 0), rtpose.cpp:349,1127
     const PostDev& pd = e->post;
     const float* poses = pd.joints + (size_t)idx * PE_MAX_PEOPLE * P * 3;
     auto heat = [&](int ch0, int nch) -> int {   // the channels a heat-map view reads, from the stride-8 maps
-        const size_t need = (size_t)nch * nw * nh * sizeof(float);
-        if (need > e->heat_cap) {
-            cudaFree(e->d_heat); e->d_heat = nullptr; e->heat_cap = 0;
-            CK(e, cudaMalloc(&e->d_heat, need));
-            e->heat_cap = need;
-        }
-        e->launches += launch_fullres_fill(pd, idx, ch0, nch, e->d_heat, e->stream);
+        CK(e, e->d_heat.reserve((size_t)nch * nw * nh * sizeof(float)));
+        e->launches += launch_fullres_fill(pd, idx, ch0, nch, e->d_heat.get<float>(), e->stream);
         return PE_OK;
     };
     int rc = PE_OK;
     if (part_to_show == 0) {
-        e->launches += launch_skeleton(e->cfg.model, e->d_canvas, W, H, poses, pd.num_people + idx, googly_eyes, e->stream);
+        e->launches += launch_skeleton(e->cfg.model, d_canvas, W, H, poses, pd.num_people + idx, googly_eyes, e->stream);
     } else if (e->cfg.model == PE_MODEL_MPI_15) {                 // render_mpi_parts: channel part_to_show-1
         if ((rc = heat(part_to_show - 1, 1))) return rc;
-        e->launches += launch_heat_view(e->d_canvas, W, H, e->d_heat, nw, nh, 0, part_to_show - 1, 1, e->stream);
+        e->launches += launch_heat_view(d_canvas, W, H, e->d_heat.get<float>(), nw, nh, 0, part_to_show - 1, 1, e->stream);
     } else if (part_to_show - 1 < P) {                            // render_coco_parts: one part map
         if ((rc = heat(part_to_show - 1, 1))) return rc;
-        e->launches += launch_heat_view(e->d_canvas, W, H, e->d_heat, nw, nh, 1, part_to_show - 1, 1, e->stream);
+        e->launches += launch_heat_view(d_canvas, W, H, e->d_heat.get<float>(), nw, nh, 1, part_to_show - 1, 1, e->stream);
     } else if (part_to_show - 1 == P) {                           // all part maps, nearest neighbour (heatmap2)
         if ((rc = heat(0, P))) return rc;
-        e->launches += launch_heat_view(e->d_canvas, W, H, e->d_heat, nw, nh, 2, 0, P, e->stream);
+        e->launches += launch_heat_view(d_canvas, W, H, e->d_heat.get<float>(), nw, nh, 2, 0, P, e->stream);
     } else {                                                      // render_coco_aff (rtpose.cpp:286-296)
         int aff_part = ((part_to_show - 1) - P - 1) * 2, accum = 1;
         if (aff_part == 0) accum = e->mt->num_limbs; else aff_part -= 2;
         aff_part += 1 + P;
         if ((rc = heat(aff_part, 2 * accum))) return rc;
-        e->launches += launch_heat_view(e->d_canvas, W, H, e->d_heat, nw, nh, 3, aff_part, 2 * accum, e->stream);
+        e->launches += launch_heat_view(d_canvas, W, H, e->d_heat.get<float>(), nw, nh, 3, aff_part, 2 * accum, e->stream);
     }
-    if (bgr) e->launches += launch_canvas_to_u8(e->d_canvas, e->d_render_u8, W, H, e->stream);   // postProcessFrame, rtpose.cpp:1286-1296
-    if (canvas) CK(e, cudaMemcpyAsync(canvas, e->d_canvas, px * 3 * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
-    if (bgr) CK(e, cudaMemcpyAsync(bgr, e->d_render_u8, px * 3, cudaMemcpyDeviceToHost, e->stream));
+    if (bgr) e->launches += launch_canvas_to_u8(d_canvas, d_u8, W, H, e->stream);   // postProcessFrame, rtpose.cpp:1286-1296
+    if (canvas) CK(e, cudaMemcpyAsync(canvas, d_canvas, px * 3 * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
+    if (bgr) CK(e, cudaMemcpyAsync(bgr, d_u8, px * 3, cudaMemcpyDeviceToHost, e->stream));
     CK(e, cudaStreamSynchronize(e->stream));
     CK(e, cudaGetLastError());
     return PE_OK;
@@ -2005,7 +1945,7 @@ extern "C" int pe_fetch(pe_engine* e, int idx, float* joints, int* num_people, f
     if (e->check_range && idx == 0) { rc = pe_range_status(e, nullptr, nullptr); if (rc) return rc; }   // PE_CHECK_RANGE=1: range problems are errors
     if (idx < e->jstatus_n) {   // a frame from a scan image whose entropy-coded data the host entropy stage rejects
         int mcu;
-        memcpy(&mcu, e->h_jstatus + 4 * idx, 4);
+        memcpy(&mcu, e->h_jstatus.get() + 4 * idx, 4);
         if (mcu != INT_MAX) return fail(e, PE_ERR_IO, "frame %d: corrupt JPEG data (DC category above 15) in MCU %d", idx, mcu);
     }
     const int P = e->mt->num_parts, MP = e->mt->max_peaks;
@@ -2018,9 +1958,10 @@ extern "C" int pe_fetch_maps(pe_engine* e, float* maps8, int n) {
     int rc = check_n(e, n); if (rc) return rc;
     CK(e, cudaSetDevice(e->cfg.device));
     const size_t cnt = (size_t)n * e->cfg.num_scales * e->mt->num_maps * e->geo[3].W * e->geo[3].H;
-    CK(e, cudaMemcpyAsync(e->h_maps, e->d_maps, cnt * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
+    if ((rc = grow_buffer(e, e->h_stage, cnt * sizeof(float)))) return rc;   // the copy queues behind the staging's readers
+    CK(e, cudaMemcpyAsync(e->h_stage.get(), e->d_maps.get(), cnt * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
     CK(e, cudaStreamSynchronize(e->stream));
-    memcpy(maps8, e->h_maps, cnt * sizeof(float));
+    memcpy(maps8, e->h_stage.get(), cnt * sizeof(float));
     return PE_OK;
 }
 static float blob_scale(const pe_engine* e, const BlobRef& b) {
@@ -2056,16 +1997,15 @@ extern "C" int pe_fetch_blob(pe_engine* e, const char* blob_name, float* out, si
         if (w) *w = g.W;
         if (!out) return PE_OK;
         if (cnt > cap) return fail(e, PE_ERR_INVALID, "blob %s needs %zu floats", blob_name, cnt);
-        float* d = nullptr;
-        CK(e, cudaMalloc(&d, cnt * sizeof(float)));
+        DeviceBuffer d;
+        CK(e, d.reserve(cnt * sizeof(float)));
         // stored value = true value * conv_scale[producer] (pools pass their producer's scale through; the net input has
         // the mode's net_input_scale); s8: q * 2^-k, exact in fp32
         const float inv = 1.f / blob_scale(e, b);
-        e->launches += launch_act_to_nchw(e->acts[b.act], e->plan.acts[b.act].C, b.coff, b.c, e->act_plane[b.act], act_fmt(e, b.act), g, inv, d,
-                                          e->stream);
-        CK(e, cudaMemcpyAsync(out, d, cnt * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
+        e->launches += launch_act_to_nchw(e->acts[b.act].get(), e->plan.acts[b.act].C, b.coff, b.c, e->act_plane[b.act], act_fmt(e, b.act), g, inv,
+                                          d.get<float>(), e->stream);
+        CK(e, cudaMemcpyAsync(out, d.get(), cnt * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
         CK(e, cudaStreamSynchronize(e->stream));
-        cudaFree(d);
         return PE_OK;
     }
     return fail(e, PE_ERR_INVALID, "unknown blob %s", blob_name);
