@@ -14,6 +14,10 @@ class Buffer {
 public:
     Buffer() = default;
     Buffer(Buffer&& o) noexcept : p_(o.p_), n_(o.n_) { o.p_ = nullptr; o.n_ = 0; }
+    Buffer& operator=(Buffer&& o) noexcept {   // frees what this buffer held, on the current device
+        if (this != &o) { if (p_) Release(p_); p_ = o.p_; n_ = o.n_; o.p_ = nullptr; o.n_ = 0; }
+        return *this;
+    }
     ~Buffer() { if (p_) Release(p_); }
     // At least `need` bytes: a no-op when the buffer holds that many, else it frees and allocates `need`.  A failed allocation
     // leaves the buffer empty, so the next reserve allocates again whatever it asks for.

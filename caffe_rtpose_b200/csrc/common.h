@@ -46,6 +46,7 @@ struct ModelTables {
 };
 const ModelTables& model_tables(int model);
 const char* model_part_name(int model, int idx);
+int model_flip_table(int model, std::vector<int>& perm, std::vector<float>& sign);   // plan.cpp: num_maps, or -1
 
 // One convolution of the deploy graph in engine form.
 struct ConvSpec {

@@ -47,8 +47,10 @@ struct pe_engine {
     Geo geo[4];
     const Precision* prec = nullptr;   // the precision mode's row (precision.h)
     bool u8 = false;                   // PE_PREC_FLAG_U8 (cfg.precision holds the mode without it): the plan's u8 activations
+    bool flip = false;                 // the flip test (pe_set_flip_test): each frame's S images plus their S mirrors in x
     // What a captured forward graph references (activations, maps, post and result buffers, packed weights, d_range, axis tables) is
-    // allocated once, in pe_create or commit, and never regrown: a replayed graph keeps its pointers.  Only input-route buffers grow.
+    // allocated once, in pe_create or commit, and never regrown: a replayed graph keeps its pointers.  Only input-route buffers grow,
+    // and the per-image buffers (activations, maps: geo[*].N images) when pe_set_flip_test doubles them, which drops the graphs.
     std::vector<DeviceBuffer> acts;
     std::vector<long long> act_plane;  // elements per plane
     std::vector<HostWeights> hw;    // per conv
@@ -121,6 +123,10 @@ struct pe_engine {
 
 static void drop_graphs(pe_engine* e);
 static int setup_lanes(pe_engine* e);
+static int bind_packed(pe_engine* e);
+
+// Images the conv stack runs per frame: the S scales, and with the flip test their S mirrors
+static int copies(const pe_engine* e) { return e->cfg.num_scales * (e->flip ? 2 : 1); }
 
 // Storage of activation i: the mode's plane count in the element kind the plan gave it (plan.cpp: the kind of the conv layers
 // that read it).  conv i's packed weights have the kind of its arithmetic, which is that of its input.
@@ -258,6 +264,49 @@ static int build_pre_tables(pe_engine* e) {
 // create / destroy
 // ---------------------------------------------------------------------------------------------
 static int pooled(int v) { return (int)ceilf((float)(v - 2) / 2) + 1; }  // pooling_layer.cpp:90-93, k=2 s=2 pad=0
+
+// The four resolution levels' geometry for N images
+static void image_geo(const pe_engine* e, int N, Geo* geo) {
+    int w = e->cfg.net_w, h = e->cfg.net_h;
+    for (int l = 0; l < 4; l++) {
+        geo[l] = make_geo(w, h, e->plan.gap[l], N);
+        w = pooled(w); h = pooled(h);
+    }
+}
+
+// The per-image buffers - activations and stride-8 maps - for N images, zeroed (gap rows must be).  They are allocated next to the
+// old ones first: when an allocation fails the engine is left as it was.  Existing layers are re-bound to the new buffers.
+static int alloc_images(pe_engine* e, int N) {
+    Geo geo[4];
+    image_geo(e, N, geo);
+    const size_t na = e->plan.acts.size();
+    std::vector<DeviceBuffer> acts(na);
+    std::vector<long long> plane(na);
+    for (size_t i = 0; i < na; i++) {
+        const ActSpec& a = e->plan.acts[i];
+        plane[i] = geo[a.level].M * a.C;
+        const size_t bytes = (size_t)plane[i] * fmt_bytes(act_fmt(e, (int)i));
+        CK(e, acts[i].reserve(bytes));
+        CK(e, cudaMemsetAsync(acts[i].get(), 0, bytes, e->stream));
+    }
+    DeviceBuffer maps;
+    const size_t maps_bytes = (size_t)N * e->mt->num_maps * geo[3].W * geo[3].H * sizeof(float);
+    CK(e, maps.reserve(maps_bytes));
+    CK(e, cudaMemsetAsync(maps.get(), 0, maps_bytes, e->stream));
+    CK(e, cudaStreamSynchronize(e->stream));   // the old buffers go below: no queued work may still use them
+    if (e->stream2) CK(e, cudaStreamSynchronize(e->stream2));
+    for (int l = 0; l < 4; l++) e->geo[l] = geo[l];
+    e->acts = std::move(acts);
+    e->act_plane = std::move(plane);
+    e->d_maps = std::move(maps);
+    e->post.maps = e->d_maps.get<float>();
+    e->pre.out = e->acts[e->plan.input_act].get();
+    e->pre.out_plane = e->act_plane[e->plan.input_act];
+    e->input_lo_dirty = false;
+    if (!e->committed) return PE_OK;
+    e->committed = false;   // until the layers point at the new buffers
+    return bind_packed(e);
+}
 
 static void set_post_params(pe_engine* e) {
     PostParams& p = e->post.p;
@@ -494,11 +543,7 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, const
             }
         }
     const int N = cfg->max_batch * cfg->num_scales;
-    int w = cfg->net_w, h = cfg->net_h;
-    for (int l = 0; l < 4; l++) {
-        e->geo[l] = make_geo(w, h, e->plan.gap[l], N);
-        w = pooled(w); h = pooled(h);
-    }
+    image_geo(e, N, e->geo);
     if (e->geo[3].W * 8 != cfg->net_w || e->geo[3].H * 8 != cfg->net_h) { fail(e, PE_ERR_INVALID, "net size not divisible by 8 after pooling"); return bail(PE_ERR_INVALID); }
     e->hw.resize(e->plan.convs.size());
     if (prec.fmt.planes && setup_lanes(e)) return bail(PE_ERR_CUDA);
@@ -509,29 +554,16 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, const
         c.flops_per_image = 2.0 * c.cout * c.cin * c.k * c.k * g.H * g.W;
         e->flops_per_scale += c.flops_per_image;
     }
-    // activations
-    e->acts.resize(e->plan.acts.size());
-    e->act_plane.assign(e->plan.acts.size(), 0);
-    for (size_t i = 0; i < e->plan.acts.size(); i++) {
-        const ActSpec& a = e->plan.acts[i];
-        const Geo& g = e->geo[a.level];
-        e->act_plane[i] = g.M * a.C;
-        const size_t bytes = (size_t)e->act_plane[i] * fmt_bytes(act_fmt(e, (int)i));
-        CKC(e->acts[i].reserve(bytes));
-        CKC(cudaMemsetAsync(e->acts[i].get(), 0, bytes, e->stream));
-    }
     // io buffers
     CKC(e->d_frames.reserve((size_t)cfg->disp_w * cfg->disp_h * 3 * cfg->max_batch));
     CKC(e->d_resized.reserve((size_t)N * cfg->net_w * cfg->net_h * 3));
     CKC(e->d_planar.reserve((size_t)N * 3 * cfg->net_w * cfg->net_h * sizeof(float)));
-    const size_t maps_bytes = (size_t)N * e->mt->num_maps * e->geo[3].W * e->geo[3].H * sizeof(float);
-    CKC(e->d_maps.reserve(maps_bytes));
-    CKC(cudaMemsetAsync(e->d_maps.get(), 0, maps_bytes, e->stream));
     if (build_pre_tables(e)) return bail(PE_ERR_INVALID);
     e->pre.frames = e->d_frames.get(); e->pre.resized = e->d_resized.get();
-    e->pre.out = e->acts[e->plan.input_act].get(); e->pre.kp = e->plan.kp_input;
-    e->pre.out_plane = e->act_plane[e->plan.input_act]; e->pre.fmt = act_fmt(e, e->plan.input_act);
+    e->pre.kp = e->plan.kp_input; e->pre.fmt = act_fmt(e, e->plan.input_act);
     e->pre.Wp = e->geo[0].Wp; e->pre.Hs = e->geo[0].Hs;
+    // activations and maps
+    if (alloc_images(e, N)) return bail(PE_ERR_CUDA);
 
     // post-processing state
     set_post_params(e);
@@ -546,13 +578,19 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, const
     }
     for (int i = 0; i < 2 * e->mt->num_limbs; i++) { pd.md.limb_seq[i] = e->mt->limb_seq[i]; pd.md.map_idx[i] = e->mt->map_idx[i]; }
     const size_t B = cfg->max_batch, P = e->mt->num_parts, MP = e->mt->max_peaks, NL = e->mt->num_limbs;
-    pd.maps = e->d_maps.get<float>();
+    pd.copies = cfg->num_scales;
+    std::vector<int> perm;
+    std::vector<float> sign;
+    if (model_flip_table(cfg->model, perm, sign) != e->mt->num_maps) { fail(e, PE_ERR_INVALID, "model %d: a part or limb has no mirror", cfg->model); return bail(PE_ERR_INVALID); }
+    std::vector<FlipTap> flip(perm.size());
+    for (size_t c = 0; c < perm.size(); c++) flip[c] = {perm[c], sign[c]};
     pd.sort_stride = 1;
     while (pd.sort_stride < (int)(MP * MP)) pd.sort_stride <<= 1;
     CKC(post_set_smem_limits());
     pd.p.max_subset_rows = (int)(NL * MP);
     CKC(reserve_carved(e->d_post, [&](Carver& d) {   // the post-processing arrays and the axis tables
         pd.xtab = e->d_xtab = d.take<AxisTap>((size_t)cfg->num_scales * cfg->net_w); pd.ytab = e->d_ytab = d.take<AxisTap>((size_t)cfg->num_scales * cfg->net_h);
+        pd.flip = d.take<FlipTap>(flip.size());
         pd.flags = d.take<unsigned>(B * P * cfg->net_h * ((cfg->net_w + 31) / 32)); pd.peaks = d.take<float>(B * P * (MP + 1) * 3);
         pd.cands = d.take<Cand>(B * NL * MP * MP); pd.cand_count = d.take<int>(B * NL);
         pd.conns = d.take<Conn>(B * NL * MP); pd.conn_count = d.take<int>(B * NL);
@@ -562,6 +600,7 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, const
     CKC(reserve_carved(e->h_results, [&](Carver& r) { e->h_joints = r.take<float>(B * PE_MAX_PEOPLE * P * 3); e->h_num_people = r.take<int>(B);
                                                        e->h_peaks = r.take<float>(B * P * (MP + 1) * 3); }));
     CKC(cudaMemset(pd.conn_count, 0, sizeof(int) * B * NL));
+    CKC(cudaMemcpy((void*)pd.flip, flip.data(), flip.size() * sizeof(FlipTap), cudaMemcpyHostToDevice));
     launch_axis_tables(e->d_xtab, e->d_ytab, pd.p, e->stream);
     e->launches += 2;
     CKC(cudaStreamSynchronize(e->stream));
@@ -1044,6 +1083,40 @@ extern "C" int pe_set_connect_params(pe_engine* e, int min_cnt, float min_score,
     return PE_OK;
 }
 
+// The flip test.  Turning it on the first time doubles the per-image buffers; they stay that size when it is turned off again (a
+// forward reads only its own images).  The results of earlier forwards are dropped: their maps have the other layout.
+extern "C" int pe_set_flip_test(pe_engine* e, int on) {
+    if (!e) return PE_ERR_INVALID;
+    if (e->collecting)
+        return fail(e, PE_ERR_STATE, "pe_set_flip_test: a calibration collection is running: call pe_calibrate_end first");
+    if ((on != 0) == e->flip) return PE_OK;
+    CK(e, cudaSetDevice(e->cfg.device));
+    const int need = 2 * e->cfg.max_batch * e->cfg.num_scales;
+    if (on && e->geo[0].N < need) { const int rc = alloc_images(e, need); if (rc) return rc; }
+    CK(e, cudaStreamSynchronize(e->stream));
+    drop_graphs(e);
+    e->flip = on != 0;
+    e->pre.flip = e->flip;
+    e->post.copies = copies(e);
+    e->last_n = 0;
+    e->jstatus_n = 0;
+    return PE_OK;
+}
+extern "C" int pe_get_flip_test(const pe_engine* e) { return e && e->flip ? 1 : 0; }
+
+extern "C" int pe_model_flip_table(int model, int* perm, float* sign, int cap) {
+    if (model != PE_MODEL_MPI_15 && model != PE_MODEL_COCO_18) return -fail(nullptr, PE_ERR_INVALID, "unknown model %d", model);
+    std::vector<int> p;
+    std::vector<float> s;
+    const int n = model_flip_table(model, p, s);
+    if (n < 0) return -fail(nullptr, PE_ERR_STATE, "model %d: a part or limb has no mirror", model);
+    if (cap >= n) {
+        if (perm) memcpy(perm, p.data(), n * sizeof(int));
+        if (sign) memcpy(sign, s.data(), n * sizeof(float));
+    }
+    return n;
+}
+
 // ---------------------------------------------------------------------------------------------
 // forward
 // ---------------------------------------------------------------------------------------------
@@ -1103,7 +1176,7 @@ static int run_post_and_return(pe_engine* e, int n) {
 
 static int run_net_eager(pe_engine* e, int n) {
     NvtxRange r("pe: conv stack + parse");
-    const int nimg = n * e->cfg.num_scales;
+    const int nimg = n * copies(e);
     if (!e->two_lanes) {
         for (const OpRef& op : e->plan.order) { const int rc = run_op(e, op, nimg); if (rc) return rc; }
         return run_post_and_return(e, n);
@@ -1625,7 +1698,7 @@ extern "C" int pe_calibrate(pe_engine* e, const uint8_t* const* frames, int n) {
     drop_graphs(e);
     if ((rc = upload_frames(e, frames, n)) || (rc = preprocess_frames(e, e->d_frames.get(), n))) return rc;
     const std::vector<float> packed_with = e->conv_scale;
-    const int nimg = n * e->cfg.num_scales;
+    const int nimg = n * copies(e);
     for (const OpRef& op : e->plan.order) {
         if (op.type != 0) { if ((rc = run_op(e, op, nimg))) return rc; continue; }
         const int i = op.idx;
@@ -1834,7 +1907,7 @@ extern "C" int pe_forward_maps(pe_engine* e, const float* maps8, int n) {
     int rc = check_n(e, n); if (rc) return rc;
     if (!maps8) return fail(e, PE_ERR_INVALID, "null maps");
     CK(e, cudaSetDevice(e->cfg.device));
-    const size_t cnt = (size_t)n * e->cfg.num_scales * e->mt->num_maps * e->geo[3].W * e->geo[3].H;
+    const size_t cnt = (size_t)n * copies(e) * e->mt->num_maps * e->geo[3].W * e->geo[3].H;
     if ((rc = stage(e, cnt * sizeof(float)))) return rc;   // a copy, so the caller may reuse its input when the call returns
     memcpy(e->h_stage.get(), maps8, cnt * sizeof(float));
     CK(e, cudaMemcpyAsync(e->d_maps.get(), e->h_stage.get(), cnt * sizeof(float), cudaMemcpyHostToDevice, e->stream));
@@ -1957,7 +2030,7 @@ extern "C" int pe_fetch(pe_engine* e, int idx, float* joints, int* num_people, f
 extern "C" int pe_fetch_maps(pe_engine* e, float* maps8, int n) {
     int rc = check_n(e, n); if (rc) return rc;
     CK(e, cudaSetDevice(e->cfg.device));
-    const size_t cnt = (size_t)n * e->cfg.num_scales * e->mt->num_maps * e->geo[3].W * e->geo[3].H;
+    const size_t cnt = (size_t)n * copies(e) * e->mt->num_maps * e->geo[3].W * e->geo[3].H;
     if ((rc = grow_buffer(e, e->h_stage, cnt * sizeof(float)))) return rc;   // the copy queues behind the staging's readers
     CK(e, cudaMemcpyAsync(e->h_stage.get(), e->d_maps.get(), cnt * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
     CK(e, cudaStreamSynchronize(e->stream));
@@ -1984,7 +2057,7 @@ extern "C" int pe_blob_log2_scale(pe_engine* e, const char* blob_name, int* k) {
 extern "C" int pe_fetch_blob(pe_engine* e, const char* blob_name, float* out, size_t cap, int* c, int* h, int* w) {
     if (!e || !blob_name) return PE_ERR_INVALID;
     CK(e, cudaSetDevice(e->cfg.device));
-    const int nimg = std::max(e->last_n, 1) * e->cfg.num_scales;
+    const int nimg = std::max(e->last_n, 1) * copies(e);
     for (const BlobRef& b : e->plan.blobs) {
         if (b.name != blob_name) continue;
         if (!b.reused_by.empty())
@@ -2103,7 +2176,7 @@ extern "C" int pe_profile_layers(pe_engine* e, int n, float* ms, char* names, do
     int rc = check_n(e, n); if (rc) return rc;
     if (!e->committed) return fail(e, PE_ERR_STATE, "pe_commit_weights has not been called");
     CK(e, cudaSetDevice(e->cfg.device));
-    const int nimg = n * e->cfg.num_scales;
+    const int nimg = n * copies(e);
     const int nops = (int)e->plan.order.size();
     std::vector<cudaEvent_t> evs(nops + 1);
     for (auto& v : evs) CK(e, cudaEventCreate(&v));

@@ -46,21 +46,39 @@ __device__ __forceinline__ float cubic_eval(const CubicTaps& t, float d, double 
 }
 
 struct FullRes {
-    const float* maps;     // this frame: [S][C][h8][w8]
+    const float* maps;     // this frame: [copies][C][h8][w8]
     const AxisTap* xt;     // [S][net_w]
     const AxisTap* yt;     // [S][net_h]
-    int S, C, h8, w8, net_w, net_h;
-    float inv_div;         // (float)S
+    const FlipTap* flip;   // [C]
+    int S, copies, C, h8, w8, net_w, net_h;
+    float inv_div;         // (float)copies
 };
 
-// resized_map[c][y][x] of the reference, evaluated from the stride-8 maps
+// The average's copies: n < S is scale n, n >= S the mirror of scale n - S (the flip test).  A mirrored copy contributes
+// sign[c] * R(M')[perm[c]][y][net_w-1-x]: its own channel and sign, and the scale's x taps read backwards.  Every reader of the
+// full-resolution maps goes through these three, so the average is defined here only.
+__device__ __forceinline__ const float* copy_plane(const FullRes& fr, int n, int c, float* sign) {
+    *sign = 1.f;
+    if (n >= fr.S) {
+        const FlipTap f = fr.flip[c];
+        c = f.ch;
+        *sign = f.sign;
+    }
+    return fr.maps + ((size_t)n * fr.C + c) * fr.h8 * fr.w8;
+}
+__device__ __forceinline__ AxisTap copy_xtap(const FullRes& fr, int n, int x) {
+    return n < fr.S ? fr.xt[n * fr.net_w + x] : fr.xt[(n - fr.S) * fr.net_w + fr.net_w - 1 - x];
+}
+__device__ __forceinline__ const AxisTap* copy_ytab(const FullRes& fr, int n) { return fr.yt + (n < fr.S ? n : n - fr.S) * fr.net_h; }
+
+// resized_map[c][y][x] of the reference, evaluated from the stride-8 maps; with the flip test the average over 2S copies
 __device__ __forceinline__ float fullres_at(const FullRes& fr, int c, int y, int x) {
     float sum = 0.f;
-    const size_t plane = (size_t)fr.h8 * fr.w8;
-    for (int n = 0; n < fr.S; n++) {
-        const AxisTap ax = fr.xt[n * fr.net_w + x];
-        const AxisTap ay = fr.yt[n * fr.net_h + y];
-        const float* s = fr.maps + ((size_t)n * fr.C + c) * plane;
+    for (int n = 0; n < fr.copies; n++) {
+        float sign;
+        const float* s = copy_plane(fr, n, c, &sign);
+        const AxisTap ax = copy_xtap(fr, n, x);
+        const AxisTap ay = copy_ytab(fr, n)[y];
         const float* r0 = s + (size_t)ay.i0 * fr.w8;
         const float* r1 = s + (size_t)ay.i1 * fr.w8;
         const float* r2 = s + (size_t)ay.i2 * fr.w8;
@@ -69,18 +87,18 @@ __device__ __forceinline__ float fullres_at(const FullRes& fr, int c, int y, int
         const float t1 = cubic_ref(__ldg(r1 + ax.i0), __ldg(r1 + ax.i1), __ldg(r1 + ax.i2), __ldg(r1 + ax.i3), ax.d);
         const float t2 = cubic_ref(__ldg(r2 + ax.i0), __ldg(r2 + ax.i1), __ldg(r2 + ax.i2), __ldg(r2 + ax.i3), ax.d);
         const float t3 = cubic_ref(__ldg(r3 + ax.i0), __ldg(r3 + ax.i1), __ldg(r3 + ax.i2), __ldg(r3 + ax.i3), ax.d);
-        sum = __fadd_rn(sum, cubic_ref(t0, t1, t2, t3, ay.d));
+        sum = __fadd_rn(sum, __fmul_rn(sign, cubic_ref(t0, t1, t2, t3, ay.d)));   // sign is +-1: exact
     }
     return __fdiv_rn(sum, fr.inv_div);
 }
 
 __device__ __forceinline__ FullRes make_fullres(const PostDev& pd, int frame) {
     FullRes fr;
-    fr.S = pd.p.num_scales; fr.C = pd.p.num_maps; fr.h8 = pd.p.h8; fr.w8 = pd.p.w8;
+    fr.S = pd.p.num_scales; fr.copies = pd.copies; fr.C = pd.p.num_maps; fr.h8 = pd.p.h8; fr.w8 = pd.p.w8;
     fr.net_w = pd.p.net_w; fr.net_h = pd.p.net_h;
-    fr.maps = pd.maps + (size_t)frame * fr.S * fr.C * fr.h8 * fr.w8;
-    fr.xt = pd.xtab; fr.yt = pd.ytab;
-    fr.inv_div = (float)fr.S;
+    fr.maps = pd.maps + (size_t)frame * fr.copies * fr.C * fr.h8 * fr.w8;
+    fr.xt = pd.xtab; fr.yt = pd.ytab; fr.flip = pd.flip;
+    fr.inv_div = (float)fr.copies;
     return fr;
 }
 

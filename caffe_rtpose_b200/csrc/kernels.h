@@ -40,11 +40,14 @@ struct AxisTap { int i0, i1, i2, i3; float d; };
 struct Cand { float conn; int p; };
 struct Conn { int a, b; float score; };
 struct ModelDev { int limb_seq[40]; int map_idx[40]; };
+struct FlipTap { int ch; float sign; };   // the flip test: channel c of the average reads channel ch of a mirrored copy, times sign
 
 struct PostDev {
     PostParams p;
     ModelDev md;
-    const float* maps;        // [frames][S][C][h8][w8]
+    const float* maps;        // [frames][copies][C][h8][w8]
+    int copies;               // stride-8 copies per frame: the S scales, then with the flip test the S mirrored ones
+    const FlipTap* flip;      // [C] (model_flip_table)
     const AxisTap* xtab;      // [S][net_w]
     const AxisTap* ytab;      // [S][net_h]
     unsigned* flags;          // [frames][parts][net_h][ceil(net_w/32)]
@@ -85,6 +88,7 @@ struct PreArgs {
     uint8_t* resized;         // [nframes][S][net_h][net_w][3] scratch (only th x tw used)
     AreaTab tab[PE_MAX_SCALES];
     int nframes, S, disp_w, disp_h, net_w, net_h;
+    int flip;                 // the flip test: frame f's scale s goes to image 2Sf + s, its mirror in x to image 2Sf + S + s
     // im2col'ed network input, flat padded level-0 geometry
     void* out; int kp; long long out_plane; PlaneFmt fmt;
     int Wp, Hs;

@@ -5,6 +5,7 @@
 // The plan is not a translation of Caffe's layer list: ReLU is fused into the conv epilogue, Concat is
 // removed (producers write channel slices of a shared buffer), Split disappears, and conv1_1 consumes an
 // im2col'ed input so that it is a K=27 1x1 GEMM.
+#include <ctype.h>
 #include <math.h>
 #include <stdio.h>
 
@@ -49,6 +50,37 @@ const char* model_part_name(int model, int idx) {
     }
     if (idx < 0 || idx >= t.num_maps) return "";
     return names[mi][idx].c_str();
+}
+
+// The flip test's channel map (DESIGN.md section 8): a part maps to its left/right twin by name ("RKnee" <-> "LKnee"; the centre
+// parts and the background to themselves), limb (a, b) to the limb (perm a, perm b), and a limb's PAF channels to its mirror's,
+// the x channel negated.  The result is an involution.  Returns num_maps, or -1 when a part or limb has no mirror.
+int model_flip_table(int model, std::vector<int>& perm, std::vector<float>& sign) {
+    const ModelTables& t = model_tables(model);
+    perm.assign(t.num_maps, -1);
+    sign.assign(t.num_maps, 1.f);
+    for (int i = 0; i <= t.num_parts; i++) {
+        const std::string n = model_part_name(model, i);
+        perm[i] = i;
+        if (n.size() < 2 || (n[0] != 'R' && n[0] != 'L') || !isupper((unsigned char)n[1])) continue;
+        const std::string twin = (n[0] == 'R' ? "L" : "R") + n.substr(1);
+        perm[i] = -1;
+        for (int j = 0; j <= t.num_parts; j++)
+            if (twin == model_part_name(model, j)) perm[i] = j;
+        if (perm[i] < 0) return -1;
+    }
+    for (int k = 0; k < t.num_limbs; k++) {
+        int m = -1;
+        for (int j = 0; j < t.num_limbs; j++)
+            if (t.limb_seq[2 * j] == perm[t.limb_seq[2 * k]] && t.limb_seq[2 * j + 1] == perm[t.limb_seq[2 * k + 1]]) m = j;
+        if (m < 0) return -1;
+        perm[t.map_idx[2 * k]] = t.map_idx[2 * m];
+        perm[t.map_idx[2 * k + 1]] = t.map_idx[2 * m + 1];
+        sign[t.map_idx[2 * k]] = -1.f;   // x points the other way in the mirror (rtpose.cpp:575-576 reads mapIdx[2k] as x)
+    }
+    for (int c = 0; c < t.num_maps; c++)
+        if (perm[c] < 0 || perm[perm[c]] != c) return -1;
+    return t.num_maps;
 }
 
 static int round_up(int v, int m) { return (v + m - 1) / m * m; }

@@ -90,25 +90,26 @@ __global__ void __launch_bounds__(NMS_THREADS) nms_flags_kernel(PostDev pd) {
     // so it is computed once per tile (<= NMS_HROWS source rows) instead of 4x per output pixel.  Same
     // operations on the same operands as fullres_at -> bit-identical values.
     bool separable = true;
-    for (int n = 0; n < fr.S; n++) {
-        const int rlo = fr.yt[n * H + ylo].i0, rhi = fr.yt[n * H + yhi].i3;
+    for (int n = 0; n < fr.copies; n++) {
+        const int rlo = copy_ytab(fr, n)[ylo].i0, rhi = copy_ytab(fr, n)[yhi].i3;
         if (rhi - rlo + 1 > NMS_HROWS) separable = false;
     }
     if (separable) {
         float acc[NMS_SEG];
 #pragma unroll
         for (int j = 0; j < NMS_SEG; j++) acc[j] = 0.f;
-        const size_t plane = (size_t)fr.h8 * fr.w8;
-        for (int n = 0; n < fr.S; n++) {
-            const int rlo = fr.yt[n * H + ylo].i0, rhi = fr.yt[n * H + yhi].i3;
+        for (int n = 0; n < fr.copies; n++) {
+            const AxisTap* yt = copy_ytab(fr, n);
+            const int rlo = yt[ylo].i0, rhi = yt[yhi].i3;
             const int nrows = rhi - rlo + 1;
-            const float* s = fr.maps + ((size_t)n * fr.C + part) * plane;
+            float sign;
+            const float* s = copy_plane(fr, n, part, &sign);
             __syncthreads();                                   // the previous scale's tables and rows have been consumed
             for (int i = threadIdx.x; i < NMS_ROWS; i += NMS_THREADS) {
                 const int y = y0 + i;
                 uint32_t pk = 0xffffffffu;                     // row outside the image
                 if (y >= 0 && y < H) {
-                    const AxisTap ay = fr.yt[n * H + y];
+                    const AxisTap ay = yt[y];
                     pk = (uint32_t)(ay.i0 - rlo) | (uint32_t)(ay.i1 - rlo) << 8 | (uint32_t)(ay.i2 - rlo) << 16 | (uint32_t)(ay.i3 - rlo) << 24;
                     s_yd[i] = ay.d;
                     s_ydd[i] = (double)ay.d;
@@ -127,7 +128,7 @@ __global__ void __launch_bounds__(NMS_THREADS) nms_flags_kernel(PostDev pd) {
                     if (tx < NMS_COLS) {
                         float v = 0.f;
                         if (x >= 0 && x < W) {
-                            const AxisTap ax = fr.xt[n * W + x];
+                            const AxisTap ax = copy_xtap(fr, n, x);
                             if (ax.i0 != p0 || ax.i1 != p1 || ax.i2 != p2 || ax.i3 != p3) {
                                 p0 = ax.i0; p1 = ax.i1; p2 = ax.i2; p3 = ax.i3;
                                 ct = cubic_prep(__ldg(row + p0), __ldg(row + p1), __ldg(row + p2), __ldg(row + p3));
@@ -153,7 +154,7 @@ __global__ void __launch_bounds__(NMS_THREADS) nms_flags_kernel(PostDev pd) {
                                 cur = pk;
                                 ct = cubic_prep(hrow[pk & 255u][ctx], hrow[(pk >> 8) & 255u][ctx], hrow[(pk >> 16) & 255u][ctx], hrow[pk >> 24][ctx]);
                             }
-                            acc[j] = __fadd_rn(acc[j], cubic_eval(ct, s_yd[ty], s_ydd[ty]));
+                            acc[j] = __fadd_rn(acc[j], __fmul_rn(sign, cubic_eval(ct, s_yd[ty], s_ydd[ty])));
                         }
                     }
                 }
@@ -163,7 +164,7 @@ __global__ void __launch_bounds__(NMS_THREADS) nms_flags_kernel(PostDev pd) {
 #pragma unroll
             for (int j = 0; j < NMS_SEG; j++) {
                 const int ty = cseg * NMS_SEG + j;
-                if (ty < NMS_ROWS) tile[ty][ctx] = fr.S == 1 ? acc[j] : __fdiv_rn(acc[j], fr.inv_div);   // x / 1.0f == x; outside the image: 0
+                if (ty < NMS_ROWS) tile[ty][ctx] = fr.copies == 1 ? acc[j] : __fdiv_rn(acc[j], fr.inv_div);   // x / 1.0f == x; outside the image: 0
             }
         }
     } else {

@@ -117,6 +117,12 @@ int launch_warp_affine(const WarpArgs& a, int nframes, cudaStream_t st) {
     return 1;
 }
 
+// The flip test (PreArgs::flip): every im2col kernel also writes the copy of its image mirrored in x over the whole net width, in the
+// same pass.  Mirrored pixel net_w-1-x holds the patch of pixel x with the taps of each row reversed: patch channel k = (r*3+s)*3+c
+// of the mirror is channel mirror_k(k) = (r*3+2-s)*3+c of the original.  Frame f's copies are [S originals][S mirrored].
+__device__ __forceinline__ int out_image(const PreArgs& a, int n) { return a.flip ? n + (n / a.S) * a.S : n; }   // source image n = S*f + s
+__host__ __device__ constexpr int mirror_k(int k) { return k < 27 ? (k / 9 * 3 + 2 - k / 3 % 3) * 3 + k % 3 : k; }
+
 // S8X1: one s8 plane of 128 channels per pixel, the 27 patch values at scale 2^8 - p - 128 from the uint8 path (exact), and
 // sat(rint(x * 256)) from a planar fp32 input - in the first 32 bytes (channels 27..31 written as 0); the rest stays zero from
 // init.  SRC as in input_im2col_kernel.  One thread = one pixel.
@@ -129,7 +135,7 @@ __global__ void __launch_bounds__(256) input_im2col_s8_kernel(PreArgs a, const f
     const int y = (int)(idx / (unsigned)a.net_w), x = (int)(idx % (unsigned)a.net_w);
     const AreaTab& t = a.tab[SRC == 0 ? n % a.S : 0];
     const uint8_t* img = a.resized + (size_t)n * a.net_h * a.net_w * 3;
-    uint32_t pk[8] = {};
+    int8_t qs[27];
 #pragma unroll
     for (int k = 0; k < 27; k++) {
         const int tap = k / 3, c = k % 3;
@@ -144,12 +150,20 @@ __global__ void __launch_bounds__(256) input_im2col_s8_kernel(PreArgs a, const f
                                                -128.f), 127.f));
             }
         }
-        pk[k / 4] |= ((uint32_t)q & 0xffu) << (8 * (k % 4));
+        qs[k] = (int8_t)q;
     }
-    const long long m = ((long long)n * a.Hs + y) * a.Wp + x;
-    uint4* o = (uint4*)((int8_t*)a.out + (size_t)m * a.kp);
-    o[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-    o[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
+    auto store = [&](int img_out, int px, bool mirrored) {
+        uint32_t pk[8] = {};
+#pragma unroll
+        for (int k = 0; k < 27; k++) pk[k / 4] |= ((uint32_t)qs[mirrored ? mirror_k(k) : k] & 0xffu) << (8 * (k % 4));
+        const long long m = ((long long)img_out * a.Hs + y) * a.Wp + px;
+        uint4* o = (uint4*)((int8_t*)a.out + (size_t)m * a.kp);
+        o[0] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+        o[1] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
+    };
+    const int no = out_image(a, n);
+    store(no, x, false);
+    if (a.flip) store(no + a.S, a.net_w - 1 - x, true);
 }
 static void launch_im2col_s8(const PreArgs& a, const float* planar, int nimages, cudaStream_t st) {
     const unsigned per = (unsigned)a.net_h * a.net_w;
@@ -164,48 +178,12 @@ template <bool F16> __device__ __forceinline__ void split3(float x, uint16_t& h,
     l = float_to_plane<F16>(__fsub_rn(r, plane_to_float<F16>(m)));
 }
 
-// SRC = 0: uint8 resized images (pad + normalise here);  SRC = 1: planar fp32 net input (already padded/normalised)
-// One thread = 8 consecutive patch channels of one pixel (k = 8*part .. 8*part+7, k = (r*3+s)*3 + c), so a row of
-// the im2col'ed input is written with coalesced 16/32-byte vector stores.
-template <int SRC>
-__global__ void __launch_bounds__(256) input_im2col_kernel(PreArgs a, const float* planar, int nimages) {
-    // uint8 pixels normalised by /256-0.5 are exact in bf16 (8 significant bits) and in fp16, so the SRC=0 path fills only the
-    // hi plane and only the 32 channels that can be non-zero (27 used); everything else stays zero from init
-    // (the engine clears the other planes when it switches from the planar-input path, see engine.cu).
-    const int parts = (SRC == 0 && a.fmt.planes > 0) ? 4 : a.kp / 8;
-    // grid.y = image; 32-bit index math inside an image (64-bit divisions cost hundreds of cycles on the GPU)
-    const int n = blockIdx.y;
-    const unsigned per_img = (unsigned)a.Hs * (unsigned)a.Wp;
-    const unsigned idx = blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= per_img * (unsigned)parts) return;
-    const int part = (int)(idx % (unsigned)parts);
-    const unsigned rem = idx / (unsigned)parts;
-    const int y = (int)(rem / (unsigned)a.Wp), x = (int)(rem % (unsigned)a.Wp);
-    const long long m = (long long)n * per_img + rem;
-    if (x >= a.net_w || y >= a.net_h) return;  // gap rows stay zero
-    const int s = n % a.S;
-    const AreaTab& t = a.tab[SRC == 0 ? s : 0];
-    const uint8_t* img = a.resized + (size_t)n * a.net_h * a.net_w * 3;
+// Row m, channels 8*part .. 8*part+7 of the im2col'ed input from patch(k), or with `mirrored` from patch(mirror_k(k))
+template <int SRC, class Patch>
+__device__ __forceinline__ void input_im2col_store(const PreArgs& a, long long m, int part, const Patch& patch, int mirrored) {
     float v[8];
 #pragma unroll
-    for (int j = 0; j < 8; j++) {
-        const int k = part * 8 + j;
-        float val = 0.f;
-        if (k < 27) {
-            const int tap = k / 3, c = k % 3;
-            const int yy = y + tap / 3 - 1, xx = x + tap % 3 - 1;
-            if (yy >= 0 && yy < a.net_h && xx >= 0 && xx < a.net_w) {
-                if (SRC == 0) {
-                    const int oy = yy - t.padh, ox = xx - t.padw;
-                    if (oy >= 0 && oy < t.th && ox >= 0 && ox < t.tw)
-                        val = __fsub_rn(__fmul_rn((float)img[((size_t)oy * t.tw + ox) * 3 + c], 0.00390625f), 0.5f);   // x/256 == x*2^-8 exactly
-                } else {
-                    val = planar[((size_t)n * 3 + c) * a.net_h * a.net_w + (size_t)yy * a.net_w + xx];
-                }
-            }
-        }
-        v[j] = val;
-    }
+    for (int j = 0; j < 8; j++) v[j] = patch(mirrored ? mirror_k(part * 8 + j) : part * 8 + j);
     if (a.fmt.planes == 0) {
         float4* o = (float4*)((float*)a.out + (size_t)m * a.kp + part * 8);
         o[0] = make_float4(v[0], v[1], v[2], v[3]);
@@ -226,6 +204,49 @@ __global__ void __launch_bounds__(256) input_im2col_kernel(PreArgs a, const floa
         for (int p = 0; p < np; p++)
             *(uint4*)(o0 + (size_t)p * a.out_plane) = make_uint4(pk[p][0], pk[p][1], pk[p][2], pk[p][3]);
     }
+}
+
+// SRC = 0: uint8 resized images (pad + normalise here);  SRC = 1: planar fp32 net input (already padded/normalised)
+// One thread = 8 consecutive patch channels of one pixel (k = 8*part .. 8*part+7, k = (r*3+s)*3 + c), so a row of
+// the im2col'ed input is written with coalesced 16/32-byte vector stores.
+template <int SRC>
+__global__ void __launch_bounds__(256) input_im2col_kernel(PreArgs a, const float* planar, int nimages) {
+    // uint8 pixels normalised by /256-0.5 are exact in bf16 (8 significant bits) and in fp16, so the SRC=0 path fills only the
+    // hi plane and only the 32 channels that can be non-zero (27 used); everything else stays zero from init
+    // (the engine clears the other planes when it switches from the planar-input path, see engine.cu).
+    const int parts = (SRC == 0 && a.fmt.planes > 0) ? 4 : a.kp / 8;
+    // grid.y = image; 32-bit index math inside an image (64-bit divisions cost hundreds of cycles on the GPU)
+    const int n = blockIdx.y;
+    const unsigned per_img = (unsigned)a.Hs * (unsigned)a.Wp;
+    const unsigned idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= per_img * (unsigned)parts) return;
+    const int part = (int)(idx % (unsigned)parts);
+    const unsigned rem = idx / (unsigned)parts;
+    const int y = (int)(rem / (unsigned)a.Wp), x = (int)(rem % (unsigned)a.Wp);
+    if (x >= a.net_w || y >= a.net_h) return;  // gap rows stay zero
+    const int s = n % a.S;
+    const AreaTab& t = a.tab[SRC == 0 ? s : 0];
+    const uint8_t* img = a.resized + (size_t)n * a.net_h * a.net_w * 3;
+    auto patch = [&](int k) {
+        float val = 0.f;
+        if (k < 27) {
+            const int tap = k / 3, c = k % 3;
+            const int yy = y + tap / 3 - 1, xx = x + tap % 3 - 1;
+            if (yy >= 0 && yy < a.net_h && xx >= 0 && xx < a.net_w) {
+                if (SRC == 0) {
+                    const int oy = yy - t.padh, ox = xx - t.padw;
+                    if (oy >= 0 && oy < t.th && ox >= 0 && ox < t.tw)
+                        val = __fsub_rn(__fmul_rn((float)img[((size_t)oy * t.tw + ox) * 3 + c], 0.00390625f), 0.5f);   // x/256 == x*2^-8 exactly
+                } else {
+                    val = planar[((size_t)n * 3 + c) * a.net_h * a.net_w + (size_t)yy * a.net_w + xx];
+                }
+            }
+        }
+        return val;
+    };
+    const int no = out_image(a, n);
+    input_im2col_store<SRC>(a, ((long long)no * a.Hs + y) * a.Wp + x, part, patch, 0);
+    if (a.flip) input_im2col_store<SRC>(a, ((long long)(no + a.S) * a.Hs + y) * a.Wp + (a.net_w - 1 - x), part, patch, 1);
 }
 
 // Fast path of input_im2col_kernel<0> for the 16-bit plane modes: one thread = one pixel, the 3x3x3 patch comes from a
@@ -256,19 +277,24 @@ __global__ void __launch_bounds__(256) input_im2col_u8_kernel(PreArgs a) {
     __syncthreads();
     const int x = x0 + threadIdx.x, y = y0 + threadIdx.y;
     if (x >= a.net_w || y >= a.net_h) return;
-    uint16_t k[32];
+    auto store = [&](int img_out, int px, bool mirrored) {
+        uint16_t k[32];
 #pragma unroll
-    for (int tap = 0; tap < 9; tap++)
+        for (int tap = 0; tap < 9; tap++)
 #pragma unroll
-        for (int c = 0; c < 3; c++) k[tap * 3 + c] = tile[c][threadIdx.y + tap / 3][threadIdx.x + tap % 3];
+            for (int c = 0; c < 3; c++) k[tap * 3 + c] = tile[c][threadIdx.y + tap / 3][threadIdx.x + (mirrored ? 2 - tap % 3 : tap % 3)];
 #pragma unroll
-    for (int j = 27; j < 32; j++) k[j] = 0;
-    const long long m = ((long long)n * a.Hs + y) * a.Wp + x;
-    uint4* o = (uint4*)((uint16_t*)a.out + (size_t)m * a.kp);
+        for (int j = 27; j < 32; j++) k[j] = 0;
+        const long long m = ((long long)img_out * a.Hs + y) * a.Wp + px;
+        uint4* o = (uint4*)((uint16_t*)a.out + (size_t)m * a.kp);
 #pragma unroll
-    for (int q = 0; q < 4; q++)
-        o[q] = make_uint4((uint32_t)k[q * 8] | ((uint32_t)k[q * 8 + 1] << 16), (uint32_t)k[q * 8 + 2] | ((uint32_t)k[q * 8 + 3] << 16),
-                          (uint32_t)k[q * 8 + 4] | ((uint32_t)k[q * 8 + 5] << 16), (uint32_t)k[q * 8 + 6] | ((uint32_t)k[q * 8 + 7] << 16));
+        for (int q = 0; q < 4; q++)
+            o[q] = make_uint4((uint32_t)k[q * 8] | ((uint32_t)k[q * 8 + 1] << 16), (uint32_t)k[q * 8 + 2] | ((uint32_t)k[q * 8 + 3] << 16),
+                              (uint32_t)k[q * 8 + 4] | ((uint32_t)k[q * 8 + 5] << 16), (uint32_t)k[q * 8 + 6] | ((uint32_t)k[q * 8 + 7] << 16));
+    };
+    const int no = out_image(a, n);
+    store(no, x, false);
+    if (a.flip) store(no + a.S, a.net_w - 1 - x, true);
 }
 
 static int launch_im2col_u8(const PreArgs& a, cudaStream_t st) {

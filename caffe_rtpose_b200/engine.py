@@ -75,7 +75,7 @@ ABI_SYMBOLS = [
     "pe_compare_results", "pe_jpeg_read_coefs", "pe_jpeg_coefs_to_bgr", "pe_forward_jpeg_coefs", "pe_video_read_coefs",
     "pe_jpeg_read_scan", "pe_jpeg_scan_to_coefs_host", "pe_forward_jpeg_scans", "pe_jpeg_decode_scans", "pe_video_read_scan",
     "pe_forward_pixels", "pe_stream_wait", "pe_pixels_to_bgr", "pe_blob_log2_scale", "pe_create_mixed", "pe_plan_formats",
-    "pe_conv_layer_sparse", "pe_prune_2to4",
+    "pe_conv_layer_sparse", "pe_prune_2to4", "pe_set_flip_test", "pe_get_flip_test", "pe_model_flip_table",
 ]
 
 
@@ -149,6 +149,9 @@ def lib():
         getattr(L, f).restype = C.POINTER(C.c_int)
     L.pe_model_part_name.argtypes = [C.c_int, C.c_int]
     L.pe_model_part_name.restype = C.c_char_p
+    L.pe_model_flip_table.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int]
+    L.pe_set_flip_test.argtypes = [C.c_void_p, C.c_int]
+    L.pe_get_flip_test.argtypes = [C.c_void_p]
     L.pe_event_record.argtypes = [C.c_void_p, C.c_int]
     L.pe_event_elapsed_ms.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_float)]
     L.pe_profile_layers.argtypes = [C.c_void_p, C.c_int, _f32p, C.c_char_p, C.c_void_p, C.c_int]
@@ -197,6 +200,18 @@ def lib():
         L.pe_yuyv_to_bgr.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_longlong, C.c_void_p]
     _lib = L
     return L
+
+
+def flip_table(model):
+    """The flip test's channel map of `model` (pe_model_flip_table): (perm int32, sign float32), one entry per map channel.
+    Channel c of the un-flipped maps is sign[c] * channel perm[c] of the mirrored copy, read at net_w-1-x."""
+    L = lib()
+    n = L.pe_model_flip_table(model, None, None, 0)
+    if n < 0:
+        raise PoseEngineError("pe_model_flip_table failed (%d): %s" % (-n, L.pe_last_error(None).decode()))
+    perm, sign = np.zeros(n, np.int32), np.zeros(n, np.float32)
+    L.pe_model_flip_table(model, perm.ctypes.data, sign.ctypes.data, n)
+    return perm, sign
 
 
 class ModelDescriptor:
@@ -292,13 +307,14 @@ class PoseEngine:
 
     def __init__(self, model=COCO_18, net_w=656, net_h=368, disp_w=1280, disp_h=720, num_scales=1, start_scale=1.0,
                  scale_gap=0.3, device=0, max_batch=1, precision=PREC_BF16X2, prototxt=None, f16_layers=None,
-                 u8_activations=False):
+                 u8_activations=False, flip_test=False):
         """prototxt: path of a deploy prototxt (`new caffe::Net(proto, TEST)`, rtpose.cpp:183); model may then be None
         and follows the Nms layer's num_parts (rtpose.cpp:212-229).  Without it the built-in graph of `model` is used.
         f16_layers: conv layer names (a list or a comma-separated string, "narrow" included) that run with PREC_F16X1's
         arithmetic inside a PREC_E4M3X1 or PREC_S8X1 engine (pe_create_mixed); see plan_formats.
         u8_activations: with PREC_S8X1, store the activations that only hold values >= 0 (post-ReLU, read only by integer
-        layers) as u8 and run their readers u8 x s8 (PE_PREC_FLAG_U8); any other precision refuses it."""
+        layers) as u8 and run their readers u8 x s8 (PE_PREC_FLAG_U8); any other precision refuses it.
+        flip_test: average every frame's maps with those of its net input mirrored in x (set_flip_test)."""
         L = lib()
         cfg = _Config(device, -1 if model is None else model, net_w, net_h, disp_w, disp_h, num_scales, start_scale, scale_gap,
                       max_batch, precision | (PREC_FLAG_U8 if u8_activations else 0))
@@ -325,6 +341,8 @@ class PoseEngine:
         self.model_descriptor = ModelDescriptorFactory.createModelDescriptor(model)
         self._keep = None
         self._held = []   # frames forward_pixels reads asynchronously: released by the next fetch, sync or close
+        if flip_test:
+            self.set_flip_test(True)
 
     def close(self):
         if getattr(self, "_h", None):
@@ -388,6 +406,21 @@ class PoseEngine:
                 rc, lib().pe_caffemodel_last_error().decode(), lib().pe_last_error(self._h).decode()))
         if commit:
             self.commit_weights()
+
+    def set_flip_test(self, on):
+        """pe_set_flip_test: with it on, each forward also runs every net input mirrored in x, and NMS, the PAF scores and the
+        renderers read the average of the 2 * num_scales copies, mirrors flipped back (flip_table).  Maps and blobs then hold
+        2 * num_scales images per frame: the scales, then their mirrors as the net produced them.  Drops the last forward's results."""
+        self._ck(lib().pe_set_flip_test(self._h, 1 if on else 0))
+
+    @property
+    def flip_test(self):
+        return lib().pe_get_flip_test(self._h) == 1
+
+    @property
+    def copies(self):
+        """Images per frame in the maps and blobs: num_scales, doubled by the flip test."""
+        return self.cfg.num_scales * (2 if self.flip_test else 1)
 
     def set_connect_params(self, min_subset_cnt, min_subset_score, inter_threshold, inter_min_above):
         self._ck(lib().pe_set_connect_params(self._h, min_subset_cnt, min_subset_score, inter_threshold, inter_min_above))
@@ -490,9 +523,13 @@ class PoseEngine:
         self._ck(lib().pe_forward_net_input(self._h, x, n))
 
     def forward_maps(self, maps8):
+        """maps8: (n * copies, C, net_h/8, net_w/8) stride-8 maps, per frame its scales (and with the flip test their mirrors)."""
         maps8 = np.ascontiguousarray(maps8, np.float32)
-        n = maps8.shape[0] // self.cfg.num_scales
-        assert maps8.shape == (n * self.cfg.num_scales, self.num_maps, self.cfg.net_h // 8, self.cfg.net_w // 8), maps8.shape
+        k = self.copies
+        n = maps8.shape[0] // k
+        if n < 1 or maps8.shape != (n * k, self.num_maps, self.cfg.net_h // 8, self.cfg.net_w // 8):
+            raise ValueError("forward_maps: maps of shape %s are not n x %d x %d x %d x %d" % (
+                maps8.shape, k, self.num_maps, self.cfg.net_h // 8, self.cfg.net_w // 8))
         self._ck(lib().pe_forward_maps(self._h, maps8, n))
 
     def calibrate(self, frames):
@@ -569,7 +606,7 @@ class PoseEngine:
         return n.value, joints[:n.value].copy(), peaks
 
     def fetch_maps(self, n=1):
-        out = np.zeros((n * self.cfg.num_scales, self.num_maps, self.cfg.net_h // 8, self.cfg.net_w // 8), np.float32)
+        out = np.zeros((n * self.copies, self.num_maps, self.cfg.net_h // 8, self.cfg.net_w // 8), np.float32)
         self._ck(lib().pe_fetch_maps(self._h, out, n))
         return out
 
@@ -577,7 +614,7 @@ class PoseEngine:
         c, h, w = C.c_int(), C.c_int(), C.c_int()
         self._ck(lib().pe_fetch_blob(self._h, name.encode(), None, 0, C.byref(c), C.byref(h), C.byref(w)))
         # number of images of the last forward is not exported; over-allocate for max_batch
-        n = self.cfg.max_batch * self.cfg.num_scales
+        n = self.cfg.max_batch * self.copies
         out = np.zeros((n, c.value, h.value, w.value), np.float32)
         self._ck(lib().pe_fetch_blob(self._h, name.encode(), out.ctypes.data_as(C.c_void_p), out.size, C.byref(c),
                                      C.byref(h), C.byref(w)))

@@ -106,6 +106,8 @@ static void define_flags() {
            "fill two waves of 128-row tiles on the GPU, e.g. 9 frames at 656x368; results do not depend on it)");
     define("engines_per_gpu", "0", "[extension] worker handles per GPU: 1 = the reference's topology (one Net per GPU), 0 = automatic (2 when "
            "--batch is automatic: the copies and the kernel tails of one batch overlap the other; weights are shared, not duplicated)");
+    define("flip_test", "false", "[extension] average every frame's maps with those of its net input mirrored in x, left/right parts and "
+           "limbs swapped (pe_set_flip_test): the conv stack runs twice the images, for every source and --precision", true);
     define("calibrate_range", "true", "[extension] fp16, e4m3 and s8 modes (--precision 2, 4, 5 and 6): derive per-layer power-of-two activation scales from one synthetic frame at start-up "
            "(pe_calibrate), so that a model of any magnitude keeps fp32-level results; --precision 6 cannot run without them", true);
     define("calibration_dir", "", "[extension] --precision 2, 4, 5 or 6: after the synthetic-frame calibration of --calibrate_range, calibrate GPU 0's "
@@ -776,6 +778,7 @@ static bool create_engines(int num_gpu, int per_gpu, int precision, const std::s
                        : global.proto_readable ? pe_create_from_prototxt(&c, proto.c_str(), &e) : pe_create(&c, &e);
         if (rc) { LOG_ERROR("GPU %d: %s", c.device, pe_last_error(nullptr)); return false; }
         engines.push_back(e);
+        if (Fb("flip_test") && pe_set_flip_test(e, 1)) { LOG_ERROR("GPU %d: --flip_test: %s", c.device, pe_last_error(e)); return false; }
     }
     if (load_weights(engines[0], Fi("start_device"))) return false;
     if ((precision & ~PE_PREC_FLAG_U8) == PE_PREC_S8X1) {   // layers the 2:4-sparse s8 kernel runs (pe_conv_layer_sparse's rules)
@@ -891,8 +894,8 @@ static void worker(int tid, pe_engine* e, pe_engine* ref) {
     caffe::ImResizeLayer<float> resize_layer(e);
     resize_layer.SetStartScale((float)Fd("start_scale"));
     resize_layer.SetScaleGap((float)Fd("scale_gap"));
-    LOG_INFO("GPU %d is ready (model %s, max_peaks %d, %d frame(s) per forward)", device, nms_layer.GetNumParts() == 15 ? "MPI" : "COCO",
-             nms_layer.GetMaxPeaks(), batch);
+    LOG_INFO("GPU %d is ready (model %s, max_peaks %d, %d frame(s) per forward%s)", device, nms_layer.GetNumParts() == 15 ? "MPI" : "COCO",
+             nms_layer.GetMaxPeaks(), batch, pe_get_flip_test(e) ? ", flip test on" : "");
     const int P = nms_layer.GetNumParts();
     std::vector<float> joints((size_t)PE_MAX_PEOPLE * P * 3), peaks((size_t)P * (nms_layer.GetMaxPeaks() + 1) * 3);
     const int audit_every = ref ? Fi("audit_every") : 0;

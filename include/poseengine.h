@@ -224,6 +224,21 @@ float pe_resize_get_scale_gap(const pe_engine* e);
 /* ---- global.connect_* thresholds                                           rtpose.cpp:106-111, 212-226 */
 int pe_set_connect_params(pe_engine* e, int min_subset_cnt, float min_subset_score, float inter_threshold,
                           int inter_min_above_threshold);
+/* ---- the flip test (off by default; the reference has none).  With it on, every forward also runs each frame's net input of
+ * every scale mirrored in x over the whole net width, and the full-resolution maps that NMS, the PAF scores and the renderers read
+ * become the average of 2 x num_scales copies: the S scales, then the S mirrors, each mirror resized as its scale, read at
+ * net_w-1-x, with left/right parts and limbs swapped and the x channels of the PAFs negated (pe_model_flip_table), divided by 2S.
+ * While it is on:
+ *   - pe_forward_maps takes and pe_fetch_maps returns n x 2S x C x net_h/8 x net_w/8 maps, per frame the S scales then the S
+ *     mirrored copies as the net produced them (not flipped back); pe_fetch_blob returns 2 x n x S images in the same order;
+ *   - pe_forward_net_input still takes n x S planar images: the engine mirrors them;
+ *   - calibration (pe_calibrate, pe_calibrate_begin / _end) counts the mirrored copies' ranges like any other image; calibration
+ *     tables do not depend on it, and pe_share_weights / pe_broadcast_weights work between handles with and without it.
+ * pe_set_flip_test is valid between forwards and drops the results of the last one.  Turning it on the first time grows the
+ * handle's per-image buffers to 2 x max_batch x num_scales images (max_batch stays the number of frames per forward); when that
+ * allocation fails it returns PE_ERR_CUDA and the engine is unchanged.  PE_ERR_STATE during a calibration collection. */
+int pe_set_flip_test(pe_engine* e, int on);
+int pe_get_flip_test(const pe_engine* e);   /* 1 when on */
 
 /* ---- per-frame hot loop (processFrame, rtpose.cpp:1099-1203).  All forwards are asynchronous on the
  * engine's stream; pe_fetch* synchronises.  n <= max_batch frames per call.
@@ -309,7 +324,7 @@ int pe_pixels_to_bgr(const pe_pixel_format* fmt, const void* frame, uint8_t* bgr
 int pe_forward_net_input(pe_engine* e, const float* net_input, int n);
 /* (PE_PREC_S8X1 quantises this input like any activation, at scale 2^8: q = sat(rint(x * 256)) in [-128, 127], so values that
  * are not multiples of 1/256 inside [-0.5, 0.496] - the frame path's p/256 - 0.5 - are rounded or saturated.) */
-/* test hook at the concat_stage7 boundary: HOST stride-8 maps n x num_scales x C x net_h/8 x net_w/8;
+/* test hook at the concat_stage7 boundary: HOST stride-8 maps n x num_scales x C x net_h/8 x net_w/8 (flip test: n x 2S x ...);
  * runs resize + NMS + connectLimbs* only (SURVEY.md section 8d "map injection") */
 int pe_forward_maps(pe_engine* e, const float* maps8, int n);
 
@@ -317,7 +332,7 @@ int pe_forward_maps(pe_engine* e, const float* maps8, int n);
  * score) as connectLimbs* fills it (rtpose.cpp:1051-1073); peaks (optional): the NMS top blob
  * num_parts x (max_peaks+1) x 3 (nms_layer.cpp:17-29), count in [part][0][0]. */
 int pe_fetch(pe_engine* e, int idx, float* joints, int* num_people, float* peaks);
-/* stride-8 net output of the last forward, n x num_scales x C x net_h/8 x net_w/8 (blob "concat_stage7") */
+/* stride-8 net output of the last forward, n x num_scales x C x net_h/8 x net_w/8 (blob "concat_stage7"; flip test: n x 2S x ...) */
 int pe_fetch_maps(pe_engine* e, float* maps8, int n);
 /* debugging / layer-wise parity: NCHW fp32 copy of an intermediate blob by its prototxt top name, in true values (the range
  * scale of pe_calibrate is divided out).  The stage outputs of the concat buffers that a later stage reuses (for the 6-stage
@@ -496,6 +511,11 @@ int pe_model_num_limbs(int model);
 const int* pe_model_limb_sequence(int model);
 const int* pe_model_map_idx(int model);
 const char* pe_model_part_name(int model, int idx);
+/* the flip test's channel map of `model` (host only): channel c of the un-flipped maps is sign[c] x channel perm[c] of the mirrored
+ * copy, read at net_w-1-x.  Parts swap with their left/right twins by pe_model_part_name, limb (a, b) with limb (perm a, perm b),
+ * the x channel of a limb's PAF pair (pe_model_map_idx[2k]) carries -1, everything else +1; perm is an involution.  Writes perm and
+ * sign (either may be NULL) when cap >= the channel count, and returns that count (num_maps), or -PE_ERR_INVALID for an unknown model. */
+int pe_model_flip_table(int model, int* perm, float* sign, int cap);
 
 /* ---- measurement support (bench.py) */
 /* device time, CUDA events on the engine stream: slot in [0,16) */
