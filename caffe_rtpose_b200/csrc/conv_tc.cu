@@ -87,7 +87,10 @@ int tc_layer_create(const TcLayerDesc& d, TcLayer& out, std::string& err) {
     if (!enc) { err = "cuTensorMapEncodeTiled unavailable"; return -1; }
     const int kb = tc_block_ch(d.fmt.elem), eb = d.fmt.elem_bytes();
     if (d.in_cused % kb) { err = "input channels not a multiple of " + std::to_string(kb); return -1; }
-    if (d.fmt.planes < 1 || d.fmt.planes > 3 || ((d.fmt.e4m3() || d.fmt.s8() || d.fmt.u8()) && d.fmt.planes != 1)) { err = "1 to 3 planes (e4m3, s8, u8: 1)"; return -1; }
+    if (d.fmt.planes < 1 || d.fmt.planes > 3 || ((d.fmt.e4m3() || d.fmt.u8()) && d.fmt.planes != 1) || (d.fmt.s8() && d.fmt.planes > 2)) {
+        err = "1 to 3 planes (e4m3, u8: 1; s8: 1 or 2)";
+        return -1;
+    }
     if (d.ksize < 1 || d.ksize > TC_KMAX) { err = "filter size above " + std::to_string(TC_KMAX) + " (A window rows)"; return -1; }
     out.d = d;
     out.bn = tc_bn(d.cout_pad, d.fmt.planes);
@@ -164,6 +167,7 @@ int tc_layer_launch(const TcLayer& l, int nimg, cudaStream_t st, int share) {
     const long long tiles = ((long long)nimg * a.tiles_img + TC_CLUSTER - 1) / TC_CLUSTER * TC_CLUSTER;
     const dim3 grid((unsigned)tiles, (unsigned)(d.cout_pad / bn), 1);
     const PlaneFmt f = d.fmt;
+    if (f.s8() && f.planes == 2) return launch_s8x2(l, a, grid, st, bmap, bn);            // conv_s8x2.cu
     if (f.u8() || d.out_elem == ELEM_U8) return launch_u8(l, a, grid, st, bmap, bn);   // conv_u8.cu
     if (f.elem != d.out_elem && d.out_elem != ELEM_E4M3) return launch_mixed(l, a, grid, st, bmap, bn);   // conv_mixed.cu
     if (d.out_elem == ELEM_E4M3) return launch_e4m3(l, a, grid, st, bmap, bn);   // conv_fp8.cu

@@ -1,5 +1,6 @@
 // Kernel side of the wgmma / TMA implicit-GEMM convolution (see conv_tc.cu for the design): argument block, PTX
-// wrappers, conv_wg_kernel and its launcher.  Shared by conv_tc.cu (16-bit planes), conv_fp8.cu (e4m3) and conv_s8.cu (s8).
+// wrappers, conv_wg_kernel and its launcher.  Shared by conv_tc.cu (16-bit planes), conv_fp8.cu (e4m3), conv_s8.cu (s8) and
+// conv_s8x2.cu (two s8 planes).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp8.h>
@@ -243,7 +244,9 @@ template <int BN, int PLANES> struct TcShape {
 // ELEM: element kind of the A windows and weight tiles; OUT: of the stored output planes (conv1_1 of the e4m3 mode reads
 // its fp16 im2col input and writes e4m3).  ELEM = OUT = s8: s32 accumulators over the whole K (the host sets chunk_iters to
 // it), and the per-channel epilogue t = acc * f_c + b'_c (no FMA) before cvt.rni.sat.s8.  ELEM = u8 (PE_PREC_FLAG_U8): the same
-// with u8 x s8 MMAs; OUT = u8: ReLU, then cvt.rni.sat.u8.
+// with u8 x s8 MMAs; OUT = u8: ReLU, then cvt.rni.sat.u8.  PLANES = 2, ELEM = OUT = s8 (PE_PREC_S8X2): hi*hi into acc_h and
+// hi*lo + lo*hi into acc_c, both s32 over the whole K; the epilogue takes S = 256 acc_h + acc_c in 64 bits (exact), t = float(S) *
+// f_c + b'_c, and stores v = sat(rint(t)) in [-32768, 32639] as the planes hi = (v + 128) >> 8, lo = v - 256 hi (s8.h).
 template <int BN, int PLANES, int ELEM, int OUT>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcArgs a) {
@@ -324,8 +327,8 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     // ===== consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile =====
     const int wg = (warp >> 2) - 1;
     using Acc = std::conditional_t<S8, int, float>;
-    Acc acc_h[NACC];
-    float sum_h[NACC], acc_c[NACC];
+    Acc acc_h[NACC], acc_c[NACC];   // acc_c: the cross products of two planes
+    float sum_h[NACC];
 #pragma unroll
     for (int j = 0; j < NACC; j++) { acc_h[j] = 0.f; sum_h[j] = 0.f; acc_c[j] = 0.f; }
     const int cs = a.chunk_iters;
@@ -398,7 +401,10 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
             for (int e = 0; e < 2; e++) {
                 float t;
-                if constexpr (S8) {
+                if constexpr (S8 && PLANES == 2) {
+                    const long long sum = 256LL * acc_h[j + e] + acc_c[j + e];
+                    t = __fadd_rn(__fmul_rn(__ll2float_rn(sum), s_bias[BN + c + e]), s_bias[c + e]);
+                } else if constexpr (S8) {
                     t = __fadd_rn(__fmul_rn(__int2float_rn(acc_h[j + e]), s_bias[BN + c + e]), s_bias[c + e]);
                 } else {
                     t = PLANES > 1 ? __fadd_rn(sum_h[j + e], acc_c[j + e]) : sum_h[j + e];
@@ -412,6 +418,20 @@ conv_wg_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
                 for (int e = 0; e < 2; e++)
                     if (co + e < a.cout) a.planar[(((size_t)n * a.planar_C + a.planar_coff + co + e) * a.H + y) * a.W + x] = v[e];
+            } else if constexpr (OUT == ELEM_S8 && PLANES == 2) {
+                if (co < cout8) {
+                    uint32_t hi = 0, lo = 0;
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        const int q = min(max(__float2int_rn(v[e]), -32768), 32639);   // rint, saturated (NaN gives 0)
+                        const int h = (q + 128) >> 8;
+                        hi |= ((uint32_t)h & 0xffu) << (8 * e);
+                        lo |= ((uint32_t)(q - 256 * h) & 0xffu) << (8 * e);
+                    }
+                    int8_t* o = (int8_t*)a.out + (size_t)m * a.out_pitch + a.out_coff + co;
+                    *(uint16_t*)o = (uint16_t)hi;
+                    *(uint16_t*)(o + a.out_plane) = (uint16_t)lo;
+                }
             } else if constexpr (OUT == ELEM_S8) {
                 if (co < cout8)
                     *(uint16_t*)((int8_t*)a.out + (size_t)m * a.out_pitch + a.out_coff + co) = (uint16_t)(f32_to_s8(v[0]) | f32_to_s8(v[1]) << 8);
@@ -471,12 +491,13 @@ static int launch_widths(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStrea
     }
 }
 
-// Layers with e4m3 output (conv_fp8.cu), s8 layers (conv_s8.cu), the format boundaries of mixed engines (conv_mixed.cu) and
-// the layers that read or store u8 (conv_u8.cu):
+// Layers with e4m3 output (conv_fp8.cu), s8 layers (conv_s8.cu), the format boundaries of mixed engines (conv_mixed.cu), the
+// layers that read or store u8 (conv_u8.cu) and the two-plane s8 layers (conv_s8x2.cu):
 // their instances live in translation units of their own.
 int launch_e4m3(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap, int bn);
 int launch_s8(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap, int bn);
 int launch_mixed(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap, int bn);
 int launch_u8(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap, int bn);
+int launch_s8x2(const TcLayer& l, const TcArgs& a, dim3 grid, cudaStream_t st, int bmap, int bn);
 
 }  // namespace pe

@@ -60,7 +60,7 @@ struct pe_engine {
     // range management of the fp16 and e4m3 modes (F16X2, F16X1, E4M3X1): per-conv-output power-of-two scale s (stored value = true value * s), the
     // weight-scale inverses the packed epilogue fields derive from (with the true biases hw[i].b), and the kernels' running max |stored value| per conv
     std::vector<float> conv_scale, wsi;   // per conv: scale of its stored output; inverse of the power of two folded into its weights
-    std::vector<std::vector<float>> wsig;   // S8X1: per conv, the per-output-channel weight step sigma_c of pack_conv_weights (s8.h)
+    std::vector<std::vector<float>> wsig;   // S8X1, S8X2: per conv, the per-output-channel weight step sigma_c of pack_conv_weights (s8.h)
     DeviceBuffer d_range;
     bool calibrated = false, check_range = false;
     // pe_calibrate_begin .. _end: per conv, the largest true |output| (recorded / conv_scale) over the forwards since begin
@@ -365,6 +365,7 @@ extern "C" int pe_plan_describe(int model, const char* prototxt_path, char* buf,
 
 static const char* elem_name(PlaneFmt f) {
     static const char* names[] = {"bf16", "f16", "e4m3", "s8", "u8"};
+    if (f.s8() && f.planes == 2) return "s8x2";   // PE_PREC_S8X2's 16-bit integers
     return f.planes == 0 ? "f32" : names[f.elem];
 }
 
@@ -373,7 +374,7 @@ static const char* elem_name(PlaneFmt f) {
 static int split_precision(int p, int* mode, bool* u8) {
     *mode = p & ~PE_PREC_FLAG_U8;
     *u8 = (p & PE_PREC_FLAG_U8) != 0;
-    if (*mode < 0 || *mode >= NUM_PRECISIONS) return fail(nullptr, PE_ERR_INVALID, "unknown precision %d", p);
+    if (!known_mode(*mode)) return fail(nullptr, PE_ERR_INVALID, "unknown precision %d", p);
     if (*u8 && *mode != PE_PREC_S8X1)
         return fail(nullptr, PE_ERR_INVALID, "PE_PREC_FLAG_U8 (u8 activations) applies to PE_PREC_S8X1 (6) only, not to precision %d: u8 "
                     "activations are read by the integer MMA (u8 x s8)", *mode);
@@ -531,14 +532,15 @@ static int create_impl(const pe_config* cfg_in, const char* prototxt_path, const
 
     // the plan first: each level's gap is the largest pad of its convolutions (common.h)
     e->plan = plan;
-    for (const ConvSpec& c : e->plan.convs)   // the s32 bound of the layers that compute in s8 or u8
+    for (const ConvSpec& c : e->plan.convs)   // the s32 bound of the layers that compute in s8, u8 or two s8 planes
         if (const long long max_k = elem_row(prec, (PlaneElem)c.elem).max_k) {
             const long long K = (long long)(c.im2col_input ? 1 : c.k * c.k) * c.in_cused;
-            const bool cu8 = c.elem == ELEM_U8;
+            const bool cu8 = c.elem == ELEM_U8, x2 = prec.fmt.planes == 2;
             if (K > max_k) {
                 fail(e, PE_ERR_INVALID, "layer %s: K = %lld (%dx%d taps x %d padded input channels) exceeds %lld, the largest K whose %s sums "
-                     "stay inside s32 (|acc| <= %s x 127 x K): PE_PREC_S8X1%s cannot run it", c.name.c_str(), K, c.k, c.k, c.in_cused, max_k,
-                     cu8 ? "u8 x s8" : "s8", cu8 ? "255" : "128", cu8 ? " with u8 activations" : "");
+                     "stay inside s32 (|acc| <= %s x K): %s cannot run it", c.name.c_str(), K, c.k, c.k, c.in_cused, max_k,
+                     cu8 ? "u8 x s8" : x2 ? "hi x lo + lo x hi" : "s8", cu8 ? "255 x 127" : x2 ? "(128 x 128 + 128 x 127)" : "128 x 127",
+                     cu8 ? "PE_PREC_S8X1 with u8 activations" : x2 ? "PE_PREC_S8X2" : "PE_PREC_S8X1");
                 return bail(PE_ERR_INVALID);
             }
         }
@@ -733,7 +735,7 @@ static size_t packed_layout(pe_engine* e) {
 // next to the previous stage's L1 / L2 outputs) folds the ratios into its weights: packed w[ci] = w[ci] * s_ref / s(ci) * 2^k, so that
 //   acc = 2^k * s_ref * sum_ci w[ci] * a[ci]     and     stored = acc * out_scale + bias,  out_scale = s_out / (2^k * s_ref),
 // bias = true bias * s_out - all factors powers of two, hence exact, and ReLU commutes with them: range scaling is free at run time.
-// S8X1 replaces 2^k by a step per output channel (sigma_c, s8.h): acc * sigma_c ~ s_ref * sum w a, and the factor of channel c
+// S8X1 and S8X2 replace 2^k by a step per output channel (sigma_c, s8.h): acc * sigma_c ~ s_ref * sum w a, and the factor of channel c
 // is f_c = sigma_c * s_out / s_ref.  The net input carries the mode's net_input_scale.
 //
 // The one rule that picks those powers of two (range scales and the weights' 2^k): the s that puts a maximum m into
@@ -755,7 +757,9 @@ static void fill_epilogue_fields(const pe_engine* e, int i, float* B) {
     const float s_out = c.out_act >= 0 ? e->conv_scale[i] : 1.f;   // the planar stride-8 maps are true values
     for (int co = 0; co < c.cout; co++) B[co] = e->hw[i].b[co] * s_out;
     if (conv_row(e, i).per_channel_epilogue) {
-        for (int co = 0; co < c.cout; co++) B[e->cout_pad[i] + co] = e->wsig[i][co] * (s_out / s_ref);
+        // S8X2's sum S = 256 acc_h + acc_c counts in units of 2^8 (the place of the dropped lo*lo): f_c carries that 2^8 too
+        const float unit = conv_row(e, i).fmt.planes == 2 ? 256.f : 1.f;
+        for (int co = 0; co < c.cout; co++) B[e->cout_pad[i] + co] = e->wsig[i][co] * (s_out / s_ref) * unit;
         return;
     }
     B[e->cout_pad[i]] = e->wsi[i] * s_out / s_ref;
@@ -764,6 +768,7 @@ static void fill_epilogue_fields(const pe_engine* e, int i, float* B) {
 // Weights of conv i into `dst` (the layer's region of the packed buffer, host copy): fp32 [K][cout_pad] for the SIMT mode, else
 // P 16-bit planes [P][cout_pad][K] (K-major rows: the wgmma B operand) of w * 2^k, the per-channel range ratios folded in.
 // Sets e->wsi[i] = 2^-k.  S8X1: one s8 plane [cout_pad][K], each output channel quantised on its own (s8.h); sets e->wsig[i].
+// S8X2: the same with 16-bit integers in two s8 planes.
 static int pack_conv_weights(pe_engine* e, int i, uint8_t* dst) {
     const ConvSpec& c = e->plan.convs[i];
     const HostWeights& hw = e->hw[i];
@@ -780,7 +785,16 @@ static int pack_conv_weights(pe_engine* e, int i, uint8_t* dst) {
     const PlaneFmt wf = conv_wfmt(e, i);
     memset(dst, 0, weight_bytes(e, i));
     float wscale_inv = 1.f;
-    if (wf.s8() || wf.u8()) {   // a u8 layer's weights are s8 too: its MMA is u8 x s8
+    if (wf.s8() && wf.planes == 2) {   // PE_PREC_S8X2: planes [hi, lo][cout_pad][K] of each channel's 16-bit integers (s8.h)
+        int8_t* hi = (int8_t*)dst;
+        int8_t* lo = hi + (size_t)cop * K;
+        std::vector<float> wc(K);
+        e->wsig[i].assign(cop, 0.f);
+        for (int co = 0; co < c.cout; co++) {
+            for (size_t kk = 0; kk < K; kk++) wc[kk] = src(co, (int)kk);
+            e->wsig[i][co] = s8x2_quantize_channel(wc.data(), K, hi + (size_t)co * K, lo + (size_t)co * K);
+        }
+    } else if (wf.s8() || wf.u8()) {   // a u8 layer's weights are s8 too: its MMA is u8 x s8
         // a sparse layer quantises into a dense plane first and stores it compressed (s8_sparse.h); quantisation only adds zeros
         std::vector<int8_t> dense(e->sparse[i] ? K * cop : 0);
         int8_t* q = e->sparse[i] ? dense.data() : (int8_t*)dst;
@@ -869,10 +883,11 @@ static int bind_packed(pe_engine* e) {
 //      1.2-2.2x the dense kernel's time), and no other shape has been measured, so no class qualifies and every layer runs dense.
 //      pe_test_force_sparse lifts this rule, so that tests and tools/sparse_s8.py can run and measure the kernel.
 // (Rule 3, the 2:4 weights, is checked by commit.)  An engine with u8 activations (PE_PREC_FLAG_U8) runs every layer dense: the
-// sparse kernel is s8 x s8 only.
+// sparse kernel is s8 x s8 only.  So does PE_PREC_S8X2: the sparse kernel reads one plane.
 static bool sparse_eligible(const pe_engine* e, int i) {
     const ConvSpec& c = e->plan.convs[i];
-    return e->force_sparse && !e->u8 && conv_wfmt(e, i).s8() && conv_out_elem(e, i) == ELEM_S8 && !c.im2col_input;
+    const PlaneFmt wf = conv_wfmt(e, i);
+    return e->force_sparse && !e->u8 && wf.s8() && wf.planes == 1 && conv_out_elem(e, i) == ELEM_S8 && !c.im2col_input;
 }
 
 // Test hook, not part of the public header: with on != 0 the next pe_commit_weights of e picks the sparse kernel for every layer
@@ -1236,7 +1251,8 @@ static int run_net(pe_engine* e, int n) {
     if (!e->committed) return fail(e, PE_ERR_STATE, "pe_commit_weights has not been called");
     // at scale 1 almost every activation of a typical net quantises to 0
     if (e->prec->needs_calibration && !e->calibrated)
-        return fail(e, PE_ERR_STATE, "PE_PREC_S8X1 runs on calibrated range scales: call pe_calibrate (on the handle that owns the weights) before the first forward");
+        return fail(e, PE_ERR_STATE, "PE_PREC_%s runs on calibrated range scales: call pe_calibrate (on the handle that owns the weights) before the first forward",
+                    e->cfg.precision == PE_PREC_S8X2 ? "S8X2" : "S8X1");
     if (e->collecting) e->collect_forwards++;   // its maxima accumulate in d_range (folded by pe_range_status and pe_calibrate_end)
     if (!e->use_graphs) return run_net_eager(e, n);
     pe_engine::GraphEntry& g = e->graphs[n];
@@ -1679,7 +1695,7 @@ static bool owns_weights(const pe_engine* e) {
 // buffer no other handle uses (a sharer would keep the old scales).
 static int calib_owner_check(pe_engine* e, const char* what) {
     if (!e->committed) return fail(e, PE_ERR_STATE, "%s: pe_commit_weights has not been called", what);
-    if (!e->prec->ranged()) return fail(e, PE_ERR_INVALID, "%s: precision %d has no range scales (only 2, 4, 5 and 6 have)", what, e->cfg.precision);
+    if (!e->prec->ranged()) return fail(e, PE_ERR_INVALID, "%s: precision %d has no range scales (only 2, 4, 5, 6 and 8 have)", what, e->cfg.precision);
     if (!owns_weights(e))
         return fail(e, PE_ERR_STATE, "%s: this handle received its weights by broadcast / sharing: calibrate the source handle, which owns them", what);
     if (e->packed.use_count() > 1)
@@ -1828,7 +1844,8 @@ extern "C" int pe_calibrate_begin(pe_engine* e) {
     int rc = calib_owner_check(e, "pe_calibrate_begin"); if (rc) return rc;
     if (e->collecting) return fail(e, PE_ERR_STATE, "pe_calibrate_begin: a collection is already running");
     if (e->prec->needs_calibration && !e->calibrated)
-        return fail(e, PE_ERR_STATE, "pe_calibrate_begin: PE_PREC_S8X1 forwards only on calibrated scales: start with pe_calibrate or pe_calibration_set");
+        return fail(e, PE_ERR_STATE, "pe_calibrate_begin: PE_PREC_%s forwards only on calibrated scales: start with pe_calibrate or pe_calibration_set",
+                    e->cfg.precision == PE_PREC_S8X2 ? "S8X2" : "S8X1");
     CK(e, cudaSetDevice(e->cfg.device));
     CK(e, cudaStreamSynchronize(e->stream));
     CK(e, cudaMemset(e->d_range.get(), 0, e->plan.convs.size() * sizeof(unsigned)));   // maxima of earlier forwards do not count

@@ -2,8 +2,8 @@
 //
 // Pooling semantics: src/caffe/layers/pooling_layer.cpp:90-93 (ceil), :128-187 (max over the window clipped
 // to the image).  Activations are either fp32 [M][C], 16-bit "planes" whose SUM is the value (split
-// precision for the wgmma conv, see conv_tc.cu), or one e4m3 or s8 plane; the max is taken on the reconstructed
-// value and the winner's planes are copied, which keeps the split exact.
+// precision for the wgmma conv, see conv_tc.cu), one e4m3, s8 or u8 plane, or two s8 planes (256 hi + lo); the max is taken on
+// the reconstructed value and the winner's planes are copied, which keeps the split exact.
 #include "common.h"
 #include "kernels.h"
 
@@ -126,6 +126,47 @@ __global__ void __launch_bounds__(256) pool_bytes_kernel(PoolArgs a) {
     *((uint4*)((uint8_t*)a.out + mo * a.C) + g) = o;
 }
 
+// PE_PREC_S8X2: two s8 planes whose value is 256 hi + lo (s8.h), 16 channels per thread.  The max of the reconstructed values is
+// exact, and the winner's hi and lo bytes are copied, which is the re-split of that maximum.
+__global__ void __launch_bounds__(256) pool_s8x2_kernel(PoolArgs a) {
+    const unsigned cv = a.C / 16;
+    const int n = blockIdx.y;
+    const unsigned per_img = (unsigned)a.Hso * (unsigned)a.Wpo;
+    const unsigned idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= per_img * cv) return;
+    const int g = (int)(idx % cv);
+    const unsigned rem = idx / cv;
+    const int yo = (int)(rem / (unsigned)a.Wpo), xo = (int)(rem % (unsigned)a.Wpo);
+    if (xo >= a.Wo || yo >= a.Ho) return;
+    const long long mo = (long long)n * per_img + rem;
+    uint4 vh[4], vl[4];
+    bool ok[4];
+#pragma unroll
+    for (int w = 0; w < 4; w++) {
+        const int yi = 2 * yo + (w >> 1), xi = 2 * xo + (w & 1);
+        ok[w] = yi < a.Hi && xi < a.Wi;
+        const long long mi = ((long long)n * a.Hsi + (ok[w] ? yi : 2 * yo)) * a.Wpi + (ok[w] ? xi : 2 * xo);
+        vh[w] = __ldg((const uint4*)((const int8_t*)a.in + mi * a.C) + g);
+        vl[w] = __ldg((const uint4*)((const int8_t*)a.in + a.in_plane + mi * a.C) + g);
+    }
+    uint4 oh, ol;
+#pragma unroll
+    for (int j = 0; j < 16; j++) {
+        int8_t h = ((const int8_t*)&vh[0])[j], l = ((const int8_t*)&vl[0])[j];
+        int best = 256 * h + l;
+#pragma unroll
+        for (int w = 1; w < 4; w++) {
+            const int8_t hw = ((const int8_t*)&vh[w])[j], lw = ((const int8_t*)&vl[w])[j];
+            const int v = 256 * hw + lw;
+            if (ok[w] && v > best) { best = v; h = hw; l = lw; }
+        }
+        ((int8_t*)&oh)[j] = h;
+        ((int8_t*)&ol)[j] = l;
+    }
+    *((uint4*)((int8_t*)a.out + mo * a.C) + g) = oh;
+    *((uint4*)((int8_t*)a.out + a.out_plane + mo * a.C) + g) = ol;
+}
+
 int launch_pool(const PoolArgs& a, cudaStream_t st) {
     const long long rows_out = (long long)a.N * a.Hso * a.Wpo;
     const PlaneFmt f = a.fmt;
@@ -135,7 +176,8 @@ int launch_pool(const PoolArgs& a, cudaStream_t st) {
     } else if (f.e4m3() || f.s8() || f.u8()) {
         const unsigned per = (unsigned)a.Hso * a.Wpo * (a.C / 16);
         const dim3 grid((per + 255) / 256, a.N);
-        if (f.s8()) pool_bytes_kernel<ELEM_S8><<<grid, 256, 0, st>>>(a);
+        if (f.s8() && f.planes == 2) pool_s8x2_kernel<<<grid, 256, 0, st>>>(a);
+        else if (f.s8()) pool_bytes_kernel<ELEM_S8><<<grid, 256, 0, st>>>(a);
         else if (f.u8()) pool_bytes_kernel<ELEM_U8><<<grid, 256, 0, st>>>(a);
         else pool_bytes_kernel<ELEM_E4M3><<<grid, 256, 0, st>>>(a);
     } else {
@@ -183,6 +225,8 @@ __global__ void __launch_bounds__(256) act_to_nchw_kernel(const void* act, int p
     float v = 0.f;
     if (fmt.planes == 0) v = ((const float*)act)[m * pitch + coff + ch];
     else if (fmt.e4m3()) v = e4m3_to_float(((const uint8_t*)act)[m * pitch + coff + ch]);
+    else if (fmt.s8() && fmt.planes == 2)   // 256 hi + lo
+        v = (float)(256 * ((const int8_t*)act)[m * pitch + coff + ch] + ((const int8_t*)act)[plane + m * pitch + coff + ch]);
     else if (fmt.s8()) v = (float)((const int8_t*)act)[m * pitch + coff + ch];
     else if (fmt.u8()) v = (float)((const uint8_t*)act)[m * pitch + coff + ch];
     else for (int p = 0; p < fmt.planes; p++) {

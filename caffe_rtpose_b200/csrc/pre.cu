@@ -125,7 +125,8 @@ __host__ __device__ constexpr int mirror_k(int k) { return k < 27 ? (k / 9 * 3 +
 
 // S8X1: one s8 plane of 128 channels per pixel, the 27 patch values at scale 2^8 - p - 128 from the uint8 path (exact), and
 // sat(rint(x * 256)) from a planar fp32 input - in the first 32 bytes (channels 27..31 written as 0); the rest stays zero from
-// init.  SRC as in input_im2col_kernel.  One thread = one pixel.
+// init.  S8X2 runs the same kernel: these bytes are its hi plane, and its lo plane stays zero from init, so it stores the
+// 16-bit integers (p - 128) x 2^8.  SRC as in input_im2col_kernel.  One thread = one pixel.
 template <int SRC>
 __global__ void __launch_bounds__(256) input_im2col_s8_kernel(PreArgs a, const float* planar, int nimages) {
     const int n = blockIdx.y;

@@ -68,8 +68,22 @@ inline constexpr Precision PRECISIONS[] = {
     {{1, ELEM_S8}, ELEM_S8, 128, 128, 16, false, 6, 127.f, 4.f, "4", "the s8 planes", 256.f, true, 132104, true},                    // S8X1
 };
 constexpr int NUM_PRECISIONS = sizeof PRECISIONS / sizeof PRECISIONS[0];
-static_assert(NUM_PRECISIONS == PE_PREC_S8X1 + 1, "one row per PE_PREC_* mode");
-inline const Precision& precision(int pe_prec) { return PRECISIONS[pe_prec]; }   // pe_prec in [0, NUM_PRECISIONS)
+static_assert(NUM_PRECISIONS == PE_PREC_S8X1 + 1, "one row per PE_PREC_* mode up to S8X1");
+
+// PE_PREC_S8X2, the 16-bit integer mode: v in [-32768, 32639] stored as two s8 planes, hi = (v + 128) >> 8 and lo = v - 256 hi
+// (s8.h), hi*hi into one s32 accumulator and hi*lo + lo*hi into a second, both over the whole K (exact, so nothing is
+// chunked); lo*lo is dropped.  |acc_c| <= (128 x 128 + 128 x 127) x K stays inside s32 up to K = 65793.  The net input keeps
+// S8X1's im2col bytes in the hi plane with a zero lo plane, so it stores (p - 128) x 2^8 = (p/256 - 0.5) x 2^16.
+// Calibration target [2^13, 2^14): the 2-4x headroom of S8X1's [32, 64) below the largest stored value 32639.  Range floor
+// 2^8: below it the hi plane carries nothing and the layer runs on the lo plane's 8 bits.  Its own row after PRECISIONS,
+// which holds the modes up to S8X1; precision() answers for every mode.
+inline constexpr Precision S8X2_ROW =
+    {{2, ELEM_S8}, ELEM_S8, 128, 128, 16, false, 14, 32639.f, 256.f, "2^8", "the s8 plane pairs", 65536.f, true, 65793, true};
+static_assert((128LL * 128 + 128LL * 127) * 65793 <= 2147483647LL && (128LL * 128 + 128LL * 127) * 65794 > 2147483647LL,
+              "65793: the largest K of an S8X2 layer");
+// The PE_PREC_* values with a row: 0 .. PE_PREC_S8X1 and PE_PREC_S8X2 (8; 7 is not assigned, poseengine.h)
+constexpr bool known_mode(int pe_prec) { return (pe_prec >= 0 && pe_prec < NUM_PRECISIONS) || pe_prec == PE_PREC_S8X2; }
+inline const Precision& precision(int pe_prec) { return pe_prec == PE_PREC_S8X2 ? S8X2_ROW : PRECISIONS[pe_prec]; }   // known_mode(pe_prec)
 
 // The u8 activations of PE_PREC_S8X1 | PE_PREC_FLAG_U8 (plan.cpp: post-ReLU values read only by integer layers), outside
 // PRECISIONS since they are no mode of their own.  S8X1's layout and per-channel epilogue; u8 x s8 sums, |acc| <= 255 x 127 x K,

@@ -23,6 +23,7 @@ PREC_F16X2 = PREC_BF16X2   # the parity mode: 2 fp16 planes, chunked round-to-ne
 PREC_F16X1 = 4             # the fast mode: the parity mode's hi plane alone, one MMA per MAC (poseengine.h)
 PREC_E4M3X1 = 5            # the FP8 mode: one e4m3 plane, one FP8 MMA per MAC; needs calibrate() (poseengine.h)
 PREC_S8X1 = 6              # the INT8 mode: one s8 plane, one s8 MMA per MAC, exact s32 sums; forward needs calibrate() first
+PREC_S8X2 = 8              # the 16-bit integer mode: two s8 planes, three s8 MMAs per MAC, exact s32 sums; needs calibrate()
 PREC_FLAG_U8 = 0x100       # PREC_S8X1 only: post-ReLU activations stored as u8, their layers u8 x s8 (poseengine.h)
 MAX_PEOPLE = 96
 # pixel formats of forward_pixels / pixels_to_bgr (PE_PIX_*, poseengine.h)

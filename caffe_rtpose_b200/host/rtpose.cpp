@@ -95,7 +95,8 @@ static void define_flags() {
            "3 three bf16 planes (A/B only), 4 fast mode (one fp16 plane, 1 MMA per MAC; see --audit_every), "
            "5 FP8 mode (one e4m3 plane, 1 FP8 MMA per MAC; needs --calibrate_range, see --audit_every), "
            "6 INT8 mode (one s8 plane, 1 s8 MMA per MAC, exact integer sums, per-channel weight scales; requires --calibrate_range, "
-           "see --audit_every)");
+           "see --audit_every), 8 16-bit integer mode (two s8 planes, 3 s8 MMAs per MAC, exact integer sums, per-channel weight scales; "
+           "requires --calibrate_range, see --audit_every)");
     define("f16_layers", "", "[extension] with --precision 5 or 6: comma-separated conv layers that run in fp16 with --precision 4's arithmetic "
            "while the others keep the FP8 / INT8 format; 'narrow' = the layers that read fewer than 128 channels (conv1_1, conv1_2, conv2_1). "
            "Layers that read one buffer go together (pe_create_mixed); empty = none");
@@ -108,13 +109,13 @@ static void define_flags() {
            "--batch is automatic: the copies and the kernel tails of one batch overlap the other; weights are shared, not duplicated)");
     define("flip_test", "false", "[extension] average every frame's maps with those of its net input mirrored in x, left/right parts and "
            "limbs swapped (pe_set_flip_test): the conv stack runs twice the images, for every source and --precision", true);
-    define("calibrate_range", "true", "[extension] fp16, e4m3 and s8 modes (--precision 2, 4, 5 and 6): derive per-layer power-of-two activation scales from one synthetic frame at start-up "
-           "(pe_calibrate), so that a model of any magnitude keeps fp32-level results; --precision 6 cannot run without them", true);
-    define("calibration_dir", "", "[extension] --precision 2, 4, 5 or 6: after the synthetic-frame calibration of --calibrate_range, calibrate GPU 0's "
+    define("calibrate_range", "true", "[extension] fp16, e4m3 and s8 modes (--precision 2, 4, 5, 6 and 8): derive per-layer power-of-two activation scales from one synthetic frame at start-up "
+           "(pe_calibrate), so that a model of any magnitude keeps fp32-level results; --precision 6 and 8 cannot run without them", true);
+    define("calibration_dir", "", "[extension] --precision 2, 4, 5, 6 or 8: after the synthetic-frame calibration of --calibrate_range, calibrate GPU 0's "
            "engine on the images of this directory (.jpg / .png / .bmp / .ppm of any size, sorted, at most --calibration_frames): passes of "
            "one forward of every batch each (pe_calibrate_begin / pe_calibrate_end) until a pass changes no layer's scale");
     define("calibration_frames", "64", "[extension] --calibration_dir: the largest number of images it reads");
-    define("calibration_table", "", "[extension] --precision 2, 4, 5 or 6: apply this calibration table (--save_calibration, pe_calibration_set) "
+    define("calibration_table", "", "[extension] --precision 2, 4, 5, 6 or 8: apply this calibration table (--save_calibration, pe_calibration_set) "
            "to GPU 0's engine instead of calibrating; a table of other weights, another precision or other --f16_layers ends start-up");
     define("save_calibration", "", "[extension] write GPU 0's calibration table (pe_calibration_get) to this file once calibration is done");
     define("audit_every", "0", "[extension] N > 0: every worker also holds a parity-mode (--precision 2) handle and forwards every N-th batch "
@@ -722,7 +723,7 @@ static std::vector<CalibImage> g_calib_images;
 
 static bool ranged_precision(int p) {
     p &= ~PE_PREC_FLAG_U8;
-    return p == PE_PREC_F16X2 || p == PE_PREC_F16X1 || p == PE_PREC_E4M3X1 || p == PE_PREC_S8X1; }
+    return p == PE_PREC_F16X2 || p == PE_PREC_F16X1 || p == PE_PREC_E4M3X1 || p == PE_PREC_S8X1 || p == PE_PREC_S8X2; }
 
 static std::string calibration_table_of(pe_engine* e) {
     const int n = pe_calibration_get(e, nullptr, 0);
@@ -1250,8 +1251,13 @@ int main(int argc, char** argv) {
         LOG_ERROR("--precision 6 (INT8) runs on calibrated per-layer range scales: at scale 1 almost every activation quantises to 0; drop --nocalibrate_range");
         return 1;
     }
+    if (Fi("precision") == PE_PREC_S8X2 && !Fb("calibrate_range")) {
+        LOG_ERROR("--precision 8 (16-bit integers) runs on calibrated per-layer range scales: at scale 1 most activations keep only a few "
+                  "of their 16 bits; drop --nocalibrate_range");
+        return 1;
+    }
     if ((!F("calibration_dir").empty() || !F("calibration_table").empty() || !F("save_calibration").empty()) && !ranged_precision(Fi("precision"))) {
-        LOG_ERROR("--calibration_dir, --calibration_table and --save_calibration are for the modes with range scales: --precision 2, 4, 5 or 6");
+        LOG_ERROR("--calibration_dir, --calibration_table and --save_calibration are for the modes with range scales: --precision 2, 4, 5 or 6, and 8");
         return 1;
     }
     if (!F("calibration_table").empty() && !F("calibration_dir").empty()) {

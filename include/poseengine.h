@@ -79,6 +79,24 @@ extern "C" {
                              * (PE_ERR_INVALID, the layer named).  No layer runs the 2:4-sparse kernel.  Calibration tables record
                              * the precision with the flag (262): an S8X1 table and a u8 table refuse each other.  pe_share_weights
                              * and pe_broadcast_weights need the flag on both sides.  DESIGN.md section 6. */
+#define PE_PREC_S8X2 8      /* wgmma 16-bit INTEGER mode: activations and weights are 16-bit integers v held in two s8 planes,
+                             * hi = (v + 128) >> 8 and lo = v - 256 hi, both in [-128, 127]; 3 s8 MMAs per MAC (wgmma k32 s8 -> s32):
+                             * hi*hi into one s32 accumulator, hi*lo + lo*hi into a second, both exact over the whole K (lo*lo is
+                             * dropped, as in the parity mode).  Activations are v = sat(rint(x * 2^k)) in [-32768, 32639] with a
+                             * power-of-two scale 2^k per conv output; zero padding is the integer 0.  Weights are quantised per
+                             * output channel after the range ratios are folded in: sigma_c = max|w| / 32639, q = clamp(rint(w /
+                             * sigma_c), -32639, 32639), split as above.  Epilogue per channel, in fp32 without FMA: S = 256 acc_h +
+                             * acc_c (exact, 64-bit; it counts in units of 2^8, the place of the dropped lo*lo), t = float(S) *
+                             * f_c + b'_c with f_c = 2^8 sigma_c * 2^(k_out - k_in) and b'_c as in PE_PREC_S8X1, ReLU, then
+                             * v = sat(rint(t)), split and stored (the fp32 maps: k_out = 0, t stored).  The net input is S8X1's
+                             * p - 128 in the hi plane with a zero lo plane, i.e. at k = 16.  A layer whose K = k*k*Cin (padded)
+                             * exceeds 65793 could overflow s32 and is refused (PE_ERR_INVALID, the layer named).  Needs pe_calibrate
+                             * (it puts each layer's largest stored value in [2^13, 2^14)): a forward before it is PE_ERR_STATE.
+                             * pe_range_status reports the largest stored value / 32639 and PE_ERR_RANGE when a layer reaches 32639
+                             * or stays below 2^8 (the hi plane then carries nothing).  PE_PREC_FLAG_U8 and pe_create_mixed refuse
+                             * this mode, and no layer runs the 2:4-sparse kernel (pe_conv_layer_sparse returns 0).  Calibration
+                             * tables record precision 8.  Precision 7 is not assigned: it stays PE_ERR_INVALID ("unknown
+                             * precision"), as it was before this mode existed.  DESIGN.md sections 3, 4, 6 and 9. */
 
 #define PE_MAX_PEOPLE 96   /* RENDER_MAX_PEOPLE, renderFunctions.h:6 / rtpose.cpp:88 */
 

@@ -1,10 +1,10 @@
 #!/usr/bin/env python3
-"""Speed and accuracy of the fast modes (PE_PREC_F16X1, PE_PREC_E4M3X1, PE_PREC_S8X1) against the parity mode (F16X2) and bf16x1, in one run
+"""Speed and accuracy of the fast modes (PE_PREC_F16X1, PE_PREC_E4M3X1, PE_PREC_S8X1, PE_PREC_S8X2) against the parity mode (F16X2) and bf16x1, in one run
 on one GPU.
 
 Workload C2 of bench.py: COCO 656x368, one scale, 9 frames per forward, the bench's seeded 720p frames (synth.make_frame(i)),
-W-he weights (E4M3X1 and S8X1 calibrated with pe_calibrate on frame 0: e4m3 has no room for an uncalibrated net, and s8
-refuses to run one).  Per mode, alternating the modes over FM_ROUNDS rounds:
+W-he weights (E4M3X1, S8X1 and S8X2 calibrated with pe_calibrate on frame 0: e4m3 has no room for an uncalibrated net, and the
+integer modes refuse to run one).  Per mode, alternating the modes over FM_ROUNDS rounds:
   * resident: frames/s of FM_STEPS forwards from device memory over two handles (CUDA events, as bench.py);
   * e2e: frames/s through forward_frames + fetch of every frame (host clock, as bench.py);
   * conv ms per layer class of one 9-frame step (pe_profile_layers, classes of tools/layer_times.py, median of 5).
@@ -14,7 +14,7 @@ the prototxt-filler net (gaussian(0.01) weights, maps ~3e-11), calibrated with p
 maps are noise with thousands of near-tie NMS decisions, so these pose statistics are a worst case, not what a trained
 model shows.  FM_MODES also takes mixed-precision entries "<base>+<fp16 layers>" (pe_create_mixed), e.g. e4m3x1+narrow or
 s8x1+conv1_1+conv1_2: calibrated like their base and reported like the other modes.  s8x1u8 is PE_PREC_S8X1 with u8 activations
-(PE_PREC_FLAG_U8), calibrated like s8x1.  Prints the card, its power limit and SM clocks, then one JSON line."""
+(PE_PREC_FLAG_U8), calibrated like s8x1.  s8x2 is the 16-bit integer mode PE_PREC_S8X2.  Prints the card, its power limit and SM clocks, then one JSON line."""
 import json
 import os
 import statistics
@@ -33,8 +33,8 @@ from layer_times import klass  # noqa: E402
 
 MODEL, NET_W, NET_H, DISP_W, DISP_H, B = engine.COCO_18, 656, 368, 1280, 720, 9
 MODES = {"f16x2": engine.PREC_F16X2, "f16x1": engine.PREC_F16X1, "e4m3x1": engine.PREC_E4M3X1, "s8x1": engine.PREC_S8X1,
-         "bf16x1": engine.PREC_BF16X1, "s8x1u8": engine.PREC_S8X1 | engine.PREC_FLAG_U8}
-CALIBRATED = ("e4m3x1", "s8x1", "s8x1u8")
+         "bf16x1": engine.PREC_BF16X1, "s8x1u8": engine.PREC_S8X1 | engine.PREC_FLAG_U8, "s8x2": engine.PREC_S8X2}
+CALIBRATED = ("e4m3x1", "s8x1", "s8x1u8", "s8x2")
 
 
 def mode_spec(m):
